@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — GC-ADPCM batch encode throughput on B200 (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py — GC-ADPCM batch encode throughput on H100 (BASELINE.json metric), one JSON line on rank 0.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--channels C] [--seconds S]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--channels C] [--seconds S] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path (coefficient analysis + exhaustive encode, GcAdpcmFormat.EncodeFromPcm16's loop)
 over one synthetic batch.  Default workload = BASELINE.json configs[1]: 1024 channels x 30 s x 48 kHz PCM16 per GPU
@@ -11,10 +11,12 @@ over one synthetic batch.  Default workload = BASELINE.json configs[1]: 1024 cha
   e2e        the same batch through the host C-ABI call (vgb_gcadpcm_encode_batch) with PINNED HOST buffers:
              H2D of the PCM, kernels, D2H of coefficients + ADPCM all inside the timed region.
   roofline   the dominant kernel (gc_encode_kernel): algorithmic bytes (2 B read + 8/14 B written per sample) over its
-             measured launch time, against the measured HBM copy bandwidth in MEASURED_PEAKS.json.
+             measured launch time, against the measured HBM copy bandwidth in MEASURED_PEAKS.json (else the H100 SXM
+             data-sheet figure, named as such).
   cpu_baseline  the CPU oracle port of the reference (oracle/, C, one task per channel on all host cores) on a bounded
              sample of the same batch.
 --impl reference times that CPU port alone (the reference itself is C#/.NET and cannot run in this image).
+--dump-outputs DIR writes what the last timed step computed (see dump_outputs) as DIR/<name>.npy.
 """
 from __future__ import annotations
 
@@ -57,7 +59,12 @@ def parse_args():
     ap.add_argument("--out-format", default="dsp", choices=["dsp", "adx", "hca"], help="batch: container to write")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="c2: write the last timed step's coefficients and a seeded sample of its ADPCM rows as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.config != "c2"):
+        ap.error("--dump-outputs is implemented for --impl ours --config c2")
+    return args
 
 
 def env_rank():
@@ -106,7 +113,7 @@ def make_batch_gpu(torch, n_channels: int, n: int, rank: int, device, degenerate
 
 
 # ------------------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler
 # ------------------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -155,6 +162,33 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_identity(gpu_index: int, torch) -> dict:
+    """The card a number was measured on and its power limit (part of every absolute number)."""
+    out = {"name": torch.cuda.get_device_name(gpu_index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                           capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
+
+
+DUMP_BYTES = 48 << 20  # budget of the sampled ADPCM rows (float32); the whole dump stays under 64 MB
+
+
+def dump_outputs(out_dir: str, coefs_dev, adpcm_dev, n_bytes: int) -> None:
+    """What a caller of vgb_gcadpcm_encode_dev receives, from the last timed step: the coefficient table of every channel
+    and the ADPCM bytes of a fixed, seeded sample of whole channel rows (all rows when they fit the budget)."""
+    n_ch = coefs_dev.shape[0]
+    rows = min(n_ch, max(1, DUMP_BYTES // (4 * max(n_bytes, 1))))
+    pick = np.sort(np.random.default_rng(0x5647).choice(n_ch, rows, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "coefs.npy"), coefs_dev.cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "adpcm_rows.npy"), pick.astype(np.float64))
+    np.save(os.path.join(out_dir, "adpcm.npy"), adpcm_dev[pick, :n_bytes].cpu().numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -324,6 +358,8 @@ def main():
         dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
         elapsed_ms = float(tmax.item())
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, coefs_dev, adpcm_dev, n_bytes)
     kernel_ms /= args.steps
     ms_per_step = elapsed_ms / args.steps
     value = world * samples_per_step / (ms_per_step / 1e3) / 1e6
@@ -345,7 +381,7 @@ def main():
             N.check(vg.lib.vgb_gcadpcm_encode_batch(in_tab, lens.ctypes.data, None, None, n_ch, coefs_host.ctypes.data,
                                                     out_tab, None, None))
 
-        e2e_steps = max(1, min(args.steps, 3))
+        e2e_steps = args.steps
         step_e2e()  # warm-up (allocates the library's own device buffers)
         barrier()
         t0 = time.perf_counter()
@@ -386,17 +422,12 @@ def main():
                   "adpcm_bytes_equal": bool((g_adpcm == o_adpcm).all())}
 
     if rank == 0:
+        gpu = gpu_identity(local_rank, torch)
         peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
         if os.path.exists(peaks_path):
             peak = float(json.load(open(peaks_path))["hbm_gbs"]); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         else:
-            peak = 6650.0; peak_src = "fallback (B200_PROFILING.md 6.65 TB/s)"
-        traffic = None
-        prof = os.path.join(ROOT, "profiles", "r02_gc_encode_kernel_0.json")  # the chain launch of the time-parallel encode
-        if not os.path.exists(prof):
-            prof = os.path.join(ROOT, "profiles", "r01_gc_encode_full.json")
-        if os.path.exists(prof) and n_ch == 1024 and n == 1440000:
-            traffic = json.load(open(prof)).get("dram_bytes_total")  # ncu --set full, same launch shape
+            peak = 3350.0; peak_src = "H100 SXM data sheet (3.35 TB/s), not measured"
         enc_ms = float(kernel_ms[2])
         achieved = samples_per_step * ALG_BYTES_PER_SAMPLE / (enc_ms / 1e3) / 1e9 if enc_ms > 0 else None
         line = {
@@ -407,13 +438,13 @@ def main():
                        "l2": "inputs (2.9 GB/GPU) larger than L2, no flush needed", "parallelism": f"dp{world} (channels sharded)"},
             "e2e": e2e,
             "gpu_launches": int(launches),
+            "gpu": gpu,
             "clocks": clocks,
             "roofline": {"bound": "hbm", "kernel": "gc_encode_kernel", "achieved": round(achieved, 2) if achieved else None,
                          "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 5) if achieved else None,
-                         "traffic": traffic, "traffic_source": f"{os.path.relpath(prof, ROOT)} (ncu dram__bytes_read+write, per launch)" if traffic else None,
                          "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": int(samples_per_step * ALG_BYTES_PER_SAMPLE),
-                         "note": "instruction-issue bound (exhaustive 8-predictor x scale search, 253 warp instructions per channel-frame, issue active 72 %), not HBM (DESIGN.md 5.3); traffic = the chain launch, 1.11 x algorithmic (trace words)"},
+                         "note": "instruction-issue bound (exhaustive 8-predictor x scale search), not HBM (DESIGN.md 5.3)"},
             "kernel_ms": {"gc_coef_frames": round(float(kernel_ms[0]), 3), "gc_coef_refine": round(float(kernel_ms[1]), 3),
                           "gc_encode": round(float(kernel_ms[2]), 3)},
             "time_parallel": splice,

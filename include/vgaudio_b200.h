@@ -1,9 +1,9 @@
 /*
- * vgaudio_b200.h — C ABI of libvgaudio_b200.so: the B200 (sm_100a) batch codec engine that replaces the
+ * vgaudio_b200.h — C ABI of libvgaudio_b200.so: the H100 (sm_90a) batch codec engine that replaces the
  * per-channel CPU hot path of Thealexbarney/VGAudio.
  *
  * This header is the drop-in boundary.  Every entry point names the reference interface it replaces
- * (paths relative to /root/reference/src/VGAudio/).  The reference-side binding (C# P/Invoke) a maintainer
+ * (paths relative to VGAudio's src/VGAudio/).  The reference-side binding (C# P/Invoke) a maintainer
  * would add is shown in INTEGRATION.md and bindings/csharp/.
  *
  * Conventions

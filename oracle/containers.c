@@ -4,7 +4,7 @@
  *
  * Pins the reference holds for this layer: build -> parse round trips only (src/VGAudio.Tests/Containers/DspTests.cs:9-19,
  * WaveTests.cs:9-55 through BuildParseTests.cs:9-16); no golden file bytes, no encryption test => header bytes and
- * key schedules are "parity unpinned" like the codecs' payloads.  Citations are relative to /root/reference/src/VGAudio/.
+ * key schedules are "parity unpinned" like the codecs' payloads.  Citations are relative to VGAudio's src/VGAudio/.
  */
 #include <stdlib.h>
 #include <string.h>

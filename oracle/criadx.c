@@ -1,7 +1,7 @@
 /*
  * oracle/criadx.c — CPU ORACLE (test infrastructure, not product) for the CRI ADX 4-bit ADPCM codec.
  *
- * Restates Codecs/CriAdx/CriAdxCodec.cs (paths relative to /root/reference/src/VGAudio/) in plain C.
+ * Restates Codecs/CriAdx/CriAdxCodec.cs (paths relative to VGAudio's src/VGAudio/) in plain C.
  * PARITY UNPINNED: the reference has no test of any kind for this codec (SURVEY.md §4/§8c: no file under
  * src/VGAudio.Tests mentions Adx) and cannot be executed here (no .NET), so this restatement is argued line by line
  * and checked only through self-consistency properties (encode->decode tracking, encoder reconstruction == decoder).

@@ -3,7 +3,7 @@
  *
  * Restates, in plain C with IEEE-754 double / wrapping int32 semantics, what the reference does in
  *   Codecs/GcAdpcm/GcAdpcmCoefficients.cs, GcAdpcmEncoder.cs, GcAdpcmDecoder.cs, GcAdpcmMath.cs and
- *   Utilities/Helpers.cs:32-58 (paths relative to /root/reference/src/VGAudio/).
+ *   Utilities/Helpers.cs:32-58 (paths relative to VGAudio's src/VGAudio/).
  * Must be compiled with -ffp-contract=off and without -ffast-math: RyuJIT emits separate SSE2
  * mul/add, and the silent-channel case relies on NaN comparison semantics (SURVEY.md Appendix A.4, A.19).
  *

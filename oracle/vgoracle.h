@@ -22,7 +22,7 @@
  *   - seek table / loop context .... pinned by the KATs of GcAdpcmLoopContextTests.cs / GcAdpcmSeekTableTests.cs
  *   - containers (containers.c) .... build -> parse round trips only (WaveTests.cs, DspTests.cs): file bytes unpinned
  *
- * All file:line citations are relative to /root/reference/src/VGAudio/.
+ * All file:line citations are relative to VGAudio's src/VGAudio/.
  * Build: see oracle/Makefile (gcc -O2 -ffp-contract=off -fno-fast-math).
  */
 #ifndef VGORACLE_H

@@ -2,7 +2,7 @@
 
 The reference has no golden bitstream for this codec (SURVEY.md §4/§8c), so the pins are its KAT tables for the
 nibble/sample math and its round-trip properties.  Sources are cited per test (paths under
-/root/reference/src/VGAudio.Tests/).
+VGAudio's src/VGAudio.Tests/).
 """
 import json
 import os

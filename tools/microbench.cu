@@ -1,5 +1,5 @@
-// tools/microbench.cu — dependent-chain latencies on sm_100a for the ops the codec kernels' critical paths use.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 --fmad=false -o tools/microbench tools/microbench.cu
+// tools/microbench.cu — dependent-chain latencies on sm_90a (H100) for the ops the codec kernels' critical paths use.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 --fmad=false -o tools/microbench tools/microbench.cu
 // One warp, one CTA; cycles per op = (clock after - clock before) / chain length.
 #include <cstdio>
 #include <cstdint>

@@ -11,7 +11,7 @@ Per entry:
   roofline         algorithmic bytes / kernel_ms against MEASURED_PEAKS.json's HBM copy bandwidth
   cpu_baseline     the oracle port on all host cores (one channel / stream per task), bounded sample
   parity           outputs of a sample of units compared with the oracle, bit-exact
-Usage: python tools/secondary_bench.py [--scale 1.0] > profiles/r02_secondary_bench.json
+Usage: python tools/secondary_bench.py [--scale 1.0] > secondary_bench.json
 """
 import argparse
 import ctypes as C
@@ -40,7 +40,7 @@ def peak_gbs():
     try:
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 def measure(call, slot, reps=3):

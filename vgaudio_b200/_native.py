@@ -217,7 +217,7 @@ def _load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  vgaudio_b200 has no CPU fallback."
+            "(nvcc, sm_90a).  vgaudio_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():

@@ -1,6 +1,6 @@
 """Host-side mirror of VGAudio.Codecs.CriAdx over the C ABI (no arithmetic here).
 
-Reference interface (paths under /root/reference/src/VGAudio/):
+Reference interface (paths under VGAudio's src/VGAudio/):
   CriAdxCodec.Encode(short[] pcm, CriAdxParameters config) -> byte[]     Codecs/CriAdx/CriAdxCodec.cs:56  (mutates config.History)
   CriAdxCodec.Decode(byte[] adpcm, int sampleCount, CriAdxParameters)    Codecs/CriAdx/CriAdxCodec.cs:9
   CriAdxParameters                                                         Codecs/CriAdx/CriAdxParameters.cs:3-13

@@ -1,6 +1,6 @@
 """Host-side mirror of VGAudio.Codecs.CriHca's encoder entry over the C ABI (no arithmetic here).
 
-Reference interface (paths under /root/reference/src/VGAudio/):
+Reference interface (paths under VGAudio's src/VGAudio/):
   CriHcaParameters / CriHcaQuality                    Codecs/CriHca/CriHcaParameters.cs:3-15, CriHcaQuality.cs:3-10
   CriHcaEncoder.InitializeNew(config) -> .Hca (HcaInfo)  Codecs/CriHca/CriHcaEncoder.cs:49-114
   CriHcaFormat.EncodeFromPcm16(pcm16, config)          Formats/CriHca/CriHcaFormat.cs:34-84  (-> byte[FrameCount][FrameSize])

@@ -1,4 +1,4 @@
-// adx.cu — CRI ADX 4-bit ADPCM encode / decode on sm_100a.
+// adx.cu — CRI ADX 4-bit ADPCM encode / decode on sm_90a (H100).
 //
 // Replaces CriAdxCodec.Encode / EncodeFrame / Decode (Codecs/CriAdx/CriAdxCodec.cs:9-171).  Like GC-ADPCM the codec
 // is a serial recurrence per channel (the next frame starts from the reconstructed last two samples, :98-99,:137),
@@ -516,9 +516,19 @@ int adx_encode_pick_segments(int n_channels, int max_whole_frames, int *min_seg_
         const int v = std::atoi(env);
         if (v >= 1) return v > kAdxMaxSegments ? kAdxMaxSegments : v;
     }
-    const long long want = (4ll * 148 * 512 + n_channels - 1) / std::max(n_channels, 1);  // about four waves of threads
+    static int sms = 0;
+    if (sms == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) {
+            (void)cudaGetLastError();
+            sms = 132;  // H100 SXM
+        }
+    }
+    const long long want = (4ll * sms * 512 + n_channels - 1) / std::max(n_channels, 1);  // about four waves of threads
     // a batch that cannot fill the machine with kAdxMinSegFrames-long segments is latency bound: quarter the minimum (the
-    // fixed predictor's run-on is some hundred frames; batch converter, 2048 files of 1-6 s: 38.6 -> 23.0 ms end to end)
+    // fixed predictor's run-on is some hundred frames, so short segments stay cheap; the batch converter's files of 1-6 s
+    // are this case)
     if (!std::getenv("VGB_ADX_MIN_SEG_FRAMES") && max_whole_frames / min_seg < want) min_seg = std::max(64, min_seg / 4);
     if (min_seg_out) *min_seg_out = min_seg;
     const int max_s = std::max(1, std::min(kAdxMaxSegments, max_whole_frames / min_seg));

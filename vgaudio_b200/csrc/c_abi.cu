@@ -407,10 +407,9 @@ bool uniform_stride(T *const *ptr, int32_t n, int64_t &stride_bytes)
 }
 
 
-// Pageable caller buffers (a C# short[] pinned by the GC is still pageable for CUDA) move at ~11 GB/s through the
-// driver's staging buffers; page-locking the region for the duration of the call costs ~20 ms/GiB and lets the copy
-// engine read it directly at PCIe speed (measured: 96 ms/GiB pageable vs 21 + 19 ms/GiB registered,
-// tools/host_register_probe.py).  Inputs only: they are touched memory; registering a freshly allocated output would
+// Pageable caller buffers (a C# short[] pinned by the GC is still pageable for CUDA) move through the driver's staging
+// buffers at a fraction of PCIe speed; page-locking the region for the duration of the call costs some ms per GiB and
+// lets the copy engine read it directly at PCIe speed (tools/host_register_probe.py compares the two).  Inputs only: they are touched memory; registering a freshly allocated output would
 // fault its pages in first and cost more than it saves.  Registrations live until the API call returns (PinScope).
 thread_local std::vector<void *> t_pins;
 

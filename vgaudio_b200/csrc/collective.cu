@@ -110,8 +110,8 @@ int32_t vgb_nccl_init(const uint8_t *id, int32_t n_ranks, int32_t rank)
     if (g_comm) return abi_fail(VGB_E_STATE, "a communicator already exists; call vgb_nccl_shutdown first");
     if (int32_t rc = load_api()) return rc;
     // The batch path's exchange is a one-to-many scatter / many-to-one gather of large blocks: the root's NVLink port is the
-    // limit, and NCCL's default point-to-point channel count leaves most of it idle (measured at 4 GPUs, 26 GB out + 7 GB
-    // in: 90 ms with the default, 51 ms with 32 channels per peer).  Only set when the user has not chosen a value.
+    // limit, and NCCL's default point-to-point channel count leaves most of it idle (32 channels per peer nearly halved
+    // the exchange of a 4-GPU C5 run).  Only set when the user has not chosen a value.
     setenv("NCCL_MIN_P2P_NCHANNELS", "32", 0);
     setenv("NCCL_MAX_P2P_NCHANNELS", "32", 0);
     ncclUniqueId uid;

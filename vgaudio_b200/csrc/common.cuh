@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for the sm_100a codec kernels.
+// common.cuh — shared device helpers for the sm_90a codec kernels.
 //
 // Numeric contract (SURVEY.md Appendix A): the reference is C# compiled by RyuJIT for x64, i.e. IEEE-754
 // binary64/binary32 with NO fused multiply-add, wrapping (unchecked) int32 arithmetic, truncating integer

@@ -11,7 +11,7 @@
 //                                                      src/VGAudio.Cli/Batch.cs:11-51 + Convert.cs:18-36
 // All of it is HBM-bound byte work (every payload byte read once, written once); headers are a few dozen bytes per file
 // and are built on the host, except the fields that only exist on the device (DSP: coefficients, first predictor/scale
-// byte, loop context), which the assemble kernel patches in.  Citations are relative to /root/reference/src/VGAudio/.
+// byte, loop context), which the assemble kernel patches in.  Citations are relative to VGAudio's src/VGAudio/.
 #include <cuda_runtime.h>
 
 #include <algorithm>

@@ -1,4 +1,4 @@
-// gc_coefs.cu — GC-ADPCM coefficient analysis on sm_100a.
+// gc_coefs.cu — GC-ADPCM coefficient analysis on sm_90a (H100).
 //
 // Replaces GcAdpcmCoefficients.CalculateCoefficients (Codecs/GcAdpcm/GcAdpcmCoefficients.cs:9-110) for a whole
 // batch of channels.  The reference is one serial fp64 loop per channel; here it is split where the data
@@ -242,8 +242,9 @@ __device__ __forceinline__ int16_t gc_quantise_coef(double v)
 //              from a ballot: record order is preserved inside a bucket);
 //   warp 0     (consumer) meanwhile walks the PREVIOUS chunk's blocks in order and lane (bucket, component) adds ONLY
 //              its bucket's records, in record order - exactly the reference's sequence of additions.
-// W warps per CTA = 1 consumer + (W - 1) producers.  W = 4 keeps seven CTAs per SM, which holds all 1024 channels of the
-// headline batch at once; W = 8 (7 producers, 61 KB of queues) is kept for experiments with small batches
+// W warps per CTA = 1 consumer + (W - 1) producers.  W = 4 keeps eight CTAs per SM (64 registers, 8 x 26 KB of shared
+// memory), which holds all 1024 channels of the headline batch at once on H100's 132 SMs (seven would leave 100 channels
+// for a second wave); W = 8 (7 producers, 61 KB of queues) is kept for experiments with small batches
 // (VGB_REFINE_WIDE_LIMIT).
 
 struct __align__(16) RefineSlot {
@@ -409,7 +410,7 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
 }
 
 template <int W>
-__global__ void __launch_bounds__(W * 32, W == 4 ? 7 : 3)  // W = 4: 7 CTAs per SM, 1024 channels are resident at once
+__global__ void __launch_bounds__(W * 32, W == 4 ? 8 : 3)  // W = 4: 8 CTAs per SM, 1024 channels are resident at once on 132 SMs
 gc_coef_refine_kernel(GcChannelTable tab, const double2 *__restrict__ records, const uint32_t *__restrict__ accept_mask,
                       int16_t *__restrict__ coefs_out)
 {

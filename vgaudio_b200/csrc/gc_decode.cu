@@ -1,4 +1,4 @@
-// gc_decode.cu — GC-ADPCM decoder on sm_100a.
+// gc_decode.cu — GC-ADPCM decoder on sm_90a (H100).
 //
 // Replaces GcAdpcmDecoder.Decode (Codecs/GcAdpcm/GcAdpcmDecoder.cs:10-54).  The recurrence
 //     s[t] = Clamp16((c1*s[t-1] + c2*s[t-2] + scale*nibble + 1024) >> 11)

@@ -1,4 +1,4 @@
-// gc_encode.cu — GC-ADPCM encoder on sm_100a.
+// gc_encode.cu — GC-ADPCM encoder on sm_90a (H100).
 //
 // Replaces GcAdpcmEncoder.Encode / DspEncodeFrame / DspEncodeCoef (Codecs/GcAdpcm/GcAdpcmEncoder.cs:14-171).
 //
@@ -758,11 +758,10 @@ int gc_encode_min_segment_frames()
 }
 
 // How many segments to cut the frame range into.  The chain launch is throughput bound once every SM sub-partition
-// holds its four warps (measured on C2: ~800 cycles per frame pair and sub-partition from 4 warps up, against the
-// 1419-cycle dependent chain of a lone warp), so the aim is (a) several full waves of (channel pair, segment) items -
-// the last, partly filled wave is the only loss - and (b) segments longer than the run-on tail (above).  Measured on C2
-// (512 item rows): 75.5 ms with one segment, 48 ms with 3, 39.0 with 17, 38.7 with 24, 38.8 with 34, 45 with 48
-// (profiles/r02_seg_sweep.md; the last two already lose boundaries to the cascade).
+// holds its four warps (a lone warp per sub-partition waits on its own dependent chain), so the aim is (a) several full
+// waves of (channel pair, segment) items on this device's SM count - the last, partly filled wave is the only loss - and
+// (b) segments longer than the run-on tail (above); too many segments lose boundaries to the cascade
+// (tools/seg_sweep.py sweeps the count).
 int gc_encode_pick_segments(int n_channels, int max_frames, int *min_seg_out)
 {
     int min_seg = gc_encode_min_segment_frames();
@@ -773,7 +772,7 @@ int gc_encode_pick_segments(int n_channels, int max_frames, int *min_seg_out)
     }
     static int slots = 0;
     if (slots == 0) {
-        int dev = 0, sms = 148, per_sm = kEncChainBlocksPerSm;
+        int dev = 0, sms = 132, per_sm = kEncChainBlocksPerSm;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gc_encode_kernel<kGcChain>, kEncWarps * 32, 0) != cudaSuccess || per_sm < 1) {
@@ -786,9 +785,9 @@ int gc_encode_pick_segments(int n_channels, int max_frames, int *min_seg_out)
     const int want = (int)((5ll * slots + rows - 1) / rows);  // about five waves of items
     // A batch of SHORT channels too small to fill the machine with kGcMinSegFrames-long segments is latency bound (a
     // segment's serial chain): halve the minimum when a channel yields fewer than eight segments.  More boundaries then end
-    // in the cascade, but a few serial repairs cost less than chains twice as long (batch converter, 2048 files of 1-6 s:
-    // encode stage 56 -> 44 ms).  Long channels keep the full minimum: with 2048-frame segments the 128-channel groups of the
-    // pipelined host call lost more to the cascade's serial repairs than they gained (C2 end to end 75 -> 80 ms).
+    // in the cascade, but a few serial repairs cost less than chains twice as long (the batch converter's files of 1-6 s).
+    // Long channels keep the full minimum: with 2048-frame segments the 128-channel groups of the pipelined host call lose
+    // more to the cascade's serial repairs than they gain.
     if (!std::getenv("VGB_GC_MIN_SEG_FRAMES") && max_frames / min_seg < std::min(want, 8)) min_seg = std::max(kEncChunkFrames, min_seg / 2);
     if (min_seg_out) *min_seg_out = min_seg;
     const int max_s = std::min(kGcMaxSegments, std::max(1, max_frames / min_seg));

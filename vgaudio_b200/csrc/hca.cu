@@ -1,4 +1,4 @@
-// hca.cu — CRI HCA encoder on sm_100a.
+// hca.cu — CRI HCA encoder on sm_90a (H100).
 //
 // Replaces CriHcaEncoder.EncodeFrame and its 12 stages (Codecs/CriHca/CriHcaEncoder.cs:271-286, :420-858),
 // CriHcaPacking.PackFrame (CriHcaPacking.cs:17-58, BitWriter.cs:26-98, Crc16.cs) and Mdct.RunMdct/Dct4

@@ -1,4 +1,4 @@
-// interleave.cu — block (de)interleave of channel payloads on sm_100a.
+// interleave.cu — block (de)interleave of channel payloads on sm_90a (H100).
 //
 // Replaces InterleaveExtensions.Interleave / DeInterleave (Utilities/Interleave.cs:9-166), the byte shuffles the
 // container writers / readers run right after / before the codec path (SURVEY.md 8f rank 2): DspWriter / BrstmWriter
@@ -130,8 +130,8 @@ deinterleave_kernel(const uint8_t *__restrict__ in, int64_t in_item_stride, uint
 // copies.  Here one elected thread per CTA moves them with the bulk-copy engine: cp.async.bulk global -> shared (completion
 // on an mbarrier), cp.async.bulk shared -> global, a ring of kBulkStages buffers of kBulkChunk bytes, persistent CTAs
 // striding over the chunk list.  No thread touches the data.  Eligible when every size, stride and address is a multiple
-// of 16 bytes and the output is fully covered (in_size == out_size); selected with VGB_INTERLEAVE_TMA=1 - measured
-// against the vector kernels in profiles/r02_interleave_tma.md (the vector kernels stay the default: they win).
+// of 16 bytes and the output is fully covered (in_size == out_size); selected with VGB_INTERLEAVE_TMA=1
+// (tools/interleave_bench.py compares it with the vector kernels, which stay the default: they keep more bytes in flight).
 constexpr int kBulkChunk = 8192, kBulkStages = 4;
 
 __device__ __forceinline__ void bulk_load(void *smem, const void *gsrc, uint32_t bytes, uint64_t *mbar)

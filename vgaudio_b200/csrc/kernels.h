@@ -1,4 +1,4 @@
-// kernels.h — host-callable launchers of the sm_100a kernels (internal to libvgaudio_b200.so).
+// kernels.h — host-callable launchers of the sm_90a kernels (internal to libvgaudio_b200.so).
 #pragma once
 
 #include <cuda_runtime.h>

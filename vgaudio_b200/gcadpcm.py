@@ -1,6 +1,6 @@
 """Host-side mirror of VGAudio.Codecs.GcAdpcm over the C ABI (no arithmetic here).
 
-Reference interface (paths under /root/reference/src/VGAudio/):
+Reference interface (paths under VGAudio's src/VGAudio/):
   GcAdpcmMath                          Codecs/GcAdpcm/GcAdpcmMath.cs:7-47
   GcAdpcmCoefficients.CalculateCoefficients(short[])            GcAdpcmCoefficients.cs:9
   GcAdpcmEncoder.Encode(short[], short[], GcAdpcmParameters)     GcAdpcmEncoder.cs:14
