@@ -384,8 +384,13 @@ typedef struct {
     double error;      /* TotalDistance */
 } gc_trial;
 
-/* DspEncodeCoef :96-171 for one predictor pair (c0 = coefs[2p], c1 = coefs[2p+1]) */
-static void try_predictor(const int16_t pcm[16], int n, int16_t c0, int16_t c1, gc_trial *t)
+/* |v| without the overflow of abs(INT32_MIN) */
+static inline uint32_t uabs32(int32_t v) { return v < 0 ? 0u - (uint32_t)v : (uint32_t)v; }
+
+/* DspEncodeCoef :96-171 for one predictor pair (c0 = coefs[2p], c1 = coefs[2p+1]).  st == NULL on the encoding path;
+ * otherwise the facts of the scale chain are recorded there (vgo_gc_encode_trace).  Recording only reads values the
+ * loop computes anyway, so the arithmetic is the same either way. */
+static void try_predictor(const int16_t pcm[16], int n, int16_t c0, int16_t c1, gc_trial *t, vgo_gc_pred_trace *st)
 {
     int32_t peak = 0;
     int32_t over;
@@ -395,7 +400,9 @@ static void try_predictor(const int16_t pcm[16], int n, int16_t c0, int16_t c1, 
 
     /* residual range against the RAW neighbours (:107-115); "/ 2048" truncates toward zero (A.6) */
     for (int s = 0; s < n; s++) {
+        int64_t wide = (int64_t)pcm[s] * c1 + (int64_t)pcm[s + 1] * c0;
         int32_t guess = wrap_add(wrap_mul(pcm[s], c1), wrap_mul(pcm[s + 1], c0)) / 2048;
+        if (st && wide != (int32_t)wide) st->wrapped = 1;
         int32_t diff = sat16(wrap_sub(pcm[s + 2], guess));
         if (abs(diff) > abs(peak)) peak = diff;
     }
@@ -407,6 +414,7 @@ static void try_predictor(const int16_t pcm[16], int n, int16_t c0, int16_t c1, 
         sp++;
     }
     sp = sp <= 1 ? -1 : sp - 2;
+    if (st) st->first_sp = (int8_t)(sp + 1);
 
     /* quantise / reconstruct, growing the scale until the nibbles fit (:127-170) */
     do {
@@ -419,6 +427,11 @@ static void try_predictor(const int16_t pcm[16], int n, int16_t c0, int16_t c1, 
             int32_t want = wrap_mul(pcm[s + 2], 2048);
             int32_t guess = wrap_add(wrap_mul(t->recon[s], c1), wrap_mul(t->recon[s + 1], c0));
             int32_t diff = wrap_sub(want, guess);
+            if (st) {
+                int64_t wide = (int64_t)t->recon[s] * c1 + (int64_t)t->recon[s + 1] * c0;
+                if (wide != (int32_t)wide || (int64_t)want - guess != diff) st->wrapped = 1;
+                if (uabs32(diff) > st->max_abs_diff) st->max_abs_diff = uabs32(diff);
+            }
             /* int -> float32 -> divide in float32 -> widen -> add float32 literal widened -> truncate (A.5) */
             float ratio = (float)diff / (float)scale;
             int32_t raw = (diff > 0) ? (int32_t)((double)ratio + (double)0.4999999f)
@@ -443,25 +456,45 @@ static void try_predictor(const int16_t pcm[16], int n, int16_t c0, int16_t c1, 
          * CalculateCoefficients cannot reach it (|diff| < 2^29 there).  Oracle and CUDA kernel both treat a pass
          * at scalePower 12 as final, which changes nothing for any input on which the reference halts. */
         const int pass_power = sp;
+        if (st) {
+            st->over[st->n_passes++] = over;  /* every pass raises sp by at least one: at most 13 passes */
+            if (over + 8 > 256 && pass_power < 12) st->bumped = 1;
+            if (pass_power >= 12 && over > 1) st->final12 = 1;
+        }
         for (int32_t x = over + 8; x > 256; x >>= 1)
             if (++sp >= 12) sp = 11;
         if (pass_power >= 12) { sp = 12; break; }
     } while (sp < 12 && over > 1);
 
     t->scale_power = sp;
+    if (st) {
+        st->final_sp = (int8_t)sp;
+        st->error = 0;
+        for (int s = 0; s < n; s++) {
+            int64_t miss = (int64_t)pcm[s + 2] - t->recon[s + 2];
+            st->error += (uint64_t)(miss * miss);
+        }
+    }
 }
 
-/* DspEncodeFrame :48-94 */
-void vgo_gc_dsp_encode_frame(int16_t pcm_in_out[16], int sample_count, uint8_t adpcm_out[8], const int16_t coefs[16])
+/* DspEncodeFrame :48-94; st == NULL on the encoding path, else the frame's trace record */
+static void dsp_encode_frame(int16_t pcm_in_out[16], int sample_count, uint8_t adpcm_out[8], const int16_t coefs[16],
+                             vgo_gc_frame_trace *st)
 {
     gc_trial trial[8];
+    if (st) memset(st, 0, sizeof *st);
     for (int p = 0; p < 8; p++)
-        try_predictor(pcm_in_out, sample_count, coefs[2 * p], coefs[2 * p + 1], &trial[p]);
+        try_predictor(pcm_in_out, sample_count, coefs[2 * p], coefs[2 * p + 1], &trial[p], st ? &st->pred[p] : NULL);
 
     int pick = 0;
     double least = 1.7976931348623157e308; /* double.MaxValue; strict < keeps the first minimum (A.9) */
     for (int p = 0; p < 8; p++)
         if (trial[p].error < least) { least = trial[p].error; pick = p; }
+    if (st) {
+        st->winner = (int8_t)pick;
+        for (int p = 0; p < 8; p++)
+            if (p != pick && st->pred[p].error == st->pred[pick].error) st->tie = 1;
+    }
 
     for (int s = 0; s < sample_count; s++) pcm_in_out[s + 2] = (int16_t)trial[pick].recon[s + 2];
     adpcm_out[0] = nibbles(pick, trial[pick].scale_power);
@@ -469,9 +502,14 @@ void vgo_gc_dsp_encode_frame(int16_t pcm_in_out[16], int sample_count, uint8_t a
     for (int i = 0; i < 7; i++) adpcm_out[i + 1] = nibbles(trial[pick].nib[2 * i], trial[pick].nib[2 * i + 1]);
 }
 
-/* Encode :14-46 */
-void vgo_gc_encode(const int16_t *pcm, int pcm_length, const int16_t coefs[16],
-                   int sample_count, int16_t history1, int16_t history2, uint8_t *adpcm_out)
+void vgo_gc_dsp_encode_frame(int16_t pcm_in_out[16], int sample_count, uint8_t adpcm_out[8], const int16_t coefs[16])
+{
+    dsp_encode_frame(pcm_in_out, sample_count, adpcm_out, coefs, NULL);
+}
+
+/* Encode :14-46; trace_out == NULL on the encoding path, else one record per frame */
+static void encode(const int16_t *pcm, int pcm_length, const int16_t coefs[16], int sample_count, int16_t history1,
+                   int16_t history2, uint8_t *adpcm_out, vgo_gc_frame_trace *trace_out)
 {
     if (sample_count == -1) sample_count = pcm_length;
     int16_t window[2 + FRAME_SAMPLES];
@@ -486,13 +524,27 @@ void vgo_gc_encode(const int16_t *pcm, int pcm_length, const int16_t coefs[16],
         memcpy(window + 2, pcm + (size_t)f * FRAME_SAMPLES, (size_t)take * sizeof(int16_t));
         memset(window + 2 + take, 0, (size_t)(FRAME_SAMPLES - take) * sizeof(int16_t));
 
-        vgo_gc_dsp_encode_frame(window, FRAME_SAMPLES, packed, coefs);
+        dsp_encode_frame(window, FRAME_SAMPLES, packed, coefs, trace_out ? &trace_out[f] : NULL);
 
         memcpy(adpcm_out + (size_t)f * FRAME_BYTES, packed, (size_t)vgo_gc_sample_count_to_byte_count(take));
         window[0] = window[14];
         window[1] = window[15];
     }
 }
+
+void vgo_gc_encode(const int16_t *pcm, int pcm_length, const int16_t coefs[16],
+                   int sample_count, int16_t history1, int16_t history2, uint8_t *adpcm_out)
+{
+    encode(pcm, pcm_length, coefs, sample_count, history1, history2, adpcm_out, NULL);
+}
+
+void vgo_gc_encode_trace(const int16_t *pcm, int pcm_length, const int16_t coefs[16], int sample_count,
+                         int16_t history1, int16_t history2, uint8_t *adpcm_out, vgo_gc_frame_trace *trace_out)
+{
+    encode(pcm, pcm_length, coefs, sample_count, history1, history2, adpcm_out, trace_out);
+}
+
+int vgo_gc_frame_trace_size(void) { return (int)sizeof(vgo_gc_frame_trace); }
 
 /* ------------------------------------------------------------------------------------------------
  * Decoder (GcAdpcmDecoder.cs:10-54)

@@ -109,6 +109,33 @@ def encode(pcm, coefs, sample_count: int = -1, history1: int = 0, history2: int 
     return out
 
 
+GC_PRED_TRACE = np.dtype([("error", np.uint64), ("max_abs_diff", np.uint32), ("over", np.int32, 13),
+                          ("first_sp", np.int8), ("n_passes", np.int8), ("final_sp", np.int8), ("bumped", np.uint8),
+                          ("final12", np.uint8), ("wrapped", np.uint8), ("pad", np.uint8, 2)], align=True)
+GC_FRAME_TRACE = np.dtype([("pred", GC_PRED_TRACE, 8), ("winner", np.int8), ("tie", np.uint8), ("pad", np.uint8, 6)],
+                          align=True)
+
+
+def gc_encode_trace(pcm, coefs, sample_count: int = -1, h1: int = 0, h2: int = 0):
+    """encode() plus one vgo_gc_frame_trace record per frame: (adpcm bytes, structured array of GC_FRAME_TRACE)."""
+    L = lib()
+    if not getattr(L, "_trace_ready", False):
+        L.vgo_gc_encode_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int16, C.c_int16, C.c_void_p,
+                                          C.c_void_p]
+        L.vgo_gc_encode_trace.restype = None
+        if L.vgo_gc_frame_trace_size() != GC_FRAME_TRACE.itemsize:
+            raise RuntimeError("vgo_gc_frame_trace layout differs from GC_FRAME_TRACE")
+        L._trace_ready = True
+    pcm = np.ascontiguousarray(pcm, dtype=np.int16)
+    coefs = np.ascontiguousarray(coefs, dtype=np.int16)
+    n = len(pcm) if sample_count == -1 else sample_count
+    out = np.zeros(sample_count_to_byte_count(n), dtype=np.uint8)
+    trace = np.zeros((n + 13) // 14, dtype=GC_FRAME_TRACE)
+    L.vgo_gc_encode_trace(pcm.ctypes.data, len(pcm), coefs.ctypes.data, sample_count, h1, h2, out.ctypes.data,
+                          trace.ctypes.data)
+    return out, trace
+
+
 def dsp_encode_frame(pcm_in_out: np.ndarray, sample_count: int, coefs) -> np.ndarray:
     assert pcm_in_out.dtype == np.int16 and pcm_in_out.flags.c_contiguous and pcm_in_out.size == 16
     coefs = np.ascontiguousarray(coefs, dtype=np.int16)

@@ -61,6 +61,30 @@ void vgo_gc_encode(const int16_t *pcm, int pcm_length, const int16_t coefs[16],
  * reconstructed samples. */
 void vgo_gc_dsp_encode_frame(int16_t pcm_in_out[16], int sample_count, uint8_t adpcm_out[8], const int16_t coefs[16]);
 
+/* Encode with a per-frame record of the reference-level facts of DspEncodeCoef's scale chain (:118-170) and of the
+ * argmin (:66-76), so that tests can show which rare paths an input reaches.  Same bytes as vgo_gc_encode. */
+typedef struct vgo_gc_pred_trace {
+    uint64_t error;          /* final TotalDistance as an exact integer */
+    uint32_t max_abs_diff;   /* max |want - guess| over all passes (wrapping int32 diff) */
+    int32_t over[13];        /* maxOverflow of every pass, in order (a chain has at most 13 passes) */
+    int8_t first_sp;         /* scalePower of the first pass */
+    int8_t n_passes;         /* number of do/while passes */
+    int8_t final_sp;         /* scalePower written to the header */
+    uint8_t bumped;          /* some pass at a power < 12 had over + 8 > 256 (:166-168) */
+    uint8_t final12;         /* the chain ended on a pass at scalePower 12 with over > 1 */
+    uint8_t wrapped;         /* some prediction sum (residual pass or any pass), or a pass's want - guess, wrapped int32 */
+    uint8_t pad[2];
+} vgo_gc_pred_trace;
+typedef struct vgo_gc_frame_trace {
+    vgo_gc_pred_trace pred[8];
+    int8_t winner;           /* the predictor written to the header */
+    uint8_t tie;             /* another predictor has exactly the winner's error */
+    uint8_t pad[6];
+} vgo_gc_frame_trace;
+void vgo_gc_encode_trace(const int16_t *pcm, int pcm_length, const int16_t coefs[16], int sample_count,
+                         int16_t history1, int16_t history2, uint8_t *adpcm_out, vgo_gc_frame_trace *trace_out);
+int vgo_gc_frame_trace_size(void); /* sizeof(vgo_gc_frame_trace), checked by the Python wrapper */
+
 /* ---- GcAdpcmDecoder.Decode (Codecs/GcAdpcm/GcAdpcmDecoder.cs:10-54) ---- */
 void vgo_gc_decode(const uint8_t *adpcm, const int16_t coefs[16], int sample_count,
                    int16_t history1, int16_t history2, int16_t *pcm_out);

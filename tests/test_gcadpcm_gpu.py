@@ -112,6 +112,7 @@ def test_extreme_coefficients_wrap_like_int32(vg, oracle):
     rng = np.random.default_rng(11)
     pcm = np.where(rng.random(14 * 400) < 0.5, -32768, 32767).astype(np.int16)
     pcm[::3] = rng.integers(-32768, 32768, len(pcm[::3]))
+    all_coefs, wants = [], []
     for trial in range(6):
         coefs = rng.choice(np.array([-32768, 32767, -20000, 20000, 0, 2048], dtype=np.int16), 16)
         got = vg.gcadpcm.encode(pcm, coefs)
@@ -119,6 +120,12 @@ def test_extreme_coefficients_wrap_like_int32(vg, oracle):
         assert got.tobytes() == want.tobytes(), trial
         dec = vg.gcadpcm.decode(got, coefs, vg.gcadpcm.GcAdpcmParameters(len(pcm)))
         assert np.array_equal(dec, oracle.decode(want, coefs, len(pcm)))
+        all_coefs.append(coefs)
+        wants.append(want)
+    # the same six trials as one batch: the hostile frames also run in quarters 1..3 of a warp
+    _, got = vg.gcadpcm.encode_batch([pcm] * 6, coefs=np.stack(all_coefs))
+    for trial in range(6):
+        assert got[trial].tobytes() == wants[trial].tobytes(), ("batch", trial)
 
 
 def test_decode_hostile_streams(vg, oracle):
@@ -214,7 +221,7 @@ def test_loud_signals_exercise_float32_rounding_regime(vg, oracle):
     n = 14 * 1500
     chans = []
     for i in range(24):
-        kind = i % 4
+        kind = (i + i // 4) % 4  # channel i runs in quarter i % 4: every kind visits every quarter
         if kind == 0:
             x = rng.integers(-32768, 32768, n)                       # white, full scale
         elif kind == 1:
