@@ -9,7 +9,7 @@
 // Mapping: ONE QUARTER-WARP OWNS ONE CHANNEL (four channels per warp).  Lane & 7 = predictor: the 8 predictors are
 // searched in parallel and each lane evaluates 2 consecutive scale powers of its predictor speculatively, as two
 // interleaved recurrences (every attempt is a pure function of (samples, history, coefs, scalePower), so the do/while
-// chain can be replayed over finished attempts inside the lane; a second round covers two more powers; the rare
+// chain can be replayed over finished attempts inside the lane; a second round covers one more power; the rare
 // overflow "bump" (:166-168) falls back to the literal loop).  The argmin over predictors (strict <, first wins,
 // :66-76) is an 8-lane butterfly MIN on an exact integer key; the winner's two newest reconstructed samples are
 // broadcast with one SHFL.  PCM is staged through shared memory 16 frames at a time with coalesced 16-byte loads
@@ -243,14 +243,15 @@ struct GcPass {
     bool valid;          // the candidate is <= 12: the chain can reach it
     int shift;           // sp + 11
     int32_t mul;         // 2^(shift-11)
-    int32_t base_m;      // tm1 = diff + half - 1 = x*2048 + base_m - c0*p1 - c1*p2   (x carries +32768: folded in)
-    int32_t base_g;      // guess + 1024 - 8*2^shift = c0*p1 + c1*p2 + base_g
+    int32_t base_g;      // wf = guess + 1024 - 8*2^shift = c0*p1 + c1*p2 + base_g
+    int32_t base_t;      // tm1 = diff + half - 1 = x*2048 + base_t - wf   (x carries +32768: folded in)
     uint32_t near_c;     // 128 << (32 - shift)
     uint32_t near_k;     // (1 << (32 - shift)) + near_c: (tm1 << lsh) + near_k = (tn << lsh) + near_c with tn = tm1 + 1
     int32_t lmul;        // 1 << (32 - shift)
     int32_t r1, r2;      // newest two reconstructed samples (biased +32768)
     int32_t rmin, rmax, raw_even;
     uint32_t nearmin;    // smallest distance of (diff + half) to a multiple of 2^shift, scaled
+    uint32_t near_even;  // that distance of the last even sample (folded in with the odd one)
     uint32_t nw0, nw1;   // nibbles, biased +8
     uint64_t e0, e1;     // squared error of even / odd samples (exact; < 2^36)
 };
@@ -261,8 +262,9 @@ __device__ __forceinline__ void gc_pass_begin(GcPass &P, int sp_raw, int32_t bia
     P.valid = sp_raw <= 12;
     P.shift = P.sp + 11;
     P.mul = (int32_t)(1u << P.sp);
-    P.base_m = wadd(bias_c, (int32_t)(1u << (P.shift - 1))) - 1 - 32768 * 2048;
     P.base_g = wsub(wsub(1024, (int32_t)(8u << P.shift)), bias_c);
+    // diff + half - 1 = (x - 32768)*2048 - (guess + 1024 - 8*2^shift) + 1024 - 8*2^shift + 2^(shift-1) - 1
+    P.base_t = wadd(P.base_g, wadd(bias_c, (int32_t)(1u << (P.shift - 1))) - 1 - 32768 * 2048);
     const int lsh = 32 - P.shift;
     P.near_c = 128u << lsh;
     P.near_k = (1u << lsh) + P.near_c;
@@ -270,22 +272,23 @@ __device__ __forceinline__ void gc_pass_begin(GcPass &P, int sp_raw, int32_t bia
     P.r1 = p1; P.r2 = p2;
     P.rmin = 0; P.rmax = 0; P.raw_even = 0;
     P.nearmin = 0xFFFFFFFFu;
+    P.near_even = 0xFFFFFFFFu;
     P.nw0 = 0; P.nw1 = 0;
     P.e0 = 0; P.e1 = 0;
 }
 
-// Sample s (a compile-time constant once unrolled) of the recurrence; xs = the sample, biased +32768.  Per sample the
-// dependent chain is IMAD -> LEA.HI -> SHF -> VIADDMNMX.RELU -> IMAD -> VIADDMNMX.RELU; range of raw (maxOverflow),
-// distance to a rounding threshold, squared error and nibble packing ride along as independent work and nothing per
-// sample is kept in registers.  The integer ALU pipe is the busiest unit of this kernel, so adds and shifts of the side
-// work are written as multiply-adds wherever that is exact.
-__device__ __forceinline__ void gc_pass_step(GcPass &P, int s, int32_t xs, int32_t c0, int32_t c1, int32_t nc0, int32_t nc1)
+// Sample s (a compile-time constant once unrolled) of the recurrence; xs = the sample, biased +32768, and xw = xs * 2048
+// (shared by the lane's passes).  Per sample the dependent chain is IMAD -> IADD3 -> LEA.HI -> SHF -> VIADDMNMX.RELU ->
+// IMAD -> VIADDMNMX.RELU; range of raw (maxOverflow), distance to a rounding threshold, squared error and nibble
+// packing ride along as independent work and nothing per sample is kept in registers.  The IMAD and the integer ALU
+// pipes each take one warp instruction every two cycles (DESIGN.md §5.3), so the side work is split between them:
+// tm1 is rebuilt from wf with one IADD3 instead of its own multiply-adds (modulo 2^32,
+// x*2048 + base_m - c0*r1 - c1*r2 == x*2048 + base_t - wf).
+__device__ __forceinline__ void gc_pass_step(GcPass &P, int s, int32_t xs, int32_t xw, int32_t c0, int32_t c1)
 {
-    const int32_t wt = imad(xs, 2048, P.base_m);
-    const int32_t an = imad(P.r2, nc1, wt);          // r2 terms: one step off the chain
-    const int32_t gn = imad(P.r2, c1, P.base_g);
-    const int32_t tm1 = imad(P.r1, nc0, an);         // diff + half - 1          <- chain
-    const int32_t wf = imad(P.r1, c0, gn);           // guess + 1024 - 8*2^shift
+    const int32_t gn = imad(P.r2, c1, P.base_g);     // r2 term: one step off the chain
+    const int32_t wf = imad(P.r1, c0, gn);           // guess + 1024 - 8*2^shift  <- chain
+    const int32_t tm1 = wsub(wadd(xw, P.base_t), wf);  // diff + half - 1 (one IADD3: wf comes out of asm, nothing to re-associate)
     // round half toward zero: (diff + half - (diff > 0)) >> shift = (tm1 + (diff <= 0)) >> shift.  diff <= 0 is
     // tm1 < half, and for 0 <= tm1 < half both tm1 and tm1 + 1 shift to 0: only the SIGN of tm1 matters
     const int32_t t2 = tm1 + (int32_t)((uint32_t)tm1 >> 31);
@@ -301,7 +304,9 @@ __device__ __forceinline__ void gc_pass_step(GcPass &P, int s, int32_t xs, int32
     } else {
         P.raw_even = raw;
     }
-    P.nearmin = min(P.nearmin, (uint32_t)imad(tm1, P.lmul, (int32_t)P.near_k));   // (tm1 << lsh) + near_k
+    const uint32_t near = (uint32_t)imad(tm1, P.lmul, (int32_t)P.near_k);   // (tm1 << lsh) + near_k
+    if (s & 1) P.nearmin = __vimin3_u32(P.nearmin, P.near_even, near);
+    else P.near_even = near;
     const int32_t miss = imad(ob, -1, xs);
     const uint64_t sq = (uint64_t)((int64_t)miss * miss);
     if (s & 1) P.e1 += sq; else P.e0 += sq;
@@ -373,7 +378,7 @@ __host__ __device__ __forceinline__ int gc_seg_len(int range_frames, int seg_cou
 // (samples, history, coefs, scalePower), so the reference's do/while chain :127-170 is replayed over finished passes
 // inside the lane: the first pass that ends the chain wins).  The reference's first guess is deliberately one power
 // low, so on real signals the chain ends at the first pass in ~11 % and at the second in ~88.6 % of predictor-frames;
-// when a predictor needs a third or fourth pass the warp runs a second round with both passes moved up by two.
+// when a predictor needs a third pass the warp runs a second round of one pass; a fourth goes to gc_slow_frame.
 //
 // The per-frame code is DspEncodeFrame (:48-94), written as one software-pipelined block:
 //   head     residual keys of samples 0,1 (they need the reconstructed history) + the 12 keys computed one frame
@@ -421,7 +426,6 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
     uint32_t *used_start = sa.used_start + (int64_t)ch * sa.seg_count;  // [segment] pair the boundary's run-on started from
     const int32_t c0 = coefs[(int64_t)ch * 16 + 2 * pred];
     const int32_t c1 = coefs[(int64_t)ch * 16 + 2 * pred + 1];
-    const int32_t nc0 = -c0, nc1 = -c1;
     const int32_t bias_c = wmul(32768, wadd(c0, c1));  // undoes the +32768 bias of both history samples
     int16_t (*const in_row)[kEncChunkSamples] = in_buf[warp][qc];
     int32_t *const x_row = x_buf[warp][qc];
@@ -575,26 +579,29 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
             bool trouble = false;
 
             // fully unrolled on purpose: in round 0 the next frame's loads/keys must sit in the same straight-line block
-            // as the recurrences to be interleaved with them; the round-1 copy is cold code
+            // as the recurrences to be interleaved with them; the round-1 copy is cold code.  Round 0 runs powers
+            // sp_first and sp_first + 1, round 1 only sp_first + 2: a chain that needs a fourth power is rare enough
+            // (none on the benchmark's signals) to go to gc_slow_frame as unresolved.
 #pragma unroll
             for (int round = 0; round < 2; round++) {
                 GcPass A, B;
                 gc_pass_begin(A, sp_first + 2 * round, bias_c, p1, p2);
-                gc_pass_begin(B, sp_first + 2 * round + 1, bias_c, p1, p2);
+                if (round == 0) gc_pass_begin(B, sp_first + 1, bias_c, p1, p2);
 #pragma unroll
                 for (int s = 0; s < 14; s++) {
-                    gc_pass_step(A, s, x[s], c0, c1, nc0, nc1);
-                    gc_pass_step(B, s, x[s], c0, c1, nc0, nc1);
+                    const int32_t xw = imad(x[s], 2048, 0);
+                    gc_pass_step(A, s, x[s], xw, c0, c1);
+                    if (round == 0) gc_pass_step(B, s, x[s], xw, c0, c1);
                     // independent work for the NEXT frame rides along (software pipelining), first round only
                     if (round == 0 && s == 4) key_rest_next = key_rest_of(frame_next);
                 }
-                bool term_a, trouble_a, term_b, trouble_b;
+                bool term_a, trouble_a, term_b = false, trouble_b = false;
                 gc_pass_end(A, term_a, trouble_a);
-                gc_pass_end(B, term_b, trouble_b);
+                if (round == 0) gc_pass_end(B, term_b, trouble_b);
                 // the first pass that ends the chain wins; B only counts when A did not end it.  Round 1 only
                 // touches predictors round 0 left unresolved.
                 const bool take = round == 0 || !resolved;
-                const bool use_b = !term_a;
+                const bool use_b = round == 0 && !term_a;
                 if (take) {
                     trouble = trouble | (active & (trouble_a | (use_b & trouble_b)));
                     err = use_b ? B.e0 + B.e1 : A.e0 + A.e1;
@@ -607,7 +614,7 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
                 }
                 if (round == 0 && !__any_sync(kFull, !resolved)) break;  // warp-uniform: every predictor of the four channels resolved
             }
-            // a predictor still unresolved after four powers leaves the window: handled as trouble
+            // a predictor still unresolved after three powers leaves the window: handled as trouble
             trouble = trouble | !resolved;
 
             // ---------------- tail: argmin over predictors ----------------
