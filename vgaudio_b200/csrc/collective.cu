@@ -19,12 +19,9 @@
 #include <string>
 #include <vector>
 
-#include "../../include/vgaudio_b200.h"
+#include "abi.cuh"
 
-namespace vgb {
-int32_t abi_fail(int32_t code, const char *fmt, ...);  // c_abi.cu: sets the thread's vgb_last_error()
-}
-using vgb::abi_fail;
+using vgb::fail;
 
 namespace {
 
@@ -53,12 +50,12 @@ int32_t load_api()
     void *h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD | RTLD_GLOBAL);  // the copy this process already uses
     if (!h) h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
     if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
-    if (!h) return abi_fail(VGB_E_NCCL, "libnccl.so.2 not found (%s)", dlerror());
+    if (!h) return fail(VGB_E_NCCL, "libnccl.so.2 not found (%s)", dlerror());
     NcclApi a;
     a.handle = h;
 #define BIND(field, sym)                                                        \
     a.field = reinterpret_cast<decltype(a.field)>(dlsym(h, sym));              \
-    if (!a.field) return abi_fail(VGB_E_NCCL, "libnccl.so.2 lacks %s", sym);
+    if (!a.field) return fail(VGB_E_NCCL, "libnccl.so.2 lacks %s", sym);
     BIND(GetUniqueId, "ncclGetUniqueId")
     BIND(CommInitRank, "ncclCommInitRank")
     BIND(CommDestroy, "ncclCommDestroy")
@@ -77,7 +74,7 @@ int32_t load_api()
 int32_t nccl_fail(const char *what, ncclResult_t r)
 {
     const char *last = (g_api.GetLastError && g_comm) ? g_api.GetLastError(g_comm) : "";
-    return abi_fail(VGB_E_NCCL, "%s failed: %s%s%s", what, g_api.GetErrorString ? g_api.GetErrorString(r) : "?", last && *last ? " - " : "",
+    return fail(VGB_E_NCCL, "%s failed: %s%s%s", what, g_api.GetErrorString ? g_api.GetErrorString(r) : "?", last && *last ? " - " : "",
                     last ? last : "");
 }
 
@@ -93,7 +90,7 @@ extern "C" {
 
 int32_t vgb_nccl_unique_id(uint8_t *id_out)
 {
-    if (!id_out) return abi_fail(VGB_E_ARG, "id_out is NULL");
+    if (!id_out) return fail(VGB_E_ARG, "id_out is NULL");
     std::lock_guard<std::mutex> lock(g_mu);
     if (int32_t rc = load_api()) return rc;
     static_assert(sizeof(ncclUniqueId) == VGB_NCCL_ID_BYTES, "ncclUniqueId is 128 bytes");
@@ -105,9 +102,9 @@ int32_t vgb_nccl_unique_id(uint8_t *id_out)
 
 int32_t vgb_nccl_init(const uint8_t *id, int32_t n_ranks, int32_t rank)
 {
-    if (!id || n_ranks < 1 || rank < 0 || rank >= n_ranks) return abi_fail(VGB_E_ARG, "bad communicator arguments");
+    if (!id || n_ranks < 1 || rank < 0 || rank >= n_ranks) return fail(VGB_E_ARG, "bad communicator arguments");
     std::lock_guard<std::mutex> lock(g_mu);
-    if (g_comm) return abi_fail(VGB_E_STATE, "a communicator already exists; call vgb_nccl_shutdown first");
+    if (g_comm) return fail(VGB_E_STATE, "a communicator already exists; call vgb_nccl_shutdown first");
     if (int32_t rc = load_api()) return rc;
     // The batch path's exchange is a one-to-many scatter / many-to-one gather of large blocks: the root's NVLink port is the
     // limit, and NCCL's default point-to-point channel count leaves most of it idle (32 channels per peer nearly halved
@@ -144,12 +141,12 @@ int32_t vgb_scatterv_dev(const void *d_send, const int64_t *send_offset, const i
                          void *cuda_stream)
 {
     std::lock_guard<std::mutex> lock(g_mu);
-    if (!g_comm) return abi_fail(VGB_E_STATE, "no communicator: call vgb_nccl_init on every rank first");
-    if (!counts || root < 0 || root >= g_ranks) return abi_fail(VGB_E_ARG, "bad arguments");
-    if (g_rank == root && (!d_send || !send_offset)) return abi_fail(VGB_E_ARG, "the root needs d_send and send_offset");
+    if (!g_comm) return fail(VGB_E_STATE, "no communicator: call vgb_nccl_init on every rank first");
+    if (!counts || root < 0 || root >= g_ranks) return fail(VGB_E_ARG, "bad arguments");
+    if (g_rank == root && (!d_send || !send_offset)) return fail(VGB_E_ARG, "the root needs d_send and send_offset");
     for (int r = 0; r < g_ranks; r++)
-        if (counts[r] < 0 || (g_rank == root && send_offset[r] < 0)) return abi_fail(VGB_E_ARG, "rank %d: negative count / offset", r);
-    if (counts[g_rank] > 0 && !d_recv) return abi_fail(VGB_E_ARG, "d_recv is NULL");
+        if (counts[r] < 0 || (g_rank == root && send_offset[r] < 0)) return fail(VGB_E_ARG, "rank %d: negative count / offset", r);
+    if (counts[g_rank] > 0 && !d_recv) return fail(VGB_E_ARG, "d_recv is NULL");
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     NCCL_TRY(g_api.GroupStart());
     if (g_rank == root) {
@@ -160,7 +157,7 @@ int32_t vgb_scatterv_dev(const void *d_send, const int64_t *send_offset, const i
                 if (src + send_offset[r] != d_recv &&
                     cudaMemcpyAsync(d_recv, src + send_offset[r], (size_t)counts[r], cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
                     g_api.GroupEnd();
-                    return abi_fail(VGB_E_CUDA, "device copy of the root's own share failed: %s", cudaGetErrorString(cudaGetLastError()));
+                    return fail(VGB_E_CUDA, "device copy of the root's own share failed: %s", cudaGetErrorString(cudaGetLastError()));
                 }
             } else {
                 NCCL_TRY(g_api.Send(src + send_offset[r], (size_t)counts[r], ncclInt8, r, g_comm, st));
@@ -177,12 +174,12 @@ int32_t vgb_gatherv_dev(const void *d_send, void *d_recv, const int64_t *recv_of
                         void *cuda_stream)
 {
     std::lock_guard<std::mutex> lock(g_mu);
-    if (!g_comm) return abi_fail(VGB_E_STATE, "no communicator: call vgb_nccl_init on every rank first");
-    if (!counts || root < 0 || root >= g_ranks) return abi_fail(VGB_E_ARG, "bad arguments");
-    if (g_rank == root && (!d_recv || !recv_offset)) return abi_fail(VGB_E_ARG, "the root needs d_recv and recv_offset");
+    if (!g_comm) return fail(VGB_E_STATE, "no communicator: call vgb_nccl_init on every rank first");
+    if (!counts || root < 0 || root >= g_ranks) return fail(VGB_E_ARG, "bad arguments");
+    if (g_rank == root && (!d_recv || !recv_offset)) return fail(VGB_E_ARG, "the root needs d_recv and recv_offset");
     for (int r = 0; r < g_ranks; r++)
-        if (counts[r] < 0 || (g_rank == root && recv_offset[r] < 0)) return abi_fail(VGB_E_ARG, "rank %d: negative count / offset", r);
-    if (counts[g_rank] > 0 && !d_send) return abi_fail(VGB_E_ARG, "d_send is NULL");
+        if (counts[r] < 0 || (g_rank == root && recv_offset[r] < 0)) return fail(VGB_E_ARG, "rank %d: negative count / offset", r);
+    if (counts[g_rank] > 0 && !d_send) return fail(VGB_E_ARG, "d_send is NULL");
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     NCCL_TRY(g_api.GroupStart());
     if (g_rank == root) {
@@ -193,7 +190,7 @@ int32_t vgb_gatherv_dev(const void *d_send, void *d_recv, const int64_t *recv_of
                 if (dst + recv_offset[r] != d_send &&
                     cudaMemcpyAsync(dst + recv_offset[r], d_send, (size_t)counts[r], cudaMemcpyDeviceToDevice, st) != cudaSuccess) {
                     g_api.GroupEnd();
-                    return abi_fail(VGB_E_CUDA, "device copy of the root's own share failed: %s", cudaGetErrorString(cudaGetLastError()));
+                    return fail(VGB_E_CUDA, "device copy of the root's own share failed: %s", cudaGetErrorString(cudaGetLastError()));
                 }
             } else {
                 NCCL_TRY(g_api.Recv(dst + recv_offset[r], (size_t)counts[r], ncclInt8, r, g_comm, st));
@@ -210,15 +207,15 @@ int32_t vgb_sendrecv_dev(const void *const *send_ptr, const int64_t *send_bytes,
                          void *const *recv_ptr, const int64_t *recv_bytes, const int32_t *recv_peer, int32_t n_recv, void *cuda_stream)
 {
     std::lock_guard<std::mutex> lock(g_mu);
-    if (!g_comm) return abi_fail(VGB_E_STATE, "no communicator: call vgb_nccl_init on every rank first");
+    if (!g_comm) return fail(VGB_E_STATE, "no communicator: call vgb_nccl_init on every rank first");
     if (n_send < 0 || n_recv < 0 || (n_send > 0 && (!send_ptr || !send_bytes || !send_peer)) || (n_recv > 0 && (!recv_ptr || !recv_bytes || !recv_peer)))
-        return abi_fail(VGB_E_ARG, "bad arguments");
+        return fail(VGB_E_ARG, "bad arguments");
     for (int i = 0; i < n_send; i++)
         if (send_bytes[i] < 0 || send_peer[i] < 0 || send_peer[i] >= g_ranks || send_peer[i] == g_rank || (send_bytes[i] > 0 && !send_ptr[i]))
-            return abi_fail(VGB_E_ARG, "send %d: bad peer / size / pointer", i);
+            return fail(VGB_E_ARG, "send %d: bad peer / size / pointer", i);
     for (int i = 0; i < n_recv; i++)
         if (recv_bytes[i] < 0 || recv_peer[i] < 0 || recv_peer[i] >= g_ranks || recv_peer[i] == g_rank || (recv_bytes[i] > 0 && !recv_ptr[i]))
-            return abi_fail(VGB_E_ARG, "recv %d: bad peer / size / pointer", i);
+            return fail(VGB_E_ARG, "recv %d: bad peer / size / pointer", i);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     NCCL_TRY(g_api.GroupStart());
     for (int i = 0; i < n_send; i++)
@@ -231,7 +228,7 @@ int32_t vgb_sendrecv_dev(const void *const *send_ptr, const int64_t *send_bytes,
 
 int32_t vgb_partition_lpt(const int64_t *weight, int32_t n_units, int32_t n_parts, int32_t *part_out, int64_t *load_out)
 {
-    if (n_units < 0 || n_parts < 1 || (n_units > 0 && (!weight || !part_out))) return abi_fail(VGB_E_ARG, "bad arguments");
+    if (n_units < 0 || n_parts < 1 || (n_units > 0 && (!weight || !part_out))) return fail(VGB_E_ARG, "bad arguments");
     std::vector<int32_t> order(n_units);
     for (int i = 0; i < n_units; i++) order[i] = i;
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] > weight[b]; });

@@ -12,45 +12,16 @@
 // All of it is HBM-bound byte work (every payload byte read once, written once); headers are a few dozen bytes per file
 // and are built on the host, except the fields that only exist on the device (DSP: coefficients, first predictor/scale
 // byte, loop context), which the assemble kernel patches in.  Citations are relative to VGAudio's src/VGAudio/.
-#include <cuda_runtime.h>
-
-#include <algorithm>
 #include <chrono>
 #include <cmath>
 #include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <mutex>
-#include <string>
-#include <vector>
 
-#include "../../include/vgaudio_b200.h"
-#include "common.cuh"
+#include "abi.cuh"
 
-namespace vgb {
-int32_t abi_fail(int32_t code, const char *fmt, ...);  // c_abi.cu: sets the thread's vgb_last_error()
-int32_t abi_ensure_ready();                            // c_abi.cu: binds / selects the primary device
-void abi_count_launches(int n);                        // c_abi.cu: vgb_kernel_launch_count bookkeeping
-}  // namespace vgb
-using vgb::abi_fail;
-using namespace vgb;  // common.cuh: GcAdpcmMath helpers, frame constants
+using namespace vgb;  // the shared host runtime; common.cuh: GcAdpcmMath helpers, frame constants
 
 namespace {
 
-#define CTN_CUDA(expr)                                                                                            \
-    do {                                                                                                          \
-        cudaError_t e_ = (expr);                                                                                  \
-        if (e_ != cudaSuccess)                                                                                    \
-            return abi_fail(e_ == cudaErrorMemoryAllocation ? VGB_E_NOMEM : VGB_E_CUDA, "%s failed: %s", #expr,   \
-                            cudaGetErrorString(e_));                                                              \
-    } while (0)
-#define CTN_TRY(expr)                \
-    do {                             \
-        int32_t s_ = (expr);         \
-        if (s_ != VGB_OK) return s_; \
-    } while (0)
-
-inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 inline int next_multiple(int value, int multiple)  // Utilities/Helpers.cs:71-80
 {
     if (multiple <= 0) return value;
@@ -480,24 +451,6 @@ __global__ void __launch_bounds__(kHcaFramesPerTile * 32) hca_assemble_kernel(co
 // ---------------------------------------------------------------------------------------------------------------
 // host state of this translation unit: its own slabs and streams on the library's primary device
 // ---------------------------------------------------------------------------------------------------------------
-struct Slab {
-    void *p = nullptr;
-    size_t cap = 0;
-    int32_t reserve(size_t bytes)
-    {
-        if (bytes <= cap && p) return VGB_OK;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
-        const size_t want = std::max<size_t>(bytes + bytes / 8, 4096);
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) { (void)cudaGetLastError(); p = nullptr; return abi_fail(VGB_E_NOMEM, "cudaMalloc(%zu) failed: %s", want, cudaGetErrorString(e)); }
-        cap = want;
-        return VGB_OK;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    char *c() const { return static_cast<char *>(p); }
-};
-
 constexpr int kWays = 4;  // groups of the batch converter in flight: each has its own working set and kernel stream
 
 struct State {
@@ -506,8 +459,8 @@ struct State {
     cudaStream_t s_in = nullptr, s_out = nullptr, s_kern[kWays] = {};
     cudaStream_t s_k = nullptr;  // = s_kern[0]: the stream of the single-shot entry points
     cudaEvent_t ev_in[kWays] = {}, ev_split[kWays] = {}, ev_k[kWays] = {}, ev_out[kWays] = {};
-    Slab in[kWays], out[kWays], tab[kWays], pcms[kWays], encs[kWays], decs[kWays], coefss[kWays], wss[kWays];
-    Slab &pcm = pcms[0], &enc = encs[0], &coefs = coefss[0];  // working set 0 doubles as the single-shot entry points'
+    DevBuf in[kWays], out[kWays], tab[kWays], pcms[kWays], encs[kWays], decs[kWays], coefss[kWays], wss[kWays];
+    DevBuf &pcm = pcms[0], &enc = encs[0], &coefs = coefss[0];  // working set 0 doubles as the single-shot entry points'
     // stage timers of the batch converter: per group 5 events (start, split done, encode done, context done, assembled)
     static constexpr int kTimedGroups = 32, kStageEvents = 5;
     cudaEvent_t stage[kTimedGroups][kStageEvents] = {};
@@ -517,19 +470,19 @@ State g_st;
 
 int32_t ensure_state()
 {
-    CTN_TRY(vgb::abi_ensure_ready());
+    VGB_TRY(vgb::abi_ensure_ready());
     if (g_st.ready) return VGB_OK;
-    CTN_CUDA(cudaStreamCreateWithFlags(&g_st.s_in, cudaStreamNonBlocking));
-    CTN_CUDA(cudaStreamCreateWithFlags(&g_st.s_out, cudaStreamNonBlocking));
+    CUDA_TRY(cudaStreamCreateWithFlags(&g_st.s_in, cudaStreamNonBlocking));
+    CUDA_TRY(cudaStreamCreateWithFlags(&g_st.s_out, cudaStreamNonBlocking));
     for (int i = 0; i < kWays; i++) {
-        CTN_CUDA(cudaStreamCreateWithFlags(&g_st.s_kern[i], cudaStreamNonBlocking));
-        CTN_CUDA(cudaEventCreateWithFlags(&g_st.ev_in[i], cudaEventDisableTiming));
-        CTN_CUDA(cudaEventCreateWithFlags(&g_st.ev_split[i], cudaEventDisableTiming));
-        CTN_CUDA(cudaEventCreateWithFlags(&g_st.ev_k[i], cudaEventDisableTiming));
-        CTN_CUDA(cudaEventCreateWithFlags(&g_st.ev_out[i], cudaEventDisableTiming));
+        CUDA_TRY(cudaStreamCreateWithFlags(&g_st.s_kern[i], cudaStreamNonBlocking));
+        CUDA_TRY(cudaEventCreateWithFlags(&g_st.ev_in[i], cudaEventDisableTiming));
+        CUDA_TRY(cudaEventCreateWithFlags(&g_st.ev_split[i], cudaEventDisableTiming));
+        CUDA_TRY(cudaEventCreateWithFlags(&g_st.ev_k[i], cudaEventDisableTiming));
+        CUDA_TRY(cudaEventCreateWithFlags(&g_st.ev_out[i], cudaEventDisableTiming));
     }
     g_st.s_k = g_st.s_kern[0];
-    for (auto &grp : g_st.stage) for (auto &e : grp) CTN_CUDA(cudaEventCreate(&e));
+    for (auto &grp : g_st.stage) for (auto &e : grp) CUDA_TRY(cudaEventCreate(&e));
     g_st.ready = true;
     return VGB_OK;
 }
@@ -545,30 +498,6 @@ struct Drain {  // no copy may be in flight on caller memory once an entry point
     }
 };
 
-// Many small copies in one driver call (cudaMemcpyBatchAsync, CUDA 12.8+): a batch of thousands of files otherwise spends
-// more host time in cudaMemcpyAsync calls than the copies take on the link.  Falls back to one call per copy.
-struct CopyList {
-    std::vector<void *> dst, src;
-    std::vector<size_t> size;
-    void add(void *d, const void *s, size_t n) { if (n) { dst.push_back(d); src.push_back(const_cast<void *>(s)); size.push_back(n); } }
-    int32_t run(cudaMemcpyKind kind, cudaStream_t st)
-    {
-        const size_t n = size.size();
-        if (n == 0) return VGB_OK;
-        static bool batch_ok = std::getenv("VGB_NO_MEMCPY_BATCH") == nullptr;
-        if (batch_ok && n >= 16) {
-            cudaMemcpyAttributes attr{};
-            attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;  // sources stay valid until the entry point has drained its streams
-            size_t attr_idx = 0, fail_idx = 0;
-            if (cudaMemcpyBatchAsync(dst.data(), src.data(), size.data(), n, &attr, &attr_idx, 1, &fail_idx, st) == cudaSuccess) return VGB_OK;
-            (void)cudaGetLastError();
-            batch_ok = false;
-        }
-        for (size_t i = 0; i < n; i++) CTN_CUDA(cudaMemcpyAsync(dst[i], src[i], size[i], kind, st));
-        return VGB_OK;
-    }
-};
-
 void be16(uint8_t *p, int v) { p[0] = (uint8_t)(v >> 8); p[1] = (uint8_t)v; }
 void be32(uint8_t *p, int32_t v) { be16(p, (int)((uint32_t)v >> 16)); be16(p + 2, (int)((uint32_t)v & 0xffff)); }
 int32_t rd_le32(const uint8_t *p) { return (int32_t)((uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24)); }
@@ -576,21 +505,18 @@ int rd_le16(const uint8_t *p) { return p[0] | (p[1] << 8); }
 int rd_be16s(const uint8_t *p) { return (int16_t)((p[0] << 8) | p[1]); }
 int32_t rd_be32(const uint8_t *p) { return (int32_t)(((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | (uint32_t)p[3]); }
 
-int gc_sample_to_nibble(int s) { return s / 14 * 16 + s % 14 + 2; }              // GcAdpcmMath.cs:38-44
-int gc_nibble_to_sample(int nib) { return 14 * (nib / 16) + nib % 16 - 2; }       // GcAdpcmMath.cs:29-36 (no clamp: header nibbles 0, 1 give -2, -1)
-
 // ---- DSP geometry (DspWriter.cs:17-36, :105-106) ----
 struct DspGeom { int align, loop_start, loop_end, sample_count, data_size, bpi, in_size; };
 int32_t dsp_geometry(const vgb_dsp_desc &d, DspGeom &g, int index)
 {
-    if (d.channel_count < 1 || d.channel_count > 255) return abi_fail(VGB_E_ARG, "file %d: channel_count %d outside 1..255", index, d.channel_count);
-    if (d.sample_count < 0) return abi_fail(VGB_E_ARG, "file %d: negative sample count", index);
+    if (d.channel_count < 1 || d.channel_count > 255) return fail(VGB_E_ARG, "file %d: channel_count %d outside 1..255", index, d.channel_count);
+    if (d.sample_count < 0) return fail(VGB_E_ARG, "file %d: negative sample count", index);
     const int spi = d.samples_per_interleave == 0 ? 0x3800 : d.samples_per_interleave;
     if (spi < 1 || spi % 14 != 0)  // DspConfiguration.cs:29-44
-        return abi_fail(VGB_E_ARG, "file %d: samples per interleave (%d) must be positive and divisible by 14", index, spi);
+        return fail(VGB_E_ARG, "file %d: samples per interleave (%d) must be positive and divisible by 14", index, spi);
     const int lpa = d.loop_point_alignment == 0 ? 1 : d.loop_point_alignment;
     if (d.looping && (d.loop_start < 0 || d.loop_end < d.loop_start || d.loop_end > d.sample_count))
-        return abi_fail(VGB_E_ARG, "file %d: loop points %d..%d outside 0..%d", index, d.loop_start, d.loop_end, d.sample_count);
+        return fail(VGB_E_ARG, "file %d: loop points %d..%d outside 0..%d", index, d.loop_start, d.loop_end, d.sample_count);
     g.align = next_multiple(d.loop_start, lpa) - d.loop_start;
     g.loop_start = d.loop_start + g.align;
     g.loop_end = d.loop_end + g.align;
@@ -600,7 +526,7 @@ int32_t dsp_geometry(const vgb_dsp_desc &d, DspGeom &g, int index)
     g.bpi = gc_sample_count_to_byte_count(spi);
     // mono: Stream.Write(array, 0, count) with count past the array throws ArgumentException (DspWriter.cs:91)
     if (d.channel_count == 1 && gc_sample_count_to_byte_count(g.sample_count) > g.in_size)
-        return abi_fail(VGB_E_ARG, "file %d: the aligned loop end (%d) lies past the encoded audio (%d samples)", index, g.loop_end, d.sample_count);
+        return fail(VGB_E_ARG, "file %d: the aligned loop end (%d) lies past the encoded audio (%d samples)", index, g.loop_end, d.sample_count);
     return VGB_OK;
 }
 
@@ -613,9 +539,9 @@ int adx_bytes(int samples, int frame_size)  // CriAdxHelpers.SampleCountToByteCo
 struct AdxGeom { int sample_count, frame_count, base_header, alignment_bytes, header_size, audio_offset, audio_size, footer_offset, footer_size, loop_start, loop_end; };
 int32_t adx_geometry(const vgb_adx_desc &d, AdxGeom &g, int index)
 {
-    if (d.channel_count < 1 || d.channel_count > 255) return abi_fail(VGB_E_ARG, "file %d: channel_count %d outside 1..255", index, d.channel_count);
-    if (d.frame_size < 3 || d.frame_size > 255) return abi_fail(VGB_E_ARG, "file %d: frame_size %d outside 3..255", index, d.frame_size);
-    if (d.sample_count < 0 || d.alignment_samples < 0) return abi_fail(VGB_E_ARG, "file %d: negative count", index);
+    if (d.channel_count < 1 || d.channel_count > 255) return fail(VGB_E_ARG, "file %d: channel_count %d outside 1..255", index, d.channel_count);
+    if (d.frame_size < 3 || d.frame_size > 255) return fail(VGB_E_ARG, "file %d: frame_size %d outside 3..255", index, d.frame_size);
+    if (d.sample_count < 0 || d.alignment_samples < 0) return fail(VGB_E_ARG, "file %d: negative count", index);
     const int spf = (d.frame_size - 2) * 2;
     g.loop_start = d.loop_start + d.alignment_samples;
     g.loop_end = d.loop_end + d.alignment_samples;
@@ -710,7 +636,7 @@ uint16_t crc16_host(const uint8_t *data, size_t n)  // Crc16.Compute (Utilities/
 int32_t hca_build_header(const vgb_hca_info &h, bool masked, int key_type, const char *comment, uint32_t volume_bits,
                          std::vector<uint8_t> &out, int index)
 {
-    if (h.header_size < 8 || h.header_size > 0xffff) return abi_fail(VGB_E_ARG, "file %d: header_size %d", index, h.header_size);
+    if (h.header_size < 8 || h.header_size > 0xffff) return fail(VGB_E_ARG, "file %d: header_size %d", index, h.header_size);
     out.assign((size_t)h.header_size + 64 + (comment ? std::strlen(comment) : 0), 0);
     uint8_t *p = out.data();
     auto id = [&](const char *s, int n) { for (int i = 0; i < n; i++) { uint8_t b = (uint8_t)s[i]; if (masked && b) b |= 0x80; p[i] = b; } p += n; };
@@ -727,7 +653,7 @@ int32_t hca_build_header(const vgb_hca_info &h, bool masked, int key_type, const
     if (comment) for (const char *c = comment; *c; c++) if (!std::strchr(" \t\n\r\v\f", *c)) blank = false;
     if (blank) id("pad", 3);
     else { id("comm\0", 5); const size_t n = std::strlen(comment); std::memcpy(p, comment, n); p += n + 1; }
-    if (p - out.data() > h.header_size - 2) return abi_fail(VGB_E_ARG, "file %d: header_size %d cannot hold the chunks (%d bytes)", index, h.header_size, (int)(p - out.data()) + 2);
+    if (p - out.data() > h.header_size - 2) return fail(VGB_E_ARG, "file %d: header_size %d cannot hold the chunks (%d bytes)", index, h.header_size, (int)(p - out.data()) + 2);
     out.resize((size_t)h.header_size);
     be16(out.data() + h.header_size - 2, crc16_host(out.data(), (size_t)h.header_size - 2));
     return VGB_OK;
@@ -767,7 +693,7 @@ int32_t hca_key_tables(int key_type, uint64_t key_code, uint8_t *dec, uint8_t *e
         for (int i = 0; i < 256; i++) { x = (uint8_t)(x + 17); if (t[x] != 0 && t[x] != 0xff) dec[pos++] = t[x]; }
         dec[0xff] = 0xff;
     } else {
-        return abi_fail(VGB_E_ARG, "HCA key type %d (0, 1 or 56)", key_type);
+        return fail(VGB_E_ARG, "HCA key type %d (0, 1 or 56)", key_type);
     }
     for (int i = 0; i < 256; i++) enc[dec[i]] = (uint8_t)i;
     return VGB_OK;
@@ -788,10 +714,10 @@ int32_t launch_wave_split(const uint8_t *d_in, std::vector<WaveItem> &items, voi
     // items without tiles must not be found by the search: drop them
     std::vector<WaveItem> live;
     for (auto &w : items) if (w.samples > 0) live.push_back(w);
-    CTN_CUDA(cudaMemcpyAsync(d_items, live.data(), live.size() * sizeof(WaveItem), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_items, live.data(), live.size() * sizeof(WaveItem), cudaMemcpyHostToDevice, st));
     wave_split_kernel<<<tiles, 256, 0, st>>>(d_in, static_cast<const WaveItem *>(d_items), (int)live.size(), d_pcm);
     vgb::abi_count_launches(1);
-    CTN_CUDA(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     return VGB_OK;
 }
 
