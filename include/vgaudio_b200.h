@@ -246,6 +246,12 @@ int32_t vgb_gcadpcm_debug_splice_stats(uint64_t *out, int32_t n);
 /* Debug/test taps (tests/ only): run coefficient phase 1 and return, per frame, the direct-form pair and the
  * accept flag the refinement consumes.  Host buffers; dir_out [frames][2] doubles, accepted_out [frames] bytes. */
 int32_t vgb_gcadpcm_debug_records(const int16_t *pcm, int32_t n_samples, double *dir_out, uint8_t *accepted_out);
+/* Debug/test tap (tests/ only): coefficient phase 1 and the refinement for a ragged batch, with what every refinement
+ * pass leaves: pass 0 is the ordered mean, passes 1..6 split and reassign with 2, 2, 4, 4, 8, 8 centroids.  warps (4 or 8)
+ * picks the refinement's CTA width directly.  Host buffers: cent_out [ch][7][8][2] doubles (c1, c2 of every centroid),
+ * hits_out [ch][7][8] (records per bucket), coefs_out [ch][16]. */
+int32_t vgb_gcadpcm_debug_refine_trace(const int16_t *const *pcm, const int32_t *n_samples, int32_t n_channels, int32_t warps,
+                                       double *cent_out, int32_t *hits_out, int16_t *coefs_out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * CRI ADX (Codecs/CriAdx/CriAdxCodec.cs), host buffers.  One call replaces one Parallel.For over channels

@@ -99,13 +99,14 @@ static void covariance(double m[3][3], const int16_t win[28])
         }
 }
 
-/* AnalyzeRanges :133-208 — scaled partial-pivot LU of the 2x2 block; returns 1 to REJECT the frame */
+/* AnalyzeRanges :133-208 — scaled partial-pivot LU of the 2x2 block; returns a VGO_GC_REJ_* reason to REJECT the frame,
+ * 0 to keep it */
 static int lu_reject(double m[3][3], int perm[3], double inv_row_max[3])
 {
     for (int r = 1; r <= 2; r++) {
         double big = fmax(fabs(m[r][1]), fabs(m[r][2]));
         if (big < 4.9406564584124654e-324) /* double.Epsilon: smallest denormal (A.2) */
-            return 1;
+            return VGO_GC_REJ_BIG;
         inv_row_max[r] = 1.0 / big;
     }
 
@@ -145,7 +146,7 @@ static int lu_reject(double m[3][3], int perm[3], double inv_row_max[3])
         if (t < lo) lo = t;
         if (t > hi) hi = t;
     }
-    return lo / hi < 1.0e-10;
+    return lo / hi < 1.0e-10 ? VGO_GC_REJ_RANGE : 0;
 }
 
 /* BidirectionalFilter :210-237 — permuted forward substitution, then back substitution */
@@ -170,17 +171,17 @@ static void lu_solve(double m[3][3], const int perm[3], double v[3])
     v[0] = 1.0;
 }
 
-/* QuadraticMerge :239-255 — returns 1 to REJECT */
+/* QuadraticMerge :239-255 — returns a VGO_GC_REJ_* reason to REJECT, 0 to keep */
 static int to_reflection(double v[3])
 {
     double k2 = v[2];
     double den = 1.0 - (k2 * k2);
-    if (den == 0.0) return 1;
+    if (den == 0.0) return VGO_GC_REJ_DEN;
     double a = (v[0] - (k2 * k2)) / den;
     double b = (v[1] - (v[1] * k2)) / den;
     v[0] = a;
     v[1] = b;
-    return fabs(b) > 1.0;
+    return fabs(b) > 1.0 ? VGO_GC_REJ_K1 : 0;
 }
 
 /* FinishRecord :257-283 (both overloads share the arithmetic) */
@@ -240,13 +241,48 @@ static double contrast(const double c[3], const double rec[3])
     return e0 + (2.0 * q * e1) + (2.0 * (-rec[1] * q + -rec[2]) * e2);
 }
 
-/* FilterRecords :344-396 — two rounds of nearest-centroid assignment + ordered mean */
-static void refine_centroids(double best[8][3], int count, const double (*records)[3], int n_records)
+/* Trace of one refinement pass: the record's minimum distance `least` is shared by more than one centroid (vgo_gc_coef_trace) */
+static void note_tie(vgo_gc_coef_pass *st, const double best[8][3], const double dist[8], int count, double least, int z)
+{
+    int lo = -1, hi = -1, n = 0, same = 1;
+    for (int c = 0; c < count; c++) {
+        if (!(dist[c] == least)) continue;
+        if (lo < 0) lo = c;
+        else if (memcmp(best[c], best[lo], sizeof best[c]) != 0) same = 0;
+        hi = c;
+        n++;
+    }
+    if (n < 2) return;
+    if (same) st->ties_same++;
+    else st->ties_distinct++;
+    if (st->tie_record < 0) {
+        st->tie_record = z;
+        st->tie_lo = lo;
+        st->tie_hi = hi;
+    }
+}
+
+/* After a pass: the centroids and bucket counts it leaves (vgo_gc_coef_trace) */
+static void note_pass(vgo_gc_coef_pass *st, const double best[8][3], const int *hits, int count)
+{
+    st->count = count;
+    for (int z = 0; z < 8; z++) {
+        st->cent[z][0] = best[z][1];
+        st->cent[z][1] = best[z][2];
+        st->hits[z] = z < count ? hits[z] : 0;
+        if (z < count && hits[z] == 0) st->empty++;
+    }
+}
+
+/* FilterRecords :344-396 — two rounds of nearest-centroid assignment + ordered mean.  st == NULL on the normal path,
+ * else the trace of the two rounds; recording only reads values the loop computes anyway. */
+static void refine_centroids(double best[8][3], int count, const double (*records)[3], int n_records, vgo_gc_coef_pass *st)
 {
     double sums[8][3];
     double m[3][3];
     int hits[8];
     double direct[3];
+    double dist[8];
     memset(m, 0, sizeof m);
 
     for (int round = 0; round < 2; round++) {
@@ -259,8 +295,10 @@ static void refine_centroids(double best[8][3], int count, const double (*record
             double least = 1.0e30;
             for (int c = 0; c < count; c++) {
                 double d = contrast(best[c], records[z]);
+                dist[c] = d;
                 if (d < least) { least = d; pick = c; }
             }
+            if (st && least < 1.0e30) note_tie(&st[round], (const double (*)[3])best, dist, count, least, z);
             hits[pick]++;
             record_to_direct(records[z], direct, m);
             for (int i = 0; i <= 2; i++) sums[pick][i] += direct[i];
@@ -269,23 +307,26 @@ static void refine_centroids(double best[8][3], int count, const double (*record
             if (hits[c] > 0)
                 for (int y = 0; y <= 2; y++) sums[c][y] /= hits[c];
         for (int c = 0; c < count; c++) centroid_from_mean(sums[c], best[c]);
+        if (st) note_pass(&st[round], (const double (*)[3])best, hits, count);
     }
 }
 
-/* One frame of phase 1.  win holds previous+current frame.  Returns 1 and fills rec[0..2] if accepted. */
+/* One frame of phase 1.  win holds previous+current frame.  Returns 0 (VGO_GC_ACCEPTED) and fills rec[0..2] if the
+ * frame gives a record, else the VGO_GC_REJ_* reason it was rejected for. */
 static int frame_record(const int16_t win[28], double rec[3])
 {
     double v[3], m[3][3], scratch[3];
     int perm[3] = {0, 0, 0};
+    int why;
     memset(m, 0, sizeof m);
     autocorr_neg(v, win);
-    if (!(fabs(v[0]) > 10.0)) return 0;
+    if (!(fabs(v[0]) > 10.0)) return VGO_GC_REJ_QUIET;
     covariance(m, win);
-    if (lu_reject(m, perm, scratch)) return 0;
+    if ((why = lu_reject(m, perm, scratch)) != 0) return why;
     lu_solve(m, perm, v);
-    if (to_reflection(v)) return 0;
+    if ((why = to_reflection(v)) != 0) return why;
     finish_record(v, rec);
-    return 1;
+    return VGO_GC_ACCEPTED;
 }
 
 /* short rounding of the final coefficients, GcAdpcmCoefficients.cs:94-108.  Math.Round = half-to-even. */
@@ -299,7 +340,7 @@ static int16_t quantise_coef(double v)
 }
 
 static int collect_records(const int16_t *source, int length, double (*records)[3], double *rec_out,
-                           double *dir_out, uint8_t *accepted_out)
+                           double *dir_out, uint8_t *accepted_out, uint8_t *outcome_out)
 {
     int16_t win[28];
     double m[3][3];
@@ -311,9 +352,11 @@ static int collect_records(const int16_t *source, int length, double (*records)[
         memset(win + 14, 0, 14 * sizeof(int16_t));
         memcpy(win + 14, source + pos, (size_t)take * sizeof(int16_t));
         double rec[3];
-        int ok = frame_record(win, rec);
+        int why = frame_record(win, rec);
+        int ok = why == VGO_GC_ACCEPTED;
         if (ok && records) memcpy(records[n_records], rec, sizeof rec);
         if (accepted_out) accepted_out[frame] = (uint8_t)ok;
+        if (outcome_out) outcome_out[frame] = (uint8_t)why;
         if (rec_out) { rec_out[2 * frame] = ok ? rec[1] : 0.0; rec_out[2 * frame + 1] = ok ? rec[2] : 0.0; }
         if (dir_out) {
             double d[3] = {0.0, 0.0, 0.0};
@@ -329,11 +372,13 @@ static int collect_records(const int16_t *source, int length, double (*records)[
 
 int vgo_gc_coef_records(const int16_t *source, int length, double *rec_out, double *dir_out, uint8_t *accepted_out)
 {
-    return collect_records(source, length, NULL, rec_out, dir_out, accepted_out);
+    return collect_records(source, length, NULL, rec_out, dir_out, accepted_out, NULL);
 }
 
-/* CalculateCoefficients :9-110 */
-void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t coefs_out[16])
+/* CalculateCoefficients :9-110.  trace_out == NULL on the normal path, else the facts of every pass and frame
+ * (vgo_gc_coef_trace); recording only reads values the loops compute anyway, so the arithmetic is the same either way. */
+static void calculate_coefficients(const int16_t *source, int length, int16_t coefs_out[16], vgo_gc_refine_trace *trace_out,
+                                   uint8_t *outcome_out)
 {
     int n_frames = vgo_divide_by_round_up(length, FRAME_SAMPLES);
     double (*records)[3] = malloc(sizeof(double[3]) * (size_t)(n_frames > 0 ? n_frames : 1));
@@ -343,7 +388,7 @@ void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t co
     memset(best, 0, sizeof best);
     memset(m, 0, sizeof m);
 
-    int n_records = collect_records(source, length, records, NULL, NULL, NULL);
+    int n_records = collect_records(source, length, records, NULL, NULL, NULL, outcome_out);
 
     /* ordered mean of the direct-form vectors :63-76 */
     mean[0] = 1.0; mean[1] = 0.0; mean[2] = 0.0;
@@ -353,6 +398,13 @@ void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t co
     }
     for (int y = 1; y <= 2; y++) mean[y] /= n_records; /* 0/0 = NaN when no frame qualified (A.19) */
     centroid_from_mean(mean, best[0]);
+    if (trace_out) {
+        memset(trace_out, 0, sizeof *trace_out);
+        for (int p = 0; p < VGO_GC_COEF_PASSES; p++) trace_out->pass[p].tie_record = trace_out->pass[p].tie_lo = trace_out->pass[p].tie_hi = -1;
+        trace_out->n_frames = n_frames;
+        trace_out->n_records = n_records;
+        note_pass(&trace_out->pass[0], (const double (*)[3])best, &n_records, 1);
+    }
 
     /* three split-and-refine generations: 1 -> 2 -> 4 -> 8 centroids :79-91 */
     int count = 1;
@@ -363,7 +415,8 @@ void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t co
                 best[count + i][y] = (0.01 * nudge[y]) + best[i][y];
         ++gen;
         count = 1 << gen;
-        refine_centroids(best, count, (const double (*)[3])records, n_records);
+        refine_centroids(best, count, (const double (*)[3])records, n_records,
+                         trace_out ? &trace_out->pass[2 * gen - 1] : NULL);
     }
 
     for (int z = 0; z < 8; z++) {
@@ -372,6 +425,19 @@ void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t co
     }
     free(records);
 }
+
+void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t coefs_out[16])
+{
+    calculate_coefficients(source, length, coefs_out, NULL, NULL);
+}
+
+void vgo_gc_coef_trace(const int16_t *source, int length, vgo_gc_refine_trace *trace_out, uint8_t *outcome_out,
+                       int16_t coefs_out[16])
+{
+    calculate_coefficients(source, length, coefs_out, trace_out, outcome_out);
+}
+
+int vgo_gc_refine_trace_size(void) { return (int)sizeof(vgo_gc_refine_trace); }
 
 /* ------------------------------------------------------------------------------------------------
  * Encoder (GcAdpcmEncoder.cs)

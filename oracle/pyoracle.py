@@ -100,6 +100,34 @@ def coef_records(pcm):
     return acc, rec, dire
 
 
+GC_COEF_PASSES = 7
+# phase-1 outcome of a frame (vgoracle.h VGO_GC_ACCEPTED / VGO_GC_REJ_*)
+GC_ACCEPTED, GC_REJ_QUIET, GC_REJ_BIG, GC_REJ_RANGE, GC_REJ_DEN, GC_REJ_K1 = range(6)
+GC_COEF_PASS = np.dtype([("cent", np.float64, (8, 2)), ("hits", np.int32, 8), ("count", np.int32), ("empty", np.int32),
+                         ("ties_same", np.int32), ("ties_distinct", np.int32), ("tie_record", np.int32),
+                         ("tie_lo", np.int32), ("tie_hi", np.int32), ("pad", np.int32)], align=True)
+GC_COEF_TRACE = np.dtype([("pass", GC_COEF_PASS, GC_COEF_PASSES), ("n_frames", np.int32), ("n_records", np.int32)],
+                         align=True)
+
+
+def gc_coef_trace(pcm):
+    """calculate_coefficients() plus the trace of every refinement pass and every frame's phase-1 outcome:
+    (coefs[16] int16, GC_COEF_TRACE record, outcome[frames] uint8)."""
+    L = lib()
+    if not getattr(L, "_coef_trace_ready", False):
+        L.vgo_gc_coef_trace.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.vgo_gc_coef_trace.restype = None
+        if L.vgo_gc_refine_trace_size() != GC_COEF_TRACE.itemsize:
+            raise RuntimeError("vgo_gc_refine_trace layout differs from GC_COEF_TRACE")
+        L._coef_trace_ready = True
+    pcm = np.ascontiguousarray(pcm, dtype=np.int16)
+    co = np.zeros(16, dtype=np.int16)
+    trace = np.zeros((), dtype=GC_COEF_TRACE)
+    outcome = np.zeros((len(pcm) + 13) // 14, dtype=np.uint8)
+    L.vgo_gc_coef_trace(pcm.ctypes.data, len(pcm), trace.ctypes.data, outcome.ctypes.data, co.ctypes.data)
+    return co, trace, outcome
+
+
 def encode(pcm, coefs, sample_count: int = -1, history1: int = 0, history2: int = 0) -> np.ndarray:
     pcm = np.ascontiguousarray(pcm, dtype=np.int16)
     coefs = np.ascontiguousarray(coefs, dtype=np.int16)

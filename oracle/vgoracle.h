@@ -53,6 +53,34 @@ void vgo_gc_calculate_coefficients(const int16_t *source, int length, int16_t co
  * Returns the number of accepted records.  Used to test the GPU phase-1 kernel in isolation. */
 int vgo_gc_coef_records(const int16_t *source, int length, double *rec_out, double *dir_out, uint8_t *accepted_out);
 
+/* CalculateCoefficients with a record of every refinement pass and of every frame's phase-1 outcome, so that tests can
+ * compare a kernel pass by pass and show which rare paths an input reaches.  Same coefficients as
+ * vgo_gc_calculate_coefficients.  Passes are numbered as gc_coef_refine_kernel numbers them: 0 is the ordered mean
+ * (:63-76), 1..6 are split + two FilterRecords rounds with 2, 4 and 8 centroids (:79-91, :344-396). */
+enum { VGO_GC_COEF_PASSES = 7 };
+/* phase-1 outcome of a frame (:40-61, :133-255) */
+enum { VGO_GC_ACCEPTED = 0, VGO_GC_REJ_QUIET = 1 /* |v0| <= 10 */, VGO_GC_REJ_BIG = 2 /* a row max < double.Epsilon */,
+       VGO_GC_REJ_RANGE = 3 /* lo / hi < 1e-10 */, VGO_GC_REJ_DEN = 4 /* 1 - k2^2 == 0 */, VGO_GC_REJ_K1 = 5 /* |k1| > 1 */ };
+typedef struct vgo_gc_coef_pass {
+    double cent[8][2];       /* best[z][1], best[z][2] after the pass, raw doubles (centroids the pass does not use: 0) */
+    int32_t hits[8];         /* records per bucket (pass 0: all records in bucket 0; unused buckets 0) */
+    int32_t count;           /* centroids of the pass: 1, 2, 2, 4, 4, 8, 8 */
+    int32_t empty;           /* buckets below count without a record */
+    int32_t ties_same;       /* records whose minimum distance (< 1e30) is shared by centroids that are all bit-identical */
+    int32_t ties_distinct;   /* ... shared by centroids of which two differ in some bit */
+    int32_t tie_record;      /* the first tied record (record order), -1: none */
+    int32_t tie_lo, tie_hi;  /* its lowest and highest centroid index at the minimum: the record went to tie_lo */
+    int32_t pad;
+} vgo_gc_coef_pass;
+typedef struct vgo_gc_refine_trace {
+    vgo_gc_coef_pass pass[VGO_GC_COEF_PASSES];
+    int32_t n_frames, n_records;
+} vgo_gc_refine_trace;
+/* outcome_out [frames]: VGO_GC_ACCEPTED or the VGO_GC_REJ_* reason; either pointer may be NULL */
+void vgo_gc_coef_trace(const int16_t *source, int length, vgo_gc_refine_trace *trace_out, uint8_t *outcome_out,
+                       int16_t coefs_out[16]);
+int vgo_gc_refine_trace_size(void); /* sizeof(vgo_gc_refine_trace), checked by the Python wrapper */
+
 /* ---- GcAdpcmEncoder (Codecs/GcAdpcm/GcAdpcmEncoder.cs) ---- */
 /* Encode :14-46.  sample_count == -1 means pcm_length.  adpcm_out holds SampleCountToByteCount(sample_count) bytes. */
 void vgo_gc_encode(const int16_t *pcm, int pcm_length, const int16_t coefs[16],

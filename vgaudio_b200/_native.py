@@ -182,6 +182,8 @@ SIGNATURES = {
     "vgb_debug_last_timeline": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_debug_last_coefs_done": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_gcadpcm_debug_records": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vgb_gcadpcm_debug_refine_trace": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p]),
     "vgb_gcadpcm_debug_splice_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_wave_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
     "vgb_wave_read_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),

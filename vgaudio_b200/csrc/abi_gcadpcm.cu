@@ -763,4 +763,48 @@ int32_t vgb_gcadpcm_debug_records(const int16_t *pcm, int32_t n_samples, double 
     return VGB_OK;
 }
 
+int32_t vgb_gcadpcm_debug_refine_trace(const int16_t *const *pcm, const int32_t *n_samples, int32_t n_channels, int32_t warps,
+                                       double *cent_out, int32_t *hits_out, int16_t *coefs_out)
+{
+    if (n_channels < 0 || (warps != 4 && warps != 8) || !cent_out || !hits_out || !coefs_out)
+        return fail(VGB_E_ARG, "bad arguments");
+    if (n_channels == 0) return VGB_OK;
+    if (!pcm) return fail(VGB_E_ARG, "pcm is NULL");
+    GcLayout lay;
+    VGB_TRY(layout_common(lay, n_samples, nullptr, n_channels, false));
+    for (int c = 0; c < n_channels; c++)
+        if (!pcm[c] && lay.n_samples[c] > 0) return fail(VGB_E_ARG, "pcm[%d] is NULL", c);
+    layout_pack_offsets(lay);
+    std::vector<int64_t> pcm_b(n_channels), pcm_len(n_channels);
+    for (int c = 0; c < n_channels; c++) {
+        pcm_b[c] = lay.pcm_off[c] * 2;
+        pcm_len[c] = (int64_t)lay.n_samples[c] * 2;
+    }
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    VGB_TRY(ensure_ready_locked());
+    cudaStream_t st = g_ctx.stream;
+    const GcWorkspace w = carve(lay.rec_total, n_channels);
+    const size_t n = (size_t)n_channels, cent_bytes = n * 7 * 8 * 2 * 8, hits_bytes = n * 7 * 8 * 4;
+    VGB_TRY(g_ctx.pcm.reserve((size_t)lay.pcm_total * 2));
+    VGB_TRY(g_ctx.ws.reserve(w.total));
+    VGB_TRY(g_ctx.coefs.reserve(n * 32));
+    VGB_TRY(g_ctx.misc.reserve(align_up(cent_bytes, 256) + hits_bytes));
+    double *d_cent = reinterpret_cast<double *>(g_ctx.misc.p);
+    int32_t *d_hits = reinterpret_cast<int32_t *>(g_ctx.misc.c() + align_up(cent_bytes, 256));
+    VGB_TRY(copy_units(cudaMemcpyHostToDevice, g_ctx.pcm.c(), pcm_b.data(), pcm, pcm_len.data(), 0, n_channels, st));
+    VGB_TRY(upload_tables(lay, w, g_ctx.ws.p, st));
+    GcChannelTable tab = table_view(g_ctx.ws.p, w, n_channels);
+    double2 *records = reinterpret_cast<double2 *>(g_ctx.ws.c() + w.off_records);
+    uint32_t *mask = reinterpret_cast<uint32_t *>(g_ctx.ws.c() + w.off_mask);
+    launch_gc_coef_frames(static_cast<const int16_t *>(g_ctx.pcm.p), tab, records, mask, lay.max_frames, 0, INT_MAX, st);
+    launch_gc_coef_refine_tap(tab, records, mask, static_cast<int16_t *>(g_ctx.coefs.p), warps, d_cent, d_hits, st);
+    g_ctx.launches += (lay.max_frames > 0 ? 1 : 0) + 1;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(cent_out, d_cent, cent_bytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(hits_out, d_hits, hits_bytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(coefs_out, g_ctx.coefs.p, n * 32, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return VGB_OK;
+}
+
 }  // extern "C"

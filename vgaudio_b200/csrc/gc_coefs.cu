@@ -409,10 +409,13 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
     }
 }
 
-template <int W>
-__global__ void __launch_bounds__(W * 32, W == 4 ? 8 : 3)  // W = 4: 8 CTAs per SM, 1024 channels are resident at once on 132 SMs
-gc_coef_refine_kernel(GcChannelTable tab, const double2 *__restrict__ records, const uint32_t *__restrict__ accept_mask,
-                      int16_t *__restrict__ coefs_out)
+// The refinement of one channel per CTA.  kTap: warp 0 also writes the centroids (c1, c2) and bucket counts every pass
+// leaves to tap_cent [ch][7][8][2] / tap_hits [ch][7][8] (vgb_gcadpcm_debug_refine_trace); the encode path instantiates
+// it with kTap = false, which compiles to the same code as without the tap.
+template <int W, bool kTap>
+__device__ __forceinline__ void gc_coef_refine(GcChannelTable tab, const double2 *__restrict__ records,
+                                               const uint32_t *__restrict__ accept_mask, int16_t *__restrict__ coefs_out,
+                                               double *__restrict__ tap_cent, int32_t *__restrict__ tap_hits)
 {
     extern __shared__ __align__(16) unsigned char refine_smem[];
     RefineShared<W> &sh = *reinterpret_cast<RefineShared<W> *>(refine_smem);
@@ -476,11 +479,33 @@ gc_coef_refine_kernel(GcChannelTable tab, const double2 *__restrict__ records, c
                 best[lane][1] = o1;
                 best[lane][2] = o2;
             }
+            if (kTap && lane < 8) {  // each lane its own centroid: just written above, or untouched by this pass
+                const int64_t at = ((int64_t)ch * 7 + pass) * 8 + lane;
+                tap_cent[2 * at] = best[lane][1];
+                tap_cent[2 * at + 1] = best[lane][2];
+                tap_hits[at] = h;
+            }
         }
         __syncthreads();  // the next pass classifies against the new centroids
     }
 
     if (threadIdx.x < 16) coefs_out[(int64_t)ch * 16 + threadIdx.x] = gc_quantise_coef(best[threadIdx.x >> 1][1 + (threadIdx.x & 1)]);
+}
+
+template <int W>
+__global__ void __launch_bounds__(W * 32, W == 4 ? 8 : 3)  // W = 4: 8 CTAs per SM, 1024 channels are resident at once on 132 SMs
+gc_coef_refine_kernel(GcChannelTable tab, const double2 *__restrict__ records, const uint32_t *__restrict__ accept_mask,
+                      int16_t *__restrict__ coefs_out)
+{
+    gc_coef_refine<W, false>(tab, records, accept_mask, coefs_out, nullptr, nullptr);
+}
+
+template <int W>
+__global__ void __launch_bounds__(W * 32, W == 4 ? 8 : 3)
+gc_coef_refine_tap_kernel(GcChannelTable tab, const double2 *__restrict__ records, const uint32_t *__restrict__ accept_mask,
+                          int16_t *__restrict__ coefs_out, double *__restrict__ tap_cent, int32_t *__restrict__ tap_hits)
+{
+    gc_coef_refine<W, true>(tab, records, accept_mask, coefs_out, tap_cent, tap_hits);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -513,6 +538,21 @@ void launch_gc_coef_refine(const GcChannelTable &tab, const double2 *records, co
         gc_coef_refine_kernel<8><<<tab.n_channels, 8 * 32, sizeof(RefineShared<8>), stream>>>(tab, records, mask, coefs_out);
     else
         gc_coef_refine_kernel<4><<<tab.n_channels, 4 * 32, sizeof(RefineShared<4>), stream>>>(tab, records, mask, coefs_out);
+}
+
+void launch_gc_coef_refine_tap(const GcChannelTable &tab, const double2 *records, const uint32_t *mask, int16_t *coefs_out,
+                               int warps, double *tap_cent, int32_t *tap_hits, cudaStream_t stream)
+{
+    if (tab.n_channels <= 0) return;
+    if (warps == 8) {
+        cudaFuncSetAttribute(gc_coef_refine_tap_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefineShared<8>));
+        gc_coef_refine_tap_kernel<8><<<tab.n_channels, 8 * 32, sizeof(RefineShared<8>), stream>>>(tab, records, mask, coefs_out,
+                                                                                                  tap_cent, tap_hits);
+    } else {
+        cudaFuncSetAttribute(gc_coef_refine_tap_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefineShared<4>));
+        gc_coef_refine_tap_kernel<4><<<tab.n_channels, 4 * 32, sizeof(RefineShared<4>), stream>>>(tab, records, mask, coefs_out,
+                                                                                                  tap_cent, tap_hits);
+    }
 }
 
 }  // namespace vgb

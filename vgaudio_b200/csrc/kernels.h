@@ -13,6 +13,9 @@ void launch_gc_coef_frames(const int16_t *pcm, const GcChannelTable &tab, double
                            int max_frames, int frame_begin, int frame_end, cudaStream_t stream);
 void launch_gc_coef_refine(const GcChannelTable &tab, const double2 *records, const uint32_t *mask,
                            int16_t *coefs_out, cudaStream_t stream);
+// the refinement with a record of every pass (vgb_gcadpcm_debug_refine_trace): warps 4 or 8 picks the CTA width directly
+void launch_gc_coef_refine_tap(const GcChannelTable &tab, const double2 *records, const uint32_t *mask, int16_t *coefs_out,
+                               int warps, double *tap_cent, int32_t *tap_hits, cudaStream_t stream);
 
 // gc_encode.cu — GcAdpcmEncoder.Encode / DspEncodeFrame / DspEncodeCoef (Codecs/GcAdpcm/GcAdpcmEncoder.cs:14-171)
 int gc_encode_pick_segments(int n_channels, int max_frames, int *min_seg_out = nullptr);  // segments per channel (and the shortest segment) for the time-parallel encode
