@@ -41,11 +41,15 @@ def wave_read_batch(files: Sequence) -> List[Tuple[N.VgbWaveInfo, List[np.ndarra
     rtab = (C.c_void_p * max(len(rows), 1))(*[r.ctypes.data for r in rows])
     lens = (C.c_int64 * max(len(arrs), 1))(*[a.size for a in arrs])
     N.check(N.lib.vgb_wave_read_batch(ftab, lens, infos, len(arrs), rtab))
+    return _rows_per_file(infos, rows)
+
+
+def _rows_per_file(infos, rows) -> list:
+    """[(info, the info's channel_count rows)] for file-major channel rows."""
     out, r = [], 0
-    for i in range(len(arrs)):
-        ch = infos[i].channel_count
-        out.append((infos[i], rows[r:r + ch]))
-        r += ch
+    for info in infos:
+        out.append((info, rows[r:r + info.channel_count]))
+        r += info.channel_count
     return out
 
 
@@ -123,12 +127,7 @@ def dsp_read_batch(files: Sequence) -> List[Tuple[N.VgbDspInfo, List[np.ndarray]
     lens = (C.c_int64 * n)(*[a.size for a in arrs])
     rtab = (C.c_void_p * max(len(rows), 1))(*[r.ctypes.data for r in rows])
     N.check(N.lib.vgb_dsp_read_batch(ftab, lens, infos, n, rtab))
-    out, r = [], 0
-    for i in range(n):
-        ch = infos[i].channel_count
-        out.append((infos[i], rows[r:r + ch]))
-        r += ch
-    return out
+    return _rows_per_file(infos, rows)
 
 
 # ---- CRI ADX (Containers/Adx/AdxWriter.cs, Codecs/CriAdx/CriAdxEncryption.cs, CriAdxKey.cs) ----------------------------
@@ -237,32 +236,29 @@ def convert_options(out_type: int, **kw) -> N.VgbConvertOptions:
     return o
 
 
-def convert_wave_batch(files: Sequence, options: N.VgbConvertOptions, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
-    """BatchConvert for WAVE inputs held in memory: ([output file bytes or None], [per-file status])."""
+def _convert(call, files) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """The two passes of a batch converter call: call(ftab, lens, n, sizes, files_out, status) sizes every file with
+    files_out NULL, then writes the files that are good into buffers of those sizes."""
     arrs = [_bytes_arr(f) for f in files]
     n = len(arrs)
     ftab = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in arrs])
     lens = (C.c_int64 * max(n, 1))(*[a.size for a in arrs])
     sizes = (C.c_int64 * max(n, 1))()
     status = (C.c_int32 * max(n, 1))()
-    N.check(N.lib.vgb_convert_wave_batch(ftab, lens, n, C.byref(options), sizes, None, status, None, None))
+    N.check(call(ftab, lens, n, sizes, None, status))
     outs = [np.zeros(sizes[i], dtype=np.uint8) if status[i] == 0 else None for i in range(n)]
     otab = (C.c_void_p * max(n, 1))(*[o.ctypes.data if o is not None else None for o in outs])
-    cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
-    N.check(N.lib.vgb_convert_wave_batch(ftab, lens, n, C.byref(options), sizes, otab, status, cb, None))
+    N.check(call(ftab, lens, n, sizes, otab, status))
     return outs, [int(status[i]) for i in range(n)]
+
+
+def convert_wave_batch(files: Sequence, options: N.VgbConvertOptions, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """BatchConvert for WAVE inputs held in memory: ([output file bytes or None], [per-file status])."""
+    cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
+    return _convert(lambda ftab, lens, n, sizes, otab, status: N.lib.vgb_convert_wave_batch(
+        ftab, lens, n, C.byref(options), sizes, otab, status, cb if otab is not None else None, None), files)
 
 
 def convert_dsp_to_wave_batch(files: Sequence) -> Tuple[List[Optional[np.ndarray]], List[int]]:
     """The decode direction of the batch job: .dsp images in, 16-bit WAVE images out (DspReader -> ToPcm16 -> WaveWriter)."""
-    arrs = [_bytes_arr(f) for f in files]
-    n = len(arrs)
-    ftab = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in arrs])
-    lens = (C.c_int64 * max(n, 1))(*[a.size for a in arrs])
-    sizes = (C.c_int64 * max(n, 1))()
-    status = (C.c_int32 * max(n, 1))()
-    N.check(N.lib.vgb_convert_dsp_to_wave_batch(ftab, lens, n, sizes, None, status))
-    outs = [np.zeros(sizes[i], dtype=np.uint8) if status[i] == 0 else None for i in range(n)]
-    otab = (C.c_void_p * max(n, 1))(*[o.ctypes.data if o is not None else None for o in outs])
-    N.check(N.lib.vgb_convert_dsp_to_wave_batch(ftab, lens, n, sizes, otab, status))
-    return outs, [int(status[i]) for i in range(n)]
+    return _convert(N.lib.vgb_convert_dsp_to_wave_batch, files)

@@ -459,8 +459,8 @@ struct State {
     cudaStream_t s_in = nullptr, s_out = nullptr, s_kern[kWays] = {};
     cudaStream_t s_k = nullptr;  // = s_kern[0]: the stream of the single-shot entry points
     cudaEvent_t ev_in[kWays] = {}, ev_split[kWays] = {}, ev_k[kWays] = {}, ev_out[kWays] = {};
+    // working set 0 doubles as the single-shot entry points' and the .dsp -> WAVE converter's
     DevBuf in[kWays], out[kWays], tab[kWays], pcms[kWays], encs[kWays], decs[kWays], coefss[kWays], wss[kWays];
-    DevBuf &pcm = pcms[0], &enc = encs[0], &coefs = coefss[0];  // working set 0 doubles as the single-shot entry points'
     // stage timers of the batch converter: per group 5 events (start, split done, encode done, context done, assembled)
     static constexpr int kTimedGroups = 32, kStageEvents = 5;
     cudaEvent_t stage[kTimedGroups][kStageEvents] = {};
@@ -703,22 +703,6 @@ int wave_tile_samples(int channels)
 {
     int t = kSplitSmemSamples / channels / 8 * 8;
     return t < 8 ? 0 : t;
-}
-
-// launch helpers ------------------------------------------------------------------------------------------------
-int32_t launch_wave_split(const uint8_t *d_in, std::vector<WaveItem> &items, void *d_items, int16_t *d_pcm, cudaStream_t st)
-{
-    int tiles = 0;
-    for (auto &w : items) { w.tile_first = tiles; tiles += w.samples > 0 ? (w.samples + w.tile_samples - 1) / w.tile_samples : 0; }
-    if (tiles == 0) return VGB_OK;
-    // items without tiles must not be found by the search: drop them
-    std::vector<WaveItem> live;
-    for (auto &w : items) if (w.samples > 0) live.push_back(w);
-    CUDA_TRY(cudaMemcpyAsync(d_items, live.data(), live.size() * sizeof(WaveItem), cudaMemcpyHostToDevice, st));
-    wave_split_kernel<<<tiles, 256, 0, st>>>(d_in, static_cast<const WaveItem *>(d_items), (int)live.size(), d_pcm);
-    vgb::abi_count_launches(1);
-    CUDA_TRY(cudaGetLastError());
-    return VGB_OK;
 }
 
 }  // namespace
