@@ -45,10 +45,12 @@ int32_t vgb_init(int32_t device, uint32_t flags);
 int32_t vgb_shutdown(void);
 /* Bind several devices (SURVEY §8b's vgb_init(n_devices, flags); the reference's counterpart is Parallel.ForEach over
  * files, src/VGAudio.Cli/Batch.cs:24-25).  devices[0] becomes the primary device (the one the *_dev entry points, timers
- * and debug taps use); every host-pointer *_batch call is then sharded over all bound devices by greedy longest-first bin
- * packing of the units' sample counts - one worker thread and one H2D / kernel / D2H pipeline per device, each over its
- * own PCIe link, results written straight into the caller's arrays (no collective: host data reaches a GPU fastest over
- * that GPU's own link).  A device may be listed more than once. */
+ * and debug taps use); every host-pointer codec *_batch call and both batch converters (vgb_convert_wave_batch,
+ * vgb_convert_dsp_to_wave_batch) are then sharded over all bound devices by greedy longest-first bin packing of the
+ * units' sample counts - one worker thread and one H2D / kernel / D2H pipeline per device, each over its own PCIe link,
+ * results written straight into the caller's arrays (no collective: host data reaches a GPU fastest over that GPU's own
+ * link).  The single-shot container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.
+ * A device may be listed more than once. */
 int32_t vgb_init_devices(const int32_t *devices, int32_t n_devices, uint32_t flags);
 int32_t vgb_device_count(void);
 
@@ -484,18 +486,24 @@ typedef struct vgb_convert_options {
     int64_t group_bytes;                /* input bytes per GPU batch; 0 = an eighth of the job, 64..512 MiB */
 } vgb_convert_options;
 /* Pass files_out == NULL for the sizing pass: out_sizes[i] = size of output i (0 for a file that failed), status_out[i]
- * (may be NULL) = VGB_OK or the error of file i - a bad file does not stop the batch (Batch.cs:39-43).  The second pass
- * fills files_out[i] for every file whose status is VGB_OK.  cb receives the number of files finished. */
+ * (may be NULL) = VGB_OK or the error of file i - a bad file does not stop the batch (Batch.cs:39-43).  The sizing pass
+ * runs on the host only and needs no device.  The second pass fills files_out[i] for every file whose status is VGB_OK.
+ * cb receives the number of files finished (positive deltas summing to the good files).  With several devices bound
+ * (vgb_init_devices) and at least two good files, the second pass is sharded: files weigh sample_count * channel_count
+ * + 1024, every device converts its share in groups of its own (group_bytes = 0: an eighth of its share's input, 64..512
+ * MiB), and an error of a device's share fails the call with " (device N)" appended to its message. */
 int32_t vgb_convert_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_convert_options *options,
                                int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
 /* The decode direction of the batch job: .dsp file images in, 16-bit WAVE file images out - DspReader (Containers/Dsp/DspReader.cs:15-127)
  * -> GcAdpcmFormat.ToPcm16 (GcAdpcmFormat.cs:42-54, from the header's coefficients and start history) -> WaveWriter
  * (Containers/Wave/WaveWriter.cs:52-132: RIFF / fmt (extensible above two channels) / smpl when looping / data).  Same two-pass
- * protocol and per-file status as vgb_convert_wave_batch. */
+ * protocol, per-file status and sharding over several devices as vgb_convert_wave_batch (files weigh their decoded
+ * samples).  A frame header that selects a predictor outside 0..7 fails the whole call (VGB_E_DATA). */
 int32_t vgb_convert_dsp_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, int64_t *out_sizes,
                                       uint8_t *const *files_out, int32_t *status_out);
-/* Measurement tap: device time of the most recent vgb_convert_wave_batch summed over its (first 32) batches, out[0..3] =
- * WAVE split, encode, loop-context decode, file assembly (ms, CUDA events on the kernel stream); returns the batches timed. */
+/* Measurement tap: device time of the most recent vgb_convert_wave_batch summed over its (first 32) batches per device,
+ * over every device that converted part of it, out[0..3] = WAVE split, encode, loop-context decode, file assembly (ms,
+ * CUDA events on the kernel streams); returns the number of batches timed on all devices together. */
 int32_t vgb_convert_debug_stage_ms(float *out, int32_t n);
 
 #ifdef __cplusplus

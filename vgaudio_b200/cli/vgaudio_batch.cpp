@@ -7,7 +7,10 @@
 //
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--adxtype Linear|Fixed|Exp|ExpEnc...]
-//                 [--framesize N] [--version 3|4] [--chunk-mb N]
+//                 [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
+//
+// --devices 0,1,2,3 binds those CUDA devices (vgb_init_devices): every chunk of files is then sharded over them, one
+// worker and one copy / kernel pipeline per device.  A device may be listed more than once.  The default is device 0.
 #include <sys/stat.h>
 
 #include <algorithm>
@@ -39,8 +42,24 @@ static int usage()
 {
     std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4]\n"
-                         "                     [--chunk-mb N]\n");
+                         "                     [--chunk-mb N] [--devices LIST]\n");
     return 2;
+}
+
+// "0,1,3": comma-separated CUDA ordinals, at least one, repeats allowed
+static bool parse_devices(const std::string &list, std::vector<int32_t> &out)
+{
+    out.clear();
+    size_t at = 0;
+    while (true) {
+        const size_t end = std::min(list.find(',', at), list.size());
+        const std::string item = list.substr(at, end - at);
+        if (item.empty() || item.size() > 4 || item.find_first_not_of("0123456789") != std::string::npos) return false;
+        out.push_back((int32_t)std::atoi(item.c_str()));
+        if (end == list.size()) break;
+        at = end + 1;
+    }
+    return out.size() <= 64;  // vgb_init_devices' limit
 }
 
 int main(int argc, char **argv)
@@ -49,6 +68,7 @@ int main(int argc, char **argv)
     bool recurse = false, have_code = false;
     uint64_t key_code = 0;
     size_t chunk_mb = 1024;
+    std::vector<int32_t> devices;  // empty: device 0 through vgb_init
     vgb_convert_options opt{};
     opt.hca_key_type = -1;
     for (int i = 1; i < argc; i++) {
@@ -66,6 +86,7 @@ int main(int argc, char **argv)
         else if (a == "--framesize") opt.adx_frame_size = std::atoi(next());
         else if (a == "--version") opt.adx_version = std::atoi(next());
         else if (a == "--chunk-mb") chunk_mb = (size_t)std::atoll(next());
+        else if (a == "--devices") { if (!parse_devices(next(), devices)) return usage(); }
         else if (a == "--hcaquality") {
             const std::string q = next();
             const char *names[] = {"", "highest", "high", "middle", "low", "lowest"};
@@ -104,7 +125,8 @@ int main(int argc, char **argv)
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
     if (ec) { std::fprintf(stderr, "cannot read %s: %s\n", in_dir.c_str(), ec.message().c_str()); return 1; }
     std::sort(files.begin(), files.end());
-    if (vgb_init(0, 0) != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
+    const int32_t bound = devices.empty() ? vgb_init(0, 0) : vgb_init_devices(devices.data(), (int32_t)devices.size(), 0);
+    if (bound != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
 
     const auto t0 = std::chrono::steady_clock::now();
     size_t done = 0, failed = 0;

@@ -78,6 +78,8 @@ constexpr int kTimers = 10;  // 0 coef phase 1, 1 coef refine, 2 gc encode, 3 gc
 constexpr int kMaxGroups = 16;   // channel groups of one host call, pipelined: H2D(g+1) || kernels(g) || D2H(g-1)
 constexpr int kCompStreams = 4;  // kernel streams the groups rotate over
 
+struct ContainerState;  // containers.cu: the container layer's streams, events and working sets on one device
+
 // One upload of the HCA codec tables per device
 struct HcaTableStore {
     bool ready = false;
@@ -102,6 +104,7 @@ struct Context {
     std::atomic<int64_t> launches{0};
     GcSegArgs last_seg{};            // bookkeeping of the most recent encode launch (vgb_gcadpcm_debug_splice_stats)
     HcaTableStore hca_tables;
+    std::atomic<ContainerState *> containers{nullptr};  // created on first use, released by containers_release
 };
 
 extern Context g_primary;                               // the device vgb_init / vgb_init_devices binds first
@@ -113,10 +116,10 @@ int32_t ensure_ready_locked();
 void hca_tables_release_locked();  // abi_hca.cu
 void tick(int slot, bool begin, cudaStream_t stream);
 
-// hooks of containers.cu, which keeps its own slabs and streams on the primary device
-int32_t abi_ensure_ready();     // binds / selects the primary device
-void abi_count_launches(int n); // vgb_kernel_launch_count bookkeeping
-void containers_release();      // vgb_shutdown
+// hooks of containers.cu, which keeps its own slabs and streams per context (Context::containers)
+int32_t abi_ensure_ready();              // readies the calling thread's context and makes its device current
+void abi_count_launches(int n);          // vgb_kernel_launch_count bookkeeping of the calling thread's context
+void containers_release(Context &ctx);   // vgb_shutdown: drains and frees ctx's container state
 
 // ---- pinning and copies ----------------------------------------------------------------------------------------
 // Pageable caller buffers (a C# short[] pinned by the GC is still pageable for CUDA) move through the driver's staging
@@ -167,9 +170,13 @@ int32_t copy_units(cudaMemcpyKind kind, char *d_base, const int64_t *d_off, T *c
     bool same = true;
     for (int c = 1; c < count; c++) same = same && bytes[c] == bytes[0];
     int64_t hstride = 0;
-    if (same && count > 1 && bytes[0] > 0 && uniform_stride(h_ptr, count, hstride) && hstride >= bytes[0]) {  // overlapping rows: per-channel copies
+    // a strided copy takes pitches below 2 GiB (cudaDevAttrMaxPitch); two separate caller arrays always look uniform, and
+    // may lie further apart than that
+    constexpr int64_t kMaxPitch = INT32_MAX;
+    if (same && count > 1 && bytes[0] > 0 && uniform_stride(h_ptr, count, hstride) && hstride >= bytes[0] &&  // overlapping rows: per-channel copies
+        hstride <= kMaxPitch) {
         const int64_t dstride = d_off[1] - d_off[0];
-        bool dsame = true;
+        bool dsame = dstride > 0 && dstride <= kMaxPitch;
         for (int c = 2; c < count; c++) dsame = dsame && (d_off[c] - d_off[c - 1] == dstride);
         if (dsame) {
             char *d = d_base + d_off[0];
@@ -292,9 +299,11 @@ struct SharedProgress {  // IProgressReport.ReportAdd from several worker thread
 };
 
 // fn(device index, units) runs on a worker thread bound to that device's context; the first failure wins and its
-// message is re-addressed from the shard-local unit index to the caller's.
+// message gets " (device N)" appended.  With `readdress`, a message that starts with "channel N" / "stream N" is also
+// re-addressed from the shard-local unit index to the caller's; callers whose messages already name the caller's
+// indices, or whose channel / stream numbers are not shard units, pass false.
 template <class Fn>
-int32_t run_sharded(const std::vector<std::vector<int>> &shards, Fn fn)
+int32_t run_sharded(const std::vector<std::vector<int>> &shards, Fn fn, bool readdress = true)
 {
     std::vector<Context *> ctxs{&g_primary};
     for (auto &c : g_extra) ctxs.push_back(c.get());
@@ -315,6 +324,7 @@ int32_t run_sharded(const std::vector<std::vector<int>> &shards, Fn fn)
         if (rc[d] != VGB_OK) {
             std::string m = err[d];
             for (const char *word : {"channel ", "stream "}) {
+                if (!readdress) break;
                 const size_t len = std::strlen(word);
                 if (m.compare(0, len, word) == 0) {
                     size_t end = len;

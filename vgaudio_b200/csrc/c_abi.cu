@@ -7,6 +7,7 @@
 // launch count, timers, debug taps, interleave); abi_gcadpcm.cu, abi_adx.cu and abi_hca.cu hold the codecs.
 #include <cstdarg>
 #include <cstdio>
+#include <map>
 
 #include "abi.cuh"
 
@@ -142,6 +143,21 @@ std::vector<int> pipeline_bounds(const std::vector<int64_t> &weight, int n_group
     return bound;
 }
 
+cudaError_t raise_dynamic_smem(const void *kernel, size_t bytes)
+{
+    static std::mutex mu;
+    static std::map<std::pair<const void *, int>, size_t> raised;  // (kernel, device) -> the attribute's value
+    int device = 0;
+    cudaError_t e = cudaGetDevice(&device);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t &now = raised[{kernel, device}];
+    if (now >= bytes) return cudaSuccess;
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) now = bytes;
+    return e;
+}
+
 bool sharding_active(int n_units) { return !g_extra.empty() && n_units >= 2 && t_ctx == &g_primary; }
 
 }  // namespace vgb
@@ -206,7 +222,9 @@ static int32_t shutdown_current(void)  // releases the context this thread point
 
 int32_t vgb_shutdown(void)
 {
-    vgb::containers_release();  // containers.cu keeps its own slabs and streams on the primary device
+    // containers.cu keeps its own slabs and streams per context: those go first, while the context's device is bound
+    vgb::containers_release(g_primary);
+    for (auto &c : g_extra) vgb::containers_release(*c);
     for (auto &c : g_extra) {
         t_ctx = c.get();
         shutdown_current();
@@ -219,26 +237,22 @@ int32_t vgb_shutdown(void)
 }  // extern "C"
 
 namespace vgb {  // hooks for containers.cu
-int32_t abi_ensure_ready()
+int32_t abi_ensure_ready()  // the primary's context on a caller thread, a worker's own in a sharded converter call
 {
-    Context &c = g_primary;
-    std::lock_guard<std::mutex> lock(c.mu);
-    Context *saved = t_ctx;
-    t_ctx = &c;
-    const int32_t s = ensure_ready_locked();
-    t_ctx = saved;
-    return s;
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    return ensure_ready_locked();
 }
-void abi_count_launches(int n) { g_primary.launches += n; }
+void abi_count_launches(int n) { g_ctx.launches += n; }
 }  // namespace vgb
 
 extern "C" {
 
 /* Bind several devices (SURVEY §8b: vgb_init(n_devices, flags)).  devices[0] becomes the primary device - the one the
- * *_dev entry points, the timers and the debug taps refer to; every host-pointer *_batch call is then sharded over all
- * of them (greedy longest-first over the units' sample counts, one worker thread and one H2D / kernel / D2H pipeline per
- * device, results written straight into the caller's arrays).  A device may be listed more than once (two pipelines on
- * one GPU; also how the sharding logic is tested on a single-GPU machine). */
+ * *_dev entry points, the timers and the debug taps refer to; every host-pointer codec *_batch call and both batch
+ * converters are then sharded over all of them (greedy longest-first over the units' sample counts, one worker thread and
+ * one H2D / kernel / D2H pipeline per device, results written straight into the caller's arrays).  The single-shot
+ * container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.  A device may be listed
+ * more than once (two pipelines on one GPU; also how the sharding logic is tested on a single-GPU machine). */
 int32_t vgb_init_devices(const int32_t *devices, int32_t n_devices, uint32_t flags)
 {
     (void)flags;

@@ -449,11 +449,17 @@ __global__ void __launch_bounds__(kHcaFramesPerTile * 32) hca_assemble_kernel(co
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// host state of this translation unit: its own slabs and streams on the library's primary device
+// host state of this translation unit: its own slabs and streams per context (Context::containers), so a converter call
+// sharded over several devices gives every worker its own on that worker's device
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kWays = 4;  // groups of the batch converter in flight: each has its own working set and kernel stream
 
-struct State {
+}  // namespace
+
+namespace vgb {
+// Created on the context's device, used and freed with that device current.  Lock order: ContainerState::mu before
+// Context::mu (the *_dev codec calls a converter group makes take the latter).
+struct ContainerState {
     std::mutex mu;
     bool ready = false;
     cudaStream_t s_in = nullptr, s_out = nullptr, s_kern[kWays] = {};
@@ -466,8 +472,30 @@ struct State {
     cudaEvent_t stage[kTimedGroups][kStageEvents] = {};
     int timed_groups = 0;
 };
-State g_st;
+}  // namespace vgb
 
+namespace {
+
+using State = vgb::ContainerState;
+
+State &state_of(Context &c)
+{
+    State *s = c.containers.load(std::memory_order_acquire);
+    if (s) return *s;
+    std::lock_guard<std::mutex> lock(c.mu);  // the only place that takes Context::mu before a State exists
+    s = c.containers.load(std::memory_order_relaxed);
+    if (!s) {
+        s = new State();
+        c.containers.store(s, std::memory_order_release);
+    }
+    return *s;
+}
+
+// the container state of the context this thread works on: the primary's on a caller thread, a worker's own in a
+// sharded converter call (as g_ctx is for the codec calls)
+#define g_st (state_of(g_ctx))
+
+// readies g_ctx, makes its device current and creates the state's streams and events there; g_st.mu is held
 int32_t ensure_state()
 {
     VGB_TRY(vgb::abi_ensure_ready());
@@ -487,15 +515,17 @@ int32_t ensure_state()
     return VGB_OK;
 }
 
-struct Drain {  // no copy may be in flight on caller memory once an entry point returns
-    ~Drain()
-    {
-        if (!g_st.ready) return;
-        cudaStreamSynchronize(g_st.s_in);
-        for (auto st : g_st.s_kern) cudaStreamSynchronize(st);
-        cudaStreamSynchronize(g_st.s_out);
-        (void)cudaGetLastError();
-    }
+void drain_state(State &s)  // with s's device current
+{
+    if (!s.ready) return;
+    cudaStreamSynchronize(s.s_in);
+    for (auto st : s.s_kern) cudaStreamSynchronize(st);
+    cudaStreamSynchronize(s.s_out);
+    (void)cudaGetLastError();
+}
+
+struct Drain {  // no copy may be in flight on caller memory once an entry point (or a converter worker) returns
+    ~Drain() { drain_state(g_st); }
 };
 
 void be16(uint8_t *p, int v) { p[0] = (uint8_t)(v >> 8); p[1] = (uint8_t)v; }
@@ -708,24 +738,28 @@ int wave_tile_samples(int channels)
 }  // namespace
 
 namespace vgb {
-void containers_release()  // vgb_shutdown
+void containers_release(Context &c)  // vgb_shutdown, once per bound context
 {
-    std::lock_guard<std::mutex> lock(g_st.mu);
-    if (!g_st.ready) return;
-    cudaStreamSynchronize(g_st.s_in);
-    for (auto st : g_st.s_kern) cudaStreamSynchronize(st);
-    cudaStreamSynchronize(g_st.s_out);
-    for (int i = 0; i < kWays; i++) {
-        g_st.in[i].release(); g_st.out[i].release(); g_st.tab[i].release();
-        g_st.pcms[i].release(); g_st.encs[i].release(); g_st.decs[i].release(); g_st.coefss[i].release(); g_st.wss[i].release();
-        cudaEventDestroy(g_st.ev_in[i]); cudaEventDestroy(g_st.ev_split[i]); cudaEventDestroy(g_st.ev_k[i]); cudaEventDestroy(g_st.ev_out[i]);
-        cudaStreamDestroy(g_st.s_kern[i]);
+    State *s = c.containers.load(std::memory_order_acquire);
+    if (!s) return;
+    {
+        std::lock_guard<std::mutex> lock(s->mu);
+        if (s->ready) {
+            cudaSetDevice(c.device);  // every stream, event and slab of the state lives on c's device
+            drain_state(*s);
+            for (int i = 0; i < kWays; i++) {
+                s->in[i].release(); s->out[i].release(); s->tab[i].release();
+                s->pcms[i].release(); s->encs[i].release(); s->decs[i].release(); s->coefss[i].release(); s->wss[i].release();
+                cudaEventDestroy(s->ev_in[i]); cudaEventDestroy(s->ev_split[i]); cudaEventDestroy(s->ev_k[i]); cudaEventDestroy(s->ev_out[i]);
+                cudaStreamDestroy(s->s_kern[i]);
+            }
+            cudaStreamDestroy(s->s_in); cudaStreamDestroy(s->s_out);
+            for (auto &grp : s->stage) for (auto &e : grp) { if (e) cudaEventDestroy(e); e = nullptr; }
+            (void)cudaGetLastError();
+        }
     }
-    cudaStreamDestroy(g_st.s_in); cudaStreamDestroy(g_st.s_out);
-    for (auto &grp : g_st.stage) for (auto &e : grp) { if (e) cudaEventDestroy(e); e = nullptr; }
-    g_st.timed_groups = 0;
-    g_st.ready = false;
-    (void)cudaGetLastError();
+    c.containers.store(nullptr, std::memory_order_release);
+    delete s;
 }
 }  // namespace vgb
 

@@ -531,13 +531,14 @@ void launch_gc_coef_refine(const GcChannelTable &tab, const double2 *records, co
     if (wide_limit < 0) {
         wide_limit = 0;
         if (const char *env = std::getenv("VGB_REFINE_WIDE_LIMIT")) wide_limit = std::atoi(env);  // tuning knob
-        cudaFuncSetAttribute(gc_coef_refine_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefineShared<8>));
-        cudaFuncSetAttribute(gc_coef_refine_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefineShared<4>));
     }
-    if (tab.n_channels <= wide_limit)
+    if (tab.n_channels <= wide_limit) {
+        raise_dynamic_smem(gc_coef_refine_kernel<8>, sizeof(RefineShared<8>));
         gc_coef_refine_kernel<8><<<tab.n_channels, 8 * 32, sizeof(RefineShared<8>), stream>>>(tab, records, mask, coefs_out);
-    else
+    } else {
+        raise_dynamic_smem(gc_coef_refine_kernel<4>, sizeof(RefineShared<4>));
         gc_coef_refine_kernel<4><<<tab.n_channels, 4 * 32, sizeof(RefineShared<4>), stream>>>(tab, records, mask, coefs_out);
+    }
 }
 
 void launch_gc_coef_refine_tap(const GcChannelTable &tab, const double2 *records, const uint32_t *mask, int16_t *coefs_out,
@@ -545,11 +546,11 @@ void launch_gc_coef_refine_tap(const GcChannelTable &tab, const double2 *records
 {
     if (tab.n_channels <= 0) return;
     if (warps == 8) {
-        cudaFuncSetAttribute(gc_coef_refine_tap_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefineShared<8>));
+        raise_dynamic_smem(gc_coef_refine_tap_kernel<8>, sizeof(RefineShared<8>));
         gc_coef_refine_tap_kernel<8><<<tab.n_channels, 8 * 32, sizeof(RefineShared<8>), stream>>>(tab, records, mask, coefs_out,
                                                                                                   tap_cent, tap_hits);
     } else {
-        cudaFuncSetAttribute(gc_coef_refine_tap_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RefineShared<4>));
+        raise_dynamic_smem(gc_coef_refine_tap_kernel<4>, sizeof(RefineShared<4>));
         gc_coef_refine_tap_kernel<4><<<tab.n_channels, 4 * 32, sizeof(RefineShared<4>), stream>>>(tab, records, mask, coefs_out,
                                                                                                   tap_cent, tap_hits);
     }

@@ -1064,7 +1064,7 @@ cudaError_t launch_hca_decode(const uint8_t *frames, const HcaStream *streams, i
 {
     if (n_streams <= 0 || max_frames <= 0 || total_frames <= 0) return cudaSuccess;
     const size_t smem_p = (size_t)cfg.channel_count * kBins * kParseThreads;
-    cudaError_t e = cudaFuncSetAttribute(hca_decode_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_p);
+    cudaError_t e = raise_dynamic_smem(hca_decode_parse_kernel, smem_p);
     if (e != cudaSuccess) return e;
     const unsigned blocks_p = (unsigned)((total_frames + kParseThreads - 1) / kParseThreads);
     hca_decode_parse_kernel<<<blocks_p, kParseThreads, smem_p, stream>>>(frames, streams, n_streams, total_frames, cfg, tables,
@@ -1072,7 +1072,7 @@ cudaError_t launch_hca_decode(const uint8_t *frames, const HcaStream *streams, i
     e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     const size_t smem = hca_decode_smem_bytes(cfg);
-    e = cudaFuncSetAttribute(hca_decode_unpack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    e = raise_dynamic_smem(hca_decode_unpack_kernel, smem);
     if (e != cudaSuccess) return e;
     dim3 grid_a((unsigned)max_frames, (unsigned)n_streams);
     hca_decode_unpack_kernel<<<grid_a, 128, smem, stream>>>(parsed_scratch, streams, cfg, tables, edge_scratch, pcm);
@@ -1096,7 +1096,7 @@ cudaError_t launch_hca_encode(const int16_t *pcm, const HcaStream *streams, int 
 {
     if (n_streams <= 0 || max_frames <= 0) return cudaSuccess;
     const size_t smem = hca_encode_smem_bytes(cfg);
-    cudaError_t e = cudaFuncSetAttribute(hca_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = raise_dynamic_smem(hca_encode_kernel, smem);
     if (e != cudaSuccess) return e;
     dim3 grid((unsigned)max_frames, (unsigned)n_streams);
     hca_encode_kernel<<<grid, 128, smem, stream>>>(pcm, streams, cfg, tables, frames_out, status_out);

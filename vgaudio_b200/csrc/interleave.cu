@@ -222,8 +222,7 @@ cudaError_t launch_tma(const void *in, void *out, int64_t planar_channel_stride,
     if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
     const size_t smem = (size_t)kBulkStages * kBulkChunk;
     auto kern = interleave_tma_kernel<kDe>;
-    static bool attr_set[2] = {false, false};
-    if (!attr_set[kDe]) { cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); attr_set[kDe] = true; }
+    raise_dynamic_smem(kern, smem);
     const int64_t cpb = (sh.interleave + kBulkChunk - 1) / kBulkChunk;
     const int64_t total = sh.blocks_to_copy * sh.count * cpb * n_items;
     const int grid = (int)std::min<int64_t>(total, (int64_t)sms * 6);

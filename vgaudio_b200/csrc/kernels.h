@@ -8,6 +8,14 @@
 
 namespace vgb {
 
+// c_abi.cu — raises cudaFuncAttributeMaxDynamicSharedMemorySize of `kernel` on the current device to `bytes` when it is
+// lower; never lowers it.  The attribute belongs to the kernel on a device, not to the calling thread: every bound device
+// needs it, and two threads launching one kernel on one device with different sizes (a device bound twice) must not
+// lower it under each other's launch.
+cudaError_t raise_dynamic_smem(const void *kernel, size_t bytes);
+template <class Kernel>
+cudaError_t raise_dynamic_smem(Kernel *kernel, size_t bytes) { return raise_dynamic_smem(reinterpret_cast<const void *>(kernel), bytes); }
+
 // gc_coefs.cu — GcAdpcmCoefficients.CalculateCoefficients (Codecs/GcAdpcm/GcAdpcmCoefficients.cs:9-110)
 void launch_gc_coef_frames(const int16_t *pcm, const GcChannelTable &tab, double2 *records, uint32_t *mask,
                            int max_frames, int frame_begin, int frame_end, cudaStream_t stream);
