@@ -355,6 +355,58 @@ def hca_unpack_ok(info, frames) -> bool:
     return bool(lib().vgo_hca_unpack_ok(C.byref(info), frames.ctypes.data))
 
 
+# per-frame records of vgo_hca_encode_trace / vgo_hca_decode_trace (vgoracle.h)
+HCA_IS_SILENT, HCA_IS_ET_ZERO, HCA_IS_CLAMP_LOW, HCA_IS_CLAMP_HIGH = 1, 2, 4, 8
+HCA_HFR_AVG_ZERO, HCA_HFR_AVG_NAN = 1, 2
+HCA_UNPACK_OK, HCA_UNPACK_BAD_SYNC, HCA_UNPACK_BAD_DELTA, HCA_UNPACK_INTENSITY_15 = range(4)
+HCA_FRAME_TRACE = np.dtype([("noise_level", np.int32), ("eval_boundary", np.int32), ("drop_rounds", np.int32),
+                            ("status", np.int32), ("delta_bits", np.int32, 8), ("escapes", np.int32, 8),
+                            ("coded", np.int32, 8), ("res_hist", np.int32, 16), ("clamped", np.int32),
+                            ("sf_zero", np.int32), ("sf_max", np.int32), ("intensity", np.int8, (8, 8)),
+                            ("is_flags", np.uint8, (8, 8)), ("hfr_flags", np.uint8, (8, 8)),
+                            ("hfr_scale", np.int8, (8, 8))], align=True)
+HCA_DFRAME_TRACE = np.dtype([("unpack", np.int32), ("delta_bits", np.int32, 8), ("hfr_index_min", np.int32),
+                             ("hfr_index_max", np.int32), ("pcm_in_range", np.int32), ("pcm_clip_high", np.int32),
+                             ("pcm_clip_low", np.int32), ("pcm_out_of_int32", np.int32)], align=True)
+
+
+def _hca_trace_lib():
+    L = lib()
+    if not getattr(L, "_hca_trace_ready", False):
+        L.vgo_hca_encode_trace.argtypes = [C.c_void_p] * 5
+        L.vgo_hca_decode_trace.argtypes = [C.c_void_p] * 4
+        if L.vgo_hca_frame_trace_size() != HCA_FRAME_TRACE.itemsize:
+            raise RuntimeError("vgo_hca_frame_trace layout differs from HCA_FRAME_TRACE")
+        if L.vgo_hca_decode_trace_size() != HCA_DFRAME_TRACE.itemsize:
+            raise RuntimeError("vgo_hca_dframe_trace layout differs from HCA_DFRAME_TRACE")
+        L._hca_trace_ready = True
+    return L
+
+
+def hca_encode_trace(channels, sample_rate=48000, quality=2, bitrate=0, limit_bitrate=False):
+    """hca_encode() plus one HCA_FRAME_TRACE record per frame, without raising on a failing stream:
+    (status, HcaInfo, frames[frame_count, frame_size], trace[frame_count]); status is vgo_hca_encode's return value."""
+    L = _hca_trace_lib()
+    arrs, tab = _chan_table(channels)
+    p = hca_params(arrs, sample_rate, quality, bitrate, limit_bitrate)
+    info = hca_init(p)
+    frames = np.zeros((info.frame_count, info.frame_size), dtype=np.uint8)
+    trace = np.zeros(info.frame_count, dtype=HCA_FRAME_TRACE)
+    rc = L.vgo_hca_encode_trace(tab, C.byref(p), C.byref(info), frames.ctypes.data, trace.ctypes.data)
+    return rc, info, frames, trace
+
+
+def hca_decode_trace(info: HcaInfo, frames):
+    """hca_decode() plus one HCA_DFRAME_TRACE record per frame: (pcm[channels, samples], trace[frame_count])."""
+    L = _hca_trace_lib()
+    frames = np.ascontiguousarray(frames, dtype=np.uint8)
+    out = np.zeros((info.channel_count, info.sample_count), dtype=np.int16)
+    tab = (C.c_void_p * info.channel_count)(*[out[c].ctypes.data for c in range(info.channel_count)])
+    trace = np.zeros(info.frame_count, dtype=HCA_DFRAME_TRACE)
+    L.vgo_hca_decode_trace(C.byref(info), frames.ctypes.data, tab, trace.ctypes.data)
+    return out, trace
+
+
 def hca_mdct(blocks: np.ndarray) -> np.ndarray:
     blocks = np.ascontiguousarray(blocks, dtype=np.float64).reshape(-1, 128)
     out = np.zeros_like(blocks)

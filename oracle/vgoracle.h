@@ -165,6 +165,43 @@ int vgo_hca_encode_ath(const int16_t *const *pcm, const vgo_hca_params *p, vgo_h
 int vgo_hca_spectra(const int16_t *const *pcm, const vgo_hca_params *p, double *spectra_out);
 int vgo_hca_decode(const vgo_hca_info *h, const uint8_t *frames, int16_t *const *pcm_out); /* CriHcaDecoder.Decode :11-25 */
 int vgo_hca_unpack_ok(const vgo_hca_info *h, const uint8_t *frames);             /* test helper: all frames well-formed */
+
+/* Encode with one record per frame of the facts of EncodeFrame's rare paths, so that tests can show which of them an
+ * input reaches.  Same return value and frame bytes as vgo_hca_encode; recording only reads values the stages compute
+ * anyway.  Frames after a failing one are not encoded (their records stay zero). */
+enum { VGO_HCA_IS_SILENT = 1 /* el == er == 0 */, VGO_HCA_IS_ET_ZERO = 2 /* et == 0 (anti-phase pair) */,
+       VGO_HCA_IS_CLAMP_LOW = 4 /* ratio < 0.5 */, VGO_HCA_IS_CLAMP_HIGH = 8 /* ratio > sqrt(2)/2 (or +inf) */ };
+enum { VGO_HCA_HFR_AVG_ZERO = 1 /* source average == 0 */, VGO_HCA_HFR_AVG_NAN = 2 /* no source band: 0/0 */ };
+typedef struct vgo_hca_frame_trace {
+    int32_t noise_level, eval_boundary;
+    int32_t drop_rounds;        /* `highest -= 2` rounds of CalculateNoiseLevel (:457-485) */
+    int32_t status;             /* EncodeFrame's outcome: 0, -2 "Bitrate is set too low.", -3 other failure */
+    int32_t delta_bits[8];      /* per channel, as written */
+    int32_t escapes[8];         /* per channel: deltas written as escape + raw value */
+    int32_t coded[8];           /* per channel: CodedScaleFactorCount */
+    int32_t res_hist[16];       /* coded bands of every channel per resolution */
+    int32_t clamped;            /* scaled coefficients clamped to +-0.999999999999 (ScaleSpectra :651-671) */
+    int32_t sf_zero, sf_max;    /* coded bands with scale factor 0 / 63, after band dropping */
+    int8_t intensity[8][8];     /* [channel][subframe]: index written for a stereo secondary, else -1 */
+    uint8_t is_flags[8][8];     /* [secondary channel][subframe]: VGO_HCA_IS_* */
+    uint8_t hfr_flags[8][8];    /* [channel][group]: VGO_HCA_HFR_* of CalculateHfrScale's source average */
+    int8_t hfr_scale[8][8];     /* [channel][group]: scale written, -1 where none */
+} vgo_hca_frame_trace;
+int vgo_hca_encode_trace(const int16_t *const *pcm, const vgo_hca_params *p, vgo_hca_info *info_out, uint8_t *frames_out,
+                         vgo_hca_frame_trace *trace_out);
+int vgo_hca_frame_trace_size(void); /* sizeof(vgo_hca_frame_trace), checked by the Python wrapper */
+
+/* Decode with one record per frame.  A frame that does not unpack the way the reference's happy path does is recorded
+ * and not decoded further (its PCM counts stay zero); vgo_hca_decode's PCM is unchanged for every other frame. */
+enum { VGO_HCA_UNPACK_OK = 0, VGO_HCA_UNPACK_BAD_SYNC = 1, VGO_HCA_UNPACK_BAD_DELTA = 2, VGO_HCA_UNPACK_INTENSITY_15 = 3 };
+typedef struct vgo_hca_dframe_trace {
+    int32_t unpack;                 /* VGO_HCA_UNPACK_* */
+    int32_t delta_bits[8];          /* per channel, as read (-1 past the channel count or an early stop) */
+    int32_t hfr_index_min, hfr_index_max; /* ScaleConversion index of ReconstructHighFrequency; -1 if none */
+    int32_t pcm_in_range, pcm_clip_high, pcm_clip_low, pcm_out_of_int32; /* PcmFloatToShort outcomes */
+} vgo_hca_dframe_trace;
+int vgo_hca_decode_trace(const vgo_hca_info *h, const uint8_t *frames, int16_t *const *pcm_out, vgo_hca_dframe_trace *trace_out);
+int vgo_hca_decode_trace_size(void); /* sizeof(vgo_hca_dframe_trace) */
 void vgo_hca_mdct_run(const double *blocks, int n, double *spectra_out);         /* Mdct.RunMdct :63-92, state from zero */
 void vgo_hca_imdct_run(const double *spectra, int n, double *blocks_out);        /* Mdct.RunImdct :94-119 */
 void vgo_hca_mdct_tables(double *sin_out, double *cos_out, int *shuffle_out, int bits); /* :183-208 */

@@ -173,3 +173,41 @@ def test_hca_encode_and_decode(vg, oracle, pipeline_groups):
     _same(dec)
     for s in range(N_UNITS):
         assert np.array_equal(dec[0][s], oracle.hca_decode(infos[s], frames[s])), s
+
+
+def test_hca_rows_of_separate_buffers_far_apart(vg, oracle):
+    """Caller buffers that are evenly spaced but not one block: the inputs of two streams 2 MiB apart, the output of the
+    first stream between them and that of the second far behind.  The call copies each buffer on its own, so it neither
+    page-locks the memory between the inputs nor copies over a span that runs from there into unregistered memory."""
+    import ctypes as C
+
+    MiB = 1 << 20
+    buf = np.zeros(16 * MiB, dtype=np.uint8)
+    pcm = [[synth.channel(930 + s, 4000, degenerate=False)] for s in range(2)]
+    o = [oracle.hca_encode(st, 48000) for st in pcm]
+    info0 = o[0][0]
+    size = info0.frame_count * info0.frame_size
+    infos = (vg._native.VgbHcaInfo * 2)()
+    for s in range(2):
+        for k, v in o[s][0].as_dict().items():
+            setattr(infos[s], k, v)
+
+    # decode: frames at 0 and 2 MiB, PCM at 1 MiB and 8 MiB
+    for s, at in enumerate((0, 2 * MiB)):
+        buf[at:at + size] = o[s][1].ravel()
+    ftab = (C.c_void_p * 2)(buf.ctypes.data, buf.ctypes.data + 2 * MiB)
+    otab = (C.c_void_p * 2)(buf.ctypes.data + MiB, buf.ctypes.data + 8 * MiB)
+    vg._native.check(vg.lib.vgb_hca_decode_batch(ftab, C.cast(infos, C.c_void_p), 2, otab))
+    for s, at in enumerate((MiB, 8 * MiB)):
+        got = buf[at:at + 2 * 4000].view(np.int16)
+        assert np.array_equal(got, oracle.hca_decode(infos[s], o[s][1])[0]), s
+
+    # encode: PCM at 0 and 2 MiB, frames at 1 MiB and 8 MiB
+    buf[:] = 0
+    for s, at in enumerate((0, 2 * MiB)):
+        buf[at:at + 8000] = pcm[s][0].view(np.uint8)
+    params = (vg._native.VgbHcaParams * 2)(*[vg._native.VgbHcaParams(2, 0, 0, 1, 48000, 4000, 0, 0, 0) for _ in range(2)])
+    vg._native.check(vg.lib.vgb_hca_encode_batch(ftab, C.cast(params, C.c_void_p), 2, C.cast(infos, C.c_void_p), otab,
+                                                 None, None))
+    for s, at in enumerate((MiB, 8 * MiB)):
+        assert np.array_equal(buf[at:at + size], o[s][1].ravel()), s

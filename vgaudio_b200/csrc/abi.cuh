@@ -155,8 +155,8 @@ bool uniform_stride(T *const *ptr, int32_t n, int64_t &stride_bytes)
 }
 
 // Copy of units [first, first + count) between the caller's buffers h_ptr[u] and the device slab (d_base + d_off[u],
-// bytes[u] bytes each): one strided 2D copy when both sides form a uniform slab, else one copy per non-empty unit.
-// Host -> device copies pin their sources.
+// bytes[u] bytes each): one 2D copy when the host rows are one contiguous block and the device rows evenly spaced, else
+// one copy per non-empty unit.  Host -> device copies pin their sources.
 template <typename T>
 int32_t copy_units(cudaMemcpyKind kind, char *d_base, const int64_t *d_off, T *const *h_ptr, const int64_t *bytes,
                    int first, int count, cudaStream_t stream)
@@ -170,10 +170,12 @@ int32_t copy_units(cudaMemcpyKind kind, char *d_base, const int64_t *d_off, T *c
     bool same = true;
     for (int c = 1; c < count; c++) same = same && bytes[c] == bytes[0];
     int64_t hstride = 0;
-    // a strided copy takes pitches below 2 GiB (cudaDevAttrMaxPitch); two separate caller arrays always look uniform, and
-    // may lie further apart than that
+    // a strided copy takes pitches below 2 GiB (cudaDevAttrMaxPitch).  The host rows must touch end to end: separate
+    // caller arrays can be evenly spaced as well, and a copy (or a page-lock) over the span between them covers memory
+    // the caller never handed over - other buffers, one of them perhaps page-locked by this call, and a host range that
+    // starts inside a registration and runs past its end is refused as an invalid argument.
     constexpr int64_t kMaxPitch = INT32_MAX;
-    if (same && count > 1 && bytes[0] > 0 && uniform_stride(h_ptr, count, hstride) && hstride >= bytes[0] &&  // overlapping rows: per-channel copies
+    if (same && count > 1 && bytes[0] > 0 && uniform_stride(h_ptr, count, hstride) && hstride == bytes[0] &&
         hstride <= kMaxPitch) {
         const int64_t dstride = d_off[1] - d_off[0];
         bool dsame = dstride > 0 && dstride <= kMaxPitch;

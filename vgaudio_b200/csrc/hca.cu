@@ -410,7 +410,9 @@ hca_encode_kernel(const int16_t *__restrict__ pcm, const HcaStream *__restrict__
         int found;
         if (low == high) found = low < 127 ? low : -1;
         else found = used_bits(noise_level, high) > available ? low : high;
-        if (found < 0) status = VGB_HCA_NOT_IMPLEMENTED;  // NotImplementedException (:499)
+        // NotImplementedException (:499).  Unreachable: `low` only ever takes a `mid` of at most 126, so low == high == 127
+        // cannot happen; the status is kept so that the restatement stays literal.
+        if (found < 0) status = VGB_HCA_NOT_IMPLEMENTED;
         else eval_boundary = found;
     }
 
@@ -711,6 +713,8 @@ hca_decode_parse_kernel(const uint8_t *__restrict__ frames, const HcaStream *__r
         const int type = cfg.channel_type[c];
         const int coded = type == 2 ? cfg.base_band_count : cfg.base_band_count + cfg.stereo_band_count;
         const int delta_bits = read(3);  // ReadScaleFactors (:108-126)
+        // DeltaDecode reads output[0] before its loop, so a channel without coded bands still consumes 6 bits (:183-186)
+        if (coded == 0 && delta_bits != 0 && delta_bits < 6) skip(6);
         int prev = 0;
         for (int b = 0; b < kBins; b++) {
             int sf = 0;
