@@ -1,9 +1,16 @@
-// bindings/csharp/GcAdpcmFormat.B200.cs — drop-in bodies for the two hot methods of
+// bindings/csharp/GcAdpcmFormat.B200.cs — drop-in bodies for the hot paths of
 // src/VGAudio/Formats/GcAdpcm/GcAdpcmFormat.cs.  Everything around them (builders, loop handling, containers) is
-// untouched: the Parallel.For over channels (GcAdpcmFormat.cs:65-68 and :45-48) becomes ONE batched native call.
+// untouched: the Parallel.For over channels (GcAdpcmFormat.cs:65-68, :45-48 and :31-38) becomes ONE batched native call.
+// GcAdpcmAlignment and GcAdpcmChannelBuilder gain `partial` and the internal members below, and GetAlignment's
+// `new GcAdpcmAlignment(LoopAlignmentMultiple, LoopStart, LoopEnd, Adpcm, Coefs)` (GcAdpcmChannelBuilder.cs:153) becomes
+// `BatchAlignment ?? new GcAdpcmAlignment(...)`: the fresh-alignment path then runs as before, including the
+// AlignedAdpcm / AlignedPcm / AlignedLoopStart assignments (:155-160) that the loop context and seek table read.  (Handing
+// the result over as PreviousAlignment would skip those assignments and change the loop context.)
 // NOT compiled here (no .NET toolchain in the build image).
 using System;
+using System.Collections.Generic;
 using System.Runtime.InteropServices;
+using System.Threading.Tasks;
 using VGAudio.Codecs.GcAdpcm;
 using VGAudio.Formats.Pcm16;
 using VGAudio.Native;
@@ -11,8 +18,103 @@ using static VGAudio.Codecs.GcAdpcm.GcAdpcmMath;
 
 namespace VGAudio.Formats.GcAdpcm
 {
+    internal partial class GcAdpcmAlignment
+    {
+        // The result of vgb_gcadpcm_align_batch for one channel: what the public constructor (:20-63) computes
+        internal GcAdpcmAlignment(int multiple, int loopStart, int loopEnd, int loopStartAligned, int sampleCountAligned,
+            byte[] adpcmAligned, short[] pcmAligned)
+        {
+            AlignmentMultiple = multiple;
+            LoopStart = loopStart;
+            LoopEnd = loopEnd;
+            AlignmentNeeded = true;
+            LoopStartAligned = loopStartAligned;
+            SampleCountAligned = sampleCountAligned;
+            AdpcmAligned = adpcmAligned;
+            PcmAligned = pcmAligned;
+        }
+    }
+
+    public partial class GcAdpcmChannelBuilder
+    {
+        // set by the GcAdpcmFormat constructor below for a channel whose alignment one batched native call computed
+        internal GcAdpcmAlignment BatchAlignment { get; set; }
+    }
+
     public partial class GcAdpcmFormat
     {
+        // replaces the body of internal GcAdpcmFormat(GcAdpcmFormatBuilder b)  (GcAdpcmFormat.cs:27-40).  Every channel
+        // whose builder would run new GcAdpcmAlignment in GetAlignment (GcAdpcmChannelBuilder.cs:148-163: looping, no
+        // reusable PreviousAlignment, loop start not on the multiple) gets it from one batched call instead, through
+        // BatchAlignment; the builder's own flow (loop context, seek table, PreviousAlignment reuse) stays managed.
+        internal unsafe GcAdpcmFormat(GcAdpcmFormatBuilder b) : base(b)
+        {
+            Channels = b.Channels;
+            AlignmentMultiple = b.AlignmentMultiple;
+
+            int n = Channels.Length;
+            var builders = new GcAdpcmChannelBuilder[n];
+            var todo = new List<int>();
+            for (int i = 0; i < n; i++)
+            {
+                builders[i] = Channels[i]
+                    .GetCloneBuilder()
+                    .WithLoop(Looping, UnalignedLoopStart, UnalignedLoopEnd)
+                    .WithLoopAlignment(b.AlignmentMultiple);
+                GcAdpcmChannelBuilder cb = builders[i];
+                if (cb.Looping && !cb.PreviousAlignmentIsValid() && !Utilities.Helpers.LoopPointsAreAligned(cb.LoopStart, cb.LoopAlignmentMultiple))
+                    todo.Add(i);
+            }
+
+            int m = todo.Count;
+            if (m > 0)
+            {
+                var prm = new VgAudioB200.VgbGcAlignParams[m];
+                var geo = new VgAudioB200.VgbGcAlignment[m];
+                var coefs = new short[m * 16];
+                var adpcmOut = new byte[m][];
+                var pcmOut = new short[m][];
+                var pins = new GCHandle[3 * m];
+                var inPtr = new IntPtr[m];
+                var adpcmPtr = new IntPtr[m];
+                var pcmPtr = new IntPtr[m];
+                var lens = new int[m];
+                try
+                {
+                    for (int k = 0; k < m; k++)
+                    {
+                        GcAdpcmChannelBuilder cb = builders[todo[k]];
+                        prm[k] = new VgAudioB200.VgbGcAlignParams { Multiple = cb.LoopAlignmentMultiple, LoopStart = cb.LoopStart, LoopEnd = cb.LoopEnd };
+                        fixed (VgAudioB200.VgbGcAlignParams* p = &prm[k])
+                        fixed (VgAudioB200.VgbGcAlignment* g = &geo[k])
+                            VgAudioB200.Check(VgAudioB200.vgb_gcadpcm_alignment(p, g));
+                        adpcmOut[k] = new byte[SampleCountToByteCount(geo[k].SampleCountAligned)];   // :33-34
+                        pcmOut[k] = new short[geo[k].SampleCountAligned];
+                        Array.Copy(cb.Coefs, 0, coefs, k * 16, 16);
+                        pins[3 * k] = GCHandle.Alloc(cb.Adpcm, GCHandleType.Pinned);
+                        pins[3 * k + 1] = GCHandle.Alloc(adpcmOut[k], GCHandleType.Pinned);
+                        pins[3 * k + 2] = GCHandle.Alloc(pcmOut[k], GCHandleType.Pinned);
+                        inPtr[k] = pins[3 * k].AddrOfPinnedObject();
+                        adpcmPtr[k] = pins[3 * k + 1].AddrOfPinnedObject();
+                        pcmPtr[k] = pins[3 * k + 2].AddrOfPinnedObject();
+                        lens[k] = cb.Adpcm.Length;
+                    }
+                    fixed (IntPtr* ip = inPtr) fixed (IntPtr* ap = adpcmPtr) fixed (IntPtr* pp = pcmPtr)
+                    fixed (int* l = lens) fixed (short* c = coefs) fixed (VgAudioB200.VgbGcAlignParams* p = prm)
+                        VgAudioB200.Check(VgAudioB200.vgb_gcadpcm_align_batch((byte**)ip, l, c, p, m, (byte**)ap, (short**)pp));
+                }
+                finally { foreach (var h in pins) if (h.IsAllocated) h.Free(); }
+
+                for (int k = 0; k < m; k++)
+                {
+                    builders[todo[k]].BatchAlignment = new GcAdpcmAlignment(prm[k].Multiple, prm[k].LoopStart, prm[k].LoopEnd,
+                        geo[k].LoopStartAligned, geo[k].SampleCountAligned, adpcmOut[k], pcmOut[k]);
+                }
+            }
+
+            Parallel.For(0, n, i => { Channels[i] = builders[i].Build(); });                  // :31-38, minus the re-encodes
+        }
+
         // replaces GcAdpcmFormat.EncodeFromPcm16(Pcm16Format, GcAdpcmParameters)  (GcAdpcmFormat.cs:58-74)
         public override unsafe GcAdpcmFormat EncodeFromPcm16(Pcm16Format pcm16, GcAdpcmParameters config)
         {

@@ -3,7 +3,7 @@
 // Two modes, both against the UNMODIFIED managed VGAudio (reference src/VGAudio/VGAudio.csproj):
 //   ParityHarness live            encodes / decodes the built-in inputs with the managed code AND with libvgaudio_b200.so
 //                                 (needs a CUDA device) and compares byte for byte - GC-ADPCM, CRI ADX (all types, versions,
-//                                 padding), CRI HCA (qualities, 1..8 channels, looping).  Modelled on the reference's own
+//                                 padding), CRI HCA (qualities, 1..8 channels, looping), GC-ADPCM loop alignment.  Modelled on the reference's own
 //                                 differential tool (src/VGAudio.Tools/GcAdpcm/Encode.cs:44-150).
 //   ParityHarness vectors <dir>   no GPU, no native library: reads the vector files tools/dump_vectors.py wrote on the GPU
 //                                 box (inputs + this repository's outputs), re-encodes every input with the managed
@@ -20,6 +20,7 @@ using VGAudio.Codecs.CriHca;
 using VGAudio.Codecs.GcAdpcm;
 using VGAudio.Formats;
 using VGAudio.Formats.CriHca;
+using VGAudio.Formats.GcAdpcm;
 using VGAudio.Formats.Pcm16;
 using VGAudio.Native;
 
@@ -179,6 +180,61 @@ internal static unsafe class ParityHarness
         return bad;
     }
 
+    // ---- GcAdpcmAlignment: the managed GcAdpcmFormat.WithAlignment path (GcAdpcmChannelBuilder.GetAlignment -> new
+    // GcAdpcmAlignment, GcAdpcmAlignment.cs:20-63) against vgb_gcadpcm_alignment + vgb_gcadpcm_align_batch ------------------
+    private static bool AlignmentCase(string name, byte[] adpcm, short[] coefs, int sampleCount, int multiple, int loopStart, int loopEnd)
+    {
+        GcAdpcmChannel managed = new GcAdpcmFormatBuilder(new[] { new GcAdpcmChannel(adpcm, coefs, sampleCount) }, 48000)
+            .WithLoop(true, loopStart, loopEnd).WithAlignment(multiple).Build().Channels[0];
+        var prm = new VgAudioB200.VgbGcAlignParams { Multiple = multiple, LoopStart = loopStart, LoopEnd = loopEnd };
+        var geo = new VgAudioB200.VgbGcAlignment();
+        VgAudioB200.Check(VgAudioB200.vgb_gcadpcm_alignment(&prm, &geo));
+        if (geo.AlignmentNeeded == 0)
+            return Report($"gcadpcm align {name} (not needed)", managed.GetAdpcmAudio(), adpcm) && managed.SampleCount == sampleCount;
+        var adpcmOurs = new byte[GcAdpcmMath.SampleCountToByteCount(geo.SampleCountAligned)];
+        var pcmOurs = new short[geo.SampleCountAligned];
+        int len = adpcm.Length;
+        fixed (byte* a0 = adpcm) fixed (short* c = coefs) fixed (byte* o0 = adpcmOurs) fixed (short* p0 = pcmOurs)
+        {
+            byte* a = a0; byte* o = o0; short* pp = p0;
+            VgAudioB200.Check(VgAudioB200.vgb_gcadpcm_align_batch(&a, &len, c, &prm, 1, &o, &pp));
+        }
+        byte[] pcmManagedBytes = managed.GetPcmAudio().SelectMany(BitConverter.GetBytes).ToArray();
+        byte[] pcmOursBytes = pcmOurs.SelectMany(BitConverter.GetBytes).ToArray();
+        bool same = Report($"gcadpcm align {name} AdpcmAligned", managed.GetAdpcmAudio(), adpcmOurs);
+        same &= Report($"gcadpcm align {name} PcmAligned", pcmManagedBytes, pcmOursBytes);
+        return same && managed.SampleCount == geo.SampleCountAligned;
+    }
+
+    private static int AlignmentCases()
+    {
+        int bad = 0;
+        // GcAdpcmAlignmentTests.cs:13-61: ADPCM of 0x40 zero bytes, zero coefficients
+        foreach (var (m, ls, le) in new[] { (0, 0, 10), (0, 5, 10), (1, 7, 10), (3, 12, 13), (5, 10, 13),     // AlignmentNotNeeded
+                                            (2, 3, 10), (4, 2, 10), (3, 31, 50), (16, 24, 50), (16, 31, 50) }) // AlignmentNeeded, AlignedLoopPoints
+            if (!AlignmentCase($"{m}/{ls}/{le}", new byte[0x40], new short[16], 112, m, ls, le)) bad++;
+        // GcAdpcmAlignmentTests.cs:64-108 (AlignedAdpcmIsCorrect / AlignedPcmIsCorrect): a sine of period 56
+        foreach (var (m, ls, cycles) in new[] { (1000, 4524, 100), (1000, 2012, 1), (1000, 60, 1), (1000, 60, 20) })
+        {
+            int le = cycles * 4 * 14 + ls;
+            short[] pcm = Sine((le + 13) / 14 * 14, 1, 14 * 4);
+            byte[] adpcm = ManagedGc(pcm, out short[] coefs);
+            if (!AlignmentCase($"sine {m}/{ls}/{le}", adpcm, coefs, pcm.Length, m, ls, le)) bad++;
+        }
+        // seeded: BRSTM's default multiple 0x3800 and others, loop points anywhere, sines at random pitches
+        var rng = new Random(0x414C49);
+        int[] multiples = { 0x3800, 0x3800, 14, 8, 1000, -3, 4096 };
+        for (int i = 0; i < 24; i++)
+        {
+            int n = rng.Next(20, 200000);
+            short[] pcm = Sine(n, 40 + rng.Next(8000), 48000);
+            byte[] adpcm = ManagedGc(pcm, out short[] coefs);
+            int le = rng.Next(1, n + 1), ls = rng.Next(0, le);
+            if (!AlignmentCase($"seeded {i}", adpcm, coefs, n, multiples[i % multiples.Length], ls, le)) bad++;
+        }
+        return bad;
+    }
+
     // ---- live mode -----------------------------------------------------------------------------------------------------
     private static int Live()
     {
@@ -222,7 +278,7 @@ internal static unsafe class ParityHarness
             byte[] ours = NativeHca(pcm, p);
             if (!Report($"crihca quality {quality} x {channels} ch", managed, ours)) bad++;
         }
-        return bad;
+        return bad + AlignmentCases();
     }
 
     private static int Main(string[] args)

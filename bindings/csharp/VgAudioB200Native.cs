@@ -59,6 +59,20 @@ namespace VGAudio.Native
         public static extern unsafe int vgb_gcadpcm_seek_context_batch(byte** adpcm, int* nBytes, short* coefs, VgbGcTapParams* parameters,
             int nChannels, short** seekTableOut, short* loopContextOut);
 
+        // GcAdpcmAlignment (GcAdpcmAlignment.cs:20-63): the loop-alignment re-encode of a batch of channels
+        [StructLayout(LayoutKind.Sequential)]
+        internal struct VgbGcAlignParams { public int Multiple, LoopStart, LoopEnd; }
+
+        [StructLayout(LayoutKind.Sequential)]
+        internal struct VgbGcAlignment { public int AlignmentNeeded, LoopStartAligned, SampleCountAligned; }
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        internal static extern int vgb_gcadpcm_alignment(VgbGcAlignParams* parameters, VgbGcAlignment* alignmentOut);
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        internal static extern int vgb_gcadpcm_align_batch(byte** adpcm, int* nBytes, short* coefs, VgbGcAlignParams* parameters,
+            int nChannels, byte** adpcmAlignedOut, short** pcmAlignedOut);
+
         public static void Check(int status)
         {
             if (status == Ok) return;

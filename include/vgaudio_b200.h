@@ -185,7 +185,8 @@ int32_t vgb_gcadpcm_decode_dev_status(const void *d_workspace, int32_t n_channel
  *                 entry 0 = (0, 0), entries = ceil(sample_count / spe)
  *   loop context  GcAdpcmLoopContext (GcAdpcmLoopContext.cs:17-26): predictor/scale byte of the frame holding the loop
  *                 start (GcAdpcmDecoder.GetPredictorScale :56-59), hist1 = pcm[loop_start - 1], hist2 = pcm[loop_start - 2]
- * Not covered: GcAdpcmAlignment's re-encode of an unaligned loop (GcAdpcmAlignment.cs:20-63).
+ *   alignment     GcAdpcmAlignment (GcAdpcmAlignment.cs:20-63): the re-encode that moves an unaligned loop start onto a
+ *                 multiple, below (vgb_gcadpcm_alignment, vgb_gcadpcm_align_batch)
  * ------------------------------------------------------------------------------------------------------- */
 typedef struct vgb_gc_tap_params {
     int32_t sample_count;
@@ -201,6 +202,35 @@ int32_t vgb_gcadpcm_seek_entry_count(int32_t sample_count, int32_t samples_per_e
 int32_t vgb_gcadpcm_seek_context_batch(const uint8_t *const *adpcm, const int32_t *n_bytes, const int16_t *coefs,
                                        const vgb_gc_tap_params *params, int32_t n_channels,
                                        int16_t *const *seek_table_out, int16_t *loop_context_out);
+
+/* Loop points of one channel before alignment (GcAdpcmAlignment's constructor arguments) and the geometry after it. */
+typedef struct vgb_gc_align_params { int32_t multiple, loop_start, loop_end; } vgb_gc_align_params;
+typedef struct vgb_gc_alignment { int32_t alignment_needed, loop_start_aligned, sample_count_aligned; } vgb_gc_alignment;
+
+/* GcAdpcmAlignment's geometry (GcAdpcmAlignment.cs:22-31 with Helpers.GetNextMultiple / LoopPointsAreAligned,
+ * Helpers.cs:71-83; C# `%` truncates toward zero).  Host only, needs no device.  Every field is 0 when no alignment is
+ * needed, as in the reference.  A multiple <= 0 leaves the loop start where it is, yet a negative multiple that does not
+ * divide the loop start still counts as "alignment needed": the tail is then re-encoded with no shift.
+ * VGB_E_ARG (out zeroed) when alignment is needed and the loop points are unusable, as for vgb_gcadpcm_align_batch. */
+int32_t vgb_gcadpcm_alignment(const vgb_gc_align_params *p, vgb_gc_alignment *out);
+
+/* new GcAdpcmAlignment(multiple, loopStart, loopEnd, adpcm, coefs) for n_channels channels, each with its own params;
+ * adpcm / n_bytes / coefs as in vgb_gcadpcm_decode_batch.  For a channel that needs alignment:
+ *   adpcm_aligned_out[c]  SampleCountToByteCount(sample_count_aligned) bytes (AdpcmAligned): the first loop_end / 14
+ *                         whole frames of adpcm[c], then the re-encoded tail
+ *   pcm_aligned_out       NULL, or pcm_aligned_out[c] receives sample_count_aligned samples (PcmAligned)
+ * Channels that need no alignment are skipped: their output rows may be NULL and are not written.
+ * Only the first SampleCountToByteCount(loop_end) bytes of a channel are read; the first decode starts from history
+ * (0, 0), not from the channel's start context (:41-42).  Errors, checked only on channels that need alignment:
+ *   VGB_E_ARG   before any device work: a negative loop point, loop_end < loop_start, n_bytes[c] shorter than loop_end
+ *               samples, sample_count_aligned past INT32_MAX, or loop_start == loop_end while the start moves.  The last
+ *               is a deliberate difference: the reference's tail loop (:48) then steps by zero and never ends.
+ *   VGB_E_DATA  a frame header below loop_end selects a predictor outside 0..7 (IndexOutOfRangeException in the first
+ *               Decode); the message names the lowest such channel.  The output rows are then unspecified.
+ * Sharded over the bound devices like the other host-pointer batch calls (weights: loop_end). */
+int32_t vgb_gcadpcm_align_batch(const uint8_t *const *adpcm, const int32_t *n_bytes, const int16_t *coefs,
+                                const vgb_gc_align_params *params, int32_t n_channels,
+                                uint8_t *const *adpcm_aligned_out, int16_t *const *pcm_aligned_out);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Block (de)interleave of channel payloads (SURVEY.md 8f rank 2): InterleaveExtensions.Interleave / DeInterleave

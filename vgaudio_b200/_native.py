@@ -40,6 +40,16 @@ class VgbGcTapParams(C.Structure):
     _fields_ = [("sample_count", C.c_int32), ("samples_per_seek_table_entry", C.c_int32), ("loop_start", C.c_int32)]
 
 
+class VgbGcAlignParams(C.Structure):
+    """GcAdpcmAlignment's constructor arguments (Formats/GcAdpcm/GcAdpcmAlignment.cs:20)."""
+
+    _fields_ = [("multiple", C.c_int32), ("loop_start", C.c_int32), ("loop_end", C.c_int32)]
+
+
+class VgbGcAlignment(C.Structure):
+    _fields_ = [("alignment_needed", C.c_int32), ("loop_start_aligned", C.c_int32), ("sample_count_aligned", C.c_int32)]
+
+
 class VgbHcaInfo(C.Structure):
     """The HcaInfo fields the codec uses (Codecs/CriHca/HcaInfo.cs:5-48)."""
 
@@ -171,6 +181,8 @@ SIGNATURES = {
     "vgb_hca_decode_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "vgb_gcadpcm_seek_entry_count": (C.c_int32, [C.c_int32, C.c_int32]),
     "vgb_gcadpcm_seek_context_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vgb_gcadpcm_alignment": (C.c_int32, [C.c_void_p, C.c_void_p]),
+    "vgb_gcadpcm_align_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "vgb_interleave_dev": (C.c_int32, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64,
                                        C.c_int32, C.c_int64, C.c_void_p]),
     "vgb_deinterleave_dev": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int64,

@@ -353,9 +353,229 @@ int32_t host_encode_sharded(const int16_t *const *pcm, const int32_t *n_samples,
     });
 }
 
+// ---- GcAdpcmAlignment (Formats/GcAdpcm/GcAdpcmAlignment.cs:20-63) --------------------------------------------------
+struct AlignGeom {
+    bool needed = false;
+    int32_t loop_start_aligned = 0, sample_count_aligned = 0;
+    int32_t keep = 0;        // samplesToKeep (:37-39): the whole frames below loop_end
+    int32_t keep_bytes = 0;  // bytesToKeep
+    int32_t count = 0;       // samplesToEncode
+};
+
+// SampleCountToNibbleCount without int32 wrap-around: where the reference's wraps, new byte[...] throws
+int64_t gc_nibble_count64(int64_t n) { return 16 * (n / kGcFrameSamples) + (n % kGcFrameSamples ? n % kGcFrameSamples + 2 : 0); }
+
+// The constructor's arithmetic (:22-39).  Returns why the loop points are unusable (the reference throws, or never
+// returns), or nullptr.
+const char *align_geometry(const vgb_gc_align_params &p, AlignGeom &g)
+{
+    g = AlignGeom{};
+    const int32_t m = p.multiple, ls = p.loop_start, le = p.loop_end;
+    if (m == -1 && ls == INT_MIN) return "loop_start % multiple overflows";  // int.MinValue % -1: OverflowException
+    g.needed = m != 0 && (m == -1 ? 0 : ls % m) != 0;                        // !Helpers.LoopPointsAreAligned
+    if (!g.needed) return nullptr;
+    if (ls < 0 || le < 0) return "negative loop point";
+    if (le < ls) return "loop_end is before loop_start";
+    const int64_t lsa = (m <= 0 || ls % m == 0) ? ls : (int64_t)ls + m - ls % m;  // Helpers.GetNextMultiple
+    const int64_t sca = (int64_t)le + (lsa - ls);
+    if (sca > INT32_MAX || gc_nibble_count64(sca) > INT32_MAX) return "the aligned sample count overflows int32";
+    // the reference's tail loop (:48) would step by loopLength == 0 forever
+    if (le == ls && lsa != ls) return "loop_start == loop_end: an empty loop cannot fill the shift of the loop start";
+    g.loop_start_aligned = (int32_t)lsa;
+    g.sample_count_aligned = (int32_t)sca;
+    g.keep = le / kGcFrameSamples * kGcFrameSamples;
+    g.keep_bytes = le / kGcFrameSamples * kGcFrameBytes;
+    g.count = g.sample_count_aligned - g.keep;
+    return nullptr;
+}
+
+// Validation of a whole batch (host only): the channels that need alignment and their geometry.
+int32_t align_plan(const uint8_t *const *adpcm, const int32_t *n_bytes, const vgb_gc_align_params *params, int32_t n_channels,
+                   uint8_t *const *adpcm_out, int16_t *const *pcm_out, std::vector<int> &idx, std::vector<AlignGeom> &geo)
+{
+    if (n_channels < 0) return fail(VGB_E_ARG, "n_channels is negative (%d)", n_channels);
+    if (n_channels > 0 && (!adpcm || !n_bytes || !params)) return fail(VGB_E_ARG, "NULL argument");
+    for (int c = 0; c < n_channels; c++) {
+        AlignGeom g;
+        if (const char *why = align_geometry(params[c], g)) return fail(VGB_E_ARG, "channel %d: %s", c, why);
+        if (!g.needed) continue;
+        const int32_t le = params[c].loop_end;
+        // GcAdpcmDecoder.Decode reads SampleCountToByteCount(loop_end) bytes (GcAdpcmChannel.cs:33-36's message)
+        if (n_bytes[c] < gc_sample_count_to_byte_count(le))  // le <= sample_count_aligned: no wrap-around
+            return fail(VGB_E_ARG, "channel %d: audio array length %d is too short for %d samples", c, n_bytes[c], le);
+        if (!adpcm[c]) return fail(VGB_E_ARG, "channel %d: NULL buffer", c);
+        if (!adpcm_out || !adpcm_out[c]) return fail(VGB_E_ARG, "channel %d: adpcm_aligned_out is NULL", c);
+        if (pcm_out && !pcm_out[c]) return fail(VGB_E_ARG, "channel %d: pcm_aligned_out is NULL", c);
+        idx.push_back(c);
+        geo.push_back(g);
+    }
+    return VGB_OK;
+}
+
+// One device: H2D of the prefixes, then decode -> tail -> encode (-> decode) on one stream, D2H into the caller's rows
+// and one synchronisation.  A predictor 8..15 below loop_end leaves the lowest such channel in *bad and returns
+// VGB_E_DATA.
+int32_t align_one(const uint8_t *const *adpcm, const int32_t *n_bytes, const int16_t *coefs, const vgb_gc_align_params *params,
+                  int32_t n_channels, uint8_t *const *adpcm_out, int16_t *const *pcm_out, int32_t *bad)
+{
+    PinScope pins;
+    std::vector<int> idx;
+    std::vector<AlignGeom> geo;
+    VGB_TRY(align_plan(adpcm, n_bytes, params, n_channels, adpcm_out, pcm_out, idx, geo));
+    const int m = (int)idx.size();
+    if (m == 0) return VGB_OK;
+    if (!coefs) return fail(VGB_E_ARG, "coefs is NULL");
+
+    // slabs: adpcm = [prefixes | tails], pcm = [decoded prefixes | tails | decoded tails]; workspaces of the three kernels
+    std::vector<int32_t> n_pre(m), n_tail(m);
+    for (int i = 0; i < m; i++) {
+        n_pre[i] = params[idx[i]].loop_end;
+        n_tail[i] = geo[i].count;
+    }
+    GcLayout pre, enc;
+    VGB_TRY(layout_common(pre, n_pre.data(), nullptr, m, true));
+    VGB_TRY(layout_common(enc, n_tail.data(), nullptr, m, true));
+    layout_pack_offsets(pre);
+    layout_pack_offsets(enc);
+    for (int i = 0; i < m; i++) {
+        enc.pcm_off[i] += pre.pcm_total;
+        enc.adpcm_off[i] += pre.adpcm_total;
+    }
+    GcLayout dec = enc;
+    for (int i = 0; i < m; i++) dec.pcm_off[i] += enc.pcm_total;
+    const GcWorkspace w_pre = carve(32, m), w_enc = carve(enc.rec_total, m), w_dec = carve(32, m);
+    const size_t at_enc = align_up(w_pre.total, 256), at_dec = at_enc + align_up(w_enc.total, 256);
+
+    std::vector<GcAlignChannel> chans(m);
+    std::vector<int16_t> co((size_t)m * 16);
+    std::vector<const uint8_t *> src(m);
+    std::vector<uint8_t *> tail_dst(m);
+    std::vector<int16_t *> pcm_pre_dst(m), pcm_tail_dst(m);
+    std::vector<int64_t> pre_bytes(m), tail_bytes(m), pre_pcm_b(m), pre_pcm_len(m), dec_pcm_b(m), dec_pcm_len(m);
+    for (int i = 0; i < m; i++) {
+        const int c = idx[i];
+        const AlignGeom &g = geo[i];
+        chans[i] = GcAlignChannel{pre.pcm_off[i], enc.pcm_off[i], params[c].loop_start, params[c].loop_end, g.keep, g.count};
+        std::copy_n(coefs + (size_t)c * 16, 16, co.begin() + (size_t)i * 16);
+        src[i] = adpcm[c];
+        pre_bytes[i] = gc_sample_count_to_byte_count(n_pre[i]);
+        tail_dst[i] = adpcm_out[c] + g.keep_bytes;
+        tail_bytes[i] = gc_sample_count_to_byte_count(g.count);
+        if (pcm_out) {
+            pcm_pre_dst[i] = pcm_out[c];
+            pcm_tail_dst[i] = pcm_out[c] + g.keep;
+        }
+        pre_pcm_b[i] = pre.pcm_off[i] * 2;
+        pre_pcm_len[i] = (int64_t)g.keep * 2;
+        dec_pcm_b[i] = dec.pcm_off[i] * 2;
+        dec_pcm_len[i] = (int64_t)g.count * 2;
+    }
+
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    VGB_TRY(ensure_ready_locked());
+    cudaStream_t st = g_ctx.stream;
+    VGB_TRY(g_ctx.adpcm.reserve((size_t)(pre.adpcm_total + enc.adpcm_total)));
+    VGB_TRY(g_ctx.pcm.reserve((size_t)(pre.pcm_total + 2 * enc.pcm_total) * 2));
+    VGB_TRY(g_ctx.coefs.reserve(co.size() * 2));
+    VGB_TRY(g_ctx.ws.reserve(at_dec + w_dec.total));
+    VGB_TRY(g_ctx.misc.reserve(chans.size() * sizeof(GcAlignChannel)));
+    int16_t *d_pcm = static_cast<int16_t *>(g_ctx.pcm.p);
+    uint8_t *d_adpcm = static_cast<uint8_t *>(g_ctx.adpcm.p);
+    const int16_t *d_coefs = static_cast<const int16_t *>(g_ctx.coefs.p);
+    const GcAlignChannel *d_chans = static_cast<const GcAlignChannel *>(g_ctx.misc.p);
+
+    VGB_TRY(copy_units(cudaMemcpyHostToDevice, g_ctx.adpcm.c(), pre.adpcm_off.data(), src.data(), pre_bytes.data(), 0, m, st));
+    // pageable sources: the runtime stages them before returning
+    CUDA_TRY(cudaMemcpyAsync(g_ctx.coefs.p, co.data(), co.size() * 2, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(g_ctx.misc.p, chans.data(), chans.size() * sizeof(GcAlignChannel), cudaMemcpyHostToDevice, st));
+    VGB_TRY(upload_tables(pre, w_pre, g_ctx.ws.p, st));
+    VGB_TRY(upload_tables(enc, w_enc, g_ctx.ws.c() + at_enc, st));
+    VGB_TRY(upload_tables(dec, w_dec, g_ctx.ws.c() + at_dec, st));
+    const GcChannelTable t_pre = table_view(g_ctx.ws.p, w_pre, m);
+    const GcChannelTable t_enc = table_view(g_ctx.ws.c() + at_enc, w_enc, m);
+    const GcChannelTable t_dec = table_view(g_ctx.ws.c() + at_dec, w_dec, m);
+
+    CUDA_TRY(cudaMemsetAsync(t_pre.status, 0x7f, 4, st));  // "no channel": any index is smaller
+    launch_gc_decode(d_adpcm, t_pre, d_coefs, d_pcm, pre.max_frames, 0, INT_MAX, st);           // :41-42
+    launch_gc_align_tail(d_pcm, d_chans, m, d_pcm, t_enc.hist, t_dec.hist, st);                 // :44-55
+    g_ctx.launches += (pre.max_frames > 0 ? 1 : 0) + 1;
+    CUDA_TRY(cudaGetLastError());
+    VGB_TRY(run_gc_encode(d_pcm, enc, d_coefs, const_cast<int16_t *>(d_coefs), d_adpcm, g_ctx.ws.c() + at_enc, w_enc, st,
+                          /*do_encode=*/true, /*timed=*/false, /*tables_uploaded=*/true));  // :57
+    if (pcm_out) {                                                                             // :61
+        launch_gc_decode(d_adpcm, t_dec, d_coefs, d_pcm, dec.max_frames, 0, INT_MAX, st);
+        g_ctx.launches += dec.max_frames > 0 ? 1 : 0;
+        CUDA_TRY(cudaGetLastError());
+    }
+    VGB_TRY(copy_units(cudaMemcpyDeviceToHost, g_ctx.adpcm.c(), enc.adpcm_off.data(), tail_dst.data(), tail_bytes.data(), 0, m, st));
+    if (pcm_out) {  // PcmAligned = first decode on [0, keep), the tail's decode on [keep, sample_count_aligned) (:43, :62)
+        VGB_TRY(copy_units(cudaMemcpyDeviceToHost, g_ctx.pcm.c(), pre_pcm_b.data(), pcm_pre_dst.data(), pre_pcm_len.data(), 0, m, st));
+        VGB_TRY(copy_units(cudaMemcpyDeviceToHost, g_ctx.pcm.c(), dec_pcm_b.data(), pcm_tail_dst.data(), dec_pcm_len.data(), 0, m, st));
+    }
+    int32_t bad_channel = INT_MAX;
+    CUDA_TRY(cudaMemcpyAsync(&bad_channel, t_pre.status, 4, cudaMemcpyDeviceToHost, st));
+    // the kept frames are the caller's own bytes (:58): copied here while the device works
+    for (int i = 0; i < m; i++) memcpy(adpcm_out[idx[i]], adpcm[idx[i]], (size_t)geo[i].keep_bytes);
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (bad_channel >= 0 && bad_channel < m) {  // IndexOutOfRangeException in the first Decode (GcAdpcmDecoder.cs:31-32)
+        if (bad) *bad = idx[bad_channel];
+        return fail(VGB_E_DATA, "channel %d: a frame header selects a predictor outside 0..7", idx[bad_channel]);
+    }
+    return VGB_OK;
+}
+
 }  // namespace
 
 extern "C" {
+
+int32_t vgb_gcadpcm_alignment(const vgb_gc_align_params *p, vgb_gc_alignment *out)
+{
+    if (!p || !out) return fail(VGB_E_ARG, "NULL argument");
+    *out = vgb_gc_alignment{0, 0, 0};
+    AlignGeom g;
+    if (const char *why = align_geometry(*p, g)) return fail(VGB_E_ARG, "%s", why);
+    if (g.needed) *out = vgb_gc_alignment{1, g.loop_start_aligned, g.sample_count_aligned};
+    return VGB_OK;
+}
+
+int32_t vgb_gcadpcm_align_batch(const uint8_t *const *adpcm, const int32_t *n_bytes, const int16_t *coefs,
+                                const vgb_gc_align_params *params, int32_t n_channels,
+                                uint8_t *const *adpcm_aligned_out, int16_t *const *pcm_aligned_out)
+{
+    if (!sharding_active(n_channels) || !adpcm || !n_bytes || !coefs || !params)
+        return align_one(adpcm, n_bytes, coefs, params, n_channels, adpcm_aligned_out, pcm_aligned_out, nullptr);
+    {  // every argument error before any device works
+        std::vector<int> idx;
+        std::vector<AlignGeom> geo;
+        VGB_TRY(align_plan(adpcm, n_bytes, params, n_channels, adpcm_aligned_out, pcm_aligned_out, idx, geo));
+        if (idx.empty()) return VGB_OK;
+    }
+    // a shard that meets a bad predictor reports its lowest channel; the call names the lowest of all shards
+    std::mutex mu;
+    int32_t lowest_bad = INT_MAX;
+    auto needed = [&](int c) { AlignGeom g; align_geometry(params[c], g); return g.needed ? params[c].loop_end : 0; };
+    VGB_TRY(run_sharded(shard_units(n_channels, needed, 64), [&](int, const std::vector<int> &u) -> int32_t {
+        auto s_in = pick_rows(adpcm, u);
+        auto s_nb = pick_rows(n_bytes, u);
+        auto s_co = pick_rows(coefs, u, 16);
+        auto s_par = pick_rows(params, u);
+        std::vector<uint8_t *> s_out;
+        std::vector<int16_t *> s_pcm;
+        if (adpcm_aligned_out) s_out = pick_rows(adpcm_aligned_out, u);
+        if (pcm_aligned_out) s_pcm = pick_rows(pcm_aligned_out, u);
+        int32_t bad = -1;
+        const int32_t rc = align_one(s_in.data(), s_nb.data(), s_co.data(), s_par.data(), (int32_t)u.size(),
+                                     adpcm_aligned_out ? s_out.data() : nullptr, pcm_aligned_out ? s_pcm.data() : nullptr, &bad);
+        if (rc == VGB_E_DATA && bad >= 0) {
+            std::lock_guard<std::mutex> lock(mu);
+            lowest_bad = std::min(lowest_bad, (int32_t)u[bad]);
+            return VGB_OK;
+        }
+        return rc;
+    }));
+    if (lowest_bad != INT_MAX) return fail(VGB_E_DATA, "channel %d: a frame header selects a predictor outside 0..7", lowest_bad);
+    return VGB_OK;
+}
 
 int32_t vgb_gcadpcm_sample_count_to_byte_count(int32_t n) { return gc_sample_count_to_byte_count(n); }
 int32_t vgb_gcadpcm_byte_count_to_sample_count(int32_t b) { return gc_nibble_count_to_sample_count(b * 2); }

@@ -76,6 +76,15 @@ struct GcTapChannel {
     int32_t loop_start;         // < 0: no loop context
 };
 
+// One channel of a loop-alignment batch (gc_align_tail_kernel, GcAdpcmAlignment.cs:44-55).
+struct GcAlignChannel {
+    int64_t src_off;     // first sample of the channel's decoded prefix [0, loop_end) in the PCM slab
+    int64_t dst_off;     // first sample of the channel's tail row (multiple of 8)
+    int32_t loop_start, loop_end;
+    int32_t keep;        // samplesToKeep: whole frames below loop_end
+    int32_t count;       // samplesToEncode: the tail's length
+};
+
 // One channel of a CRI ADX batch (mirror of CriAdxParameters, Codecs/CriAdx/CriAdxParameters.cs:3-13, plus layout).
 struct AdxChannel {
     int64_t pcm_off;     // sample offset in the PCM slab

@@ -40,6 +40,11 @@ void launch_gc_decode(const uint8_t *adpcm, const GcChannelTable &tab, const int
 void launch_gc_taps(const uint8_t *adpcm, const GcChannelTable &tab, const int16_t *coefs, const GcTapChannel *taps,
                     int16_t *tap_slab, int max_frames, cudaStream_t stream);
 
+// gc_align.cu — GcAdpcmAlignment's tail (Formats/GcAdpcm/GcAdpcmAlignment.cs:44-55): per channel, the samples to re-encode
+// into the 16-byte aligned row tail + dst_off, and the history pair into hist_enc[2c..] and hist_dec[2c..]
+void launch_gc_align_tail(const int16_t *pcm, const GcAlignChannel *chans, int n_channels, int16_t *tail, int16_t *hist_enc,
+                          int16_t *hist_dec, cudaStream_t stream);
+
 // adx.cu — CriAdxCodec.Encode / Decode (Codecs/CriAdx/CriAdxCodec.cs:9-171)
 int adx_encode_pick_segments(int n_channels, int max_whole_frames, int *min_seg_out = nullptr);
 void launch_adx_encode(const int16_t *pcm, const AdxChannel *tab, int n_channels, uint8_t *adpcm, int16_t *history_out,

@@ -90,9 +90,6 @@ class GcAdpcmFormat:
 
 
 # ---- GcAdpcmAlignment (Formats/GcAdpcm/GcAdpcmAlignment.cs:20-63) -------------------------------------------------
-# The loop-alignment re-encode is a composition of primitives the library already has - decode, encode with given
-# coefficients / history / sample count, decode - plus array copies; batched over channels it is three native calls.
-
 @dataclass
 class GcAdpcmAlignment:
     alignment_needed: bool
@@ -106,46 +103,11 @@ class GcAdpcmAlignment:
 
 def align_loops(adpcm_channels, coefs, multiple: int, loop_start: int, loop_end: int) -> List[GcAdpcmAlignment]:
     """GcAdpcmAlignment(multiple, loopStart, loopEnd, adpcm, coefs) for every channel of a format (the channels of one
-    stream share the loop points).  Mirrors the reference step by step; the arithmetic happens in the three batched
-    native calls."""
+    stream share the loop points): one native call, vgb_gcadpcm_align_batch."""
     n = len(adpcm_channels)
-    co = np.ascontiguousarray(coefs, dtype=np.int16).reshape(n, 16)
-    needed = not (multiple == 0 or loop_start % multiple == 0)  # Helpers.LoopPointsAreAligned
+    needed, loop_start_aligned, sample_count_aligned = gcadpcm.alignment(multiple, loop_start, loop_end)
     if not needed or n == 0:
         return [GcAdpcmAlignment(False, loop_start, loop_end) for _ in range(n)]
-    loop_length = loop_end - loop_start
-    loop_start_aligned = loop_start + (multiple - loop_start % multiple)  # GetNextMultiple
-    sample_count_aligned = loop_end + (loop_start_aligned - loop_start)
-    frames_to_keep = loop_end // gcadpcm.SAMPLES_PER_FRAME
-    bytes_to_keep = frames_to_keep * gcadpcm.BYTES_PER_FRAME
-    samples_to_keep = frames_to_keep * gcadpcm.SAMPLES_PER_FRAME
-    samples_to_encode = sample_count_aligned - samples_to_keep
-
-    old_pcm = gcadpcm.decode_batch(adpcm_channels, co, [GcAdpcmParameters(sample_count=loop_end)] * n)   # :42
-    new_pcm, configs, pcm_aligned = [], [], []
-    for c in range(n):
-        aligned = np.zeros(sample_count_aligned, dtype=np.int16)
-        aligned[:loop_end] = old_pcm[c][:loop_end]
-        tail = np.zeros(samples_to_encode, dtype=np.int16)
-        tail[: loop_end - samples_to_keep] = old_pcm[c][samples_to_keep:loop_end]
-        cur = loop_end - samples_to_keep
-        while cur < samples_to_encode:                                                                     # :48-51
-            k = min(loop_length, samples_to_encode - cur)
-            tail[cur:cur + k] = aligned[loop_start:loop_start + k]
-            cur += loop_length
-        new_pcm.append(tail)
-        pcm_aligned.append(aligned)
-        configs.append(GcAdpcmParameters(sample_count=samples_to_encode,
-                                         history1=int(old_pcm[c][samples_to_keep - 1]) if samples_to_keep >= 1 else 0,
-                                         history2=int(old_pcm[c][samples_to_keep - 2]) if samples_to_keep >= 2 else 0))
-    _, new_adpcm = gcadpcm.encode_batch(new_pcm, coefs=co, configs=configs)                               # :57
-    decoded = gcadpcm.decode_batch(new_adpcm, co, configs)                                                 # :61
-    out = []
-    for c in range(n):
-        adpcm_aligned = np.zeros(gcadpcm.sample_count_to_byte_count(sample_count_aligned), dtype=np.uint8)
-        adpcm_aligned[:bytes_to_keep] = np.asarray(adpcm_channels[c], dtype=np.uint8)[:bytes_to_keep]
-        adpcm_aligned[bytes_to_keep:bytes_to_keep + len(new_adpcm[c])] = new_adpcm[c]
-        pcm_aligned[c][samples_to_keep:samples_to_keep + samples_to_encode] = decoded[c][:samples_to_encode]
-        out.append(GcAdpcmAlignment(True, loop_start, loop_end, loop_start_aligned, sample_count_aligned,
-                                    adpcm_aligned, pcm_aligned[c]))
-    return out
+    adpcm_aligned, pcm_aligned = gcadpcm.align_batch(adpcm_channels, coefs, (multiple, loop_start, loop_end))
+    return [GcAdpcmAlignment(True, loop_start, loop_end, loop_start_aligned, sample_count_aligned, adpcm_aligned[c],
+                             pcm_aligned[c]) for c in range(n)]

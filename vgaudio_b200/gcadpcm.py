@@ -233,6 +233,41 @@ def seek_table_and_loop_context(adpcm, coefs, sample_counts, samples_per_seek_ta
     return seek, contexts
 
 
+def alignment(multiple: int, loop_start: int, loop_end: int):
+    """GcAdpcmAlignment's geometry (GcAdpcmAlignment.cs:22-31), host only: (alignment_needed, loop_start_aligned,
+    sample_count_aligned), all zero when no alignment is needed."""
+    out = N.VgbGcAlignment()
+    N.check(N.lib.vgb_gcadpcm_alignment(C.byref(N.VgbGcAlignParams(multiple, loop_start, loop_end)), C.byref(out)))
+    return bool(out.alignment_needed), out.loop_start_aligned, out.sample_count_aligned
+
+
+def align_batch(adpcm, coefs, params, pcm: bool = True):
+    """new GcAdpcmAlignment(multiple, loopStart, loopEnd, adpcm, coefs) (GcAdpcmAlignment.cs:20-63) for every channel in
+    one call.  params: one (multiple, loop_start, loop_end) per channel, or one for all.  Returns (adpcm_aligned,
+    pcm_aligned): per channel the AdpcmAligned bytes / PcmAligned samples, None where no alignment is needed (and for
+    every PcmAligned when pcm is False)."""
+    chans = _channel_list(adpcm, _as_u8)
+    n = len(chans)
+    lens = np.array([len(c) for c in chans], dtype=np.int32)
+    co = np.ascontiguousarray(coefs, dtype=np.int16).reshape(n, 16)
+    if n and np.ndim(params) == 1:
+        params = [params] * n
+    if len(params) != n:
+        raise ValueError("one (multiple, loop_start, loop_end) per channel expected")
+    par = (N.VgbGcAlignParams * max(n, 1))(*[N.VgbGcAlignParams(*map(int, p)) for p in params])
+    out_a, out_p = [None] * n, [None] * n
+    for i, p in enumerate(params):
+        needed, _, count = alignment(*map(int, p))
+        if needed:
+            out_a[i] = np.zeros(sample_count_to_byte_count(count), dtype=np.uint8)
+            out_p[i] = np.zeros(count, dtype=np.int16) if pcm else None
+    ptab = (C.c_void_p * max(n, 1))(*[a.ctypes.data if a is not None else None for a in out_p])
+    N.check(N.lib.vgb_gcadpcm_align_batch(_ptr_table(chans), lens.ctypes.data, co.ctypes.data, C.cast(par, C.c_void_p), n,
+                                          (C.c_void_p * max(n, 1))(*[a.ctypes.data if a is not None else None for a in out_a]),
+                                          ptab if pcm else None))
+    return out_a, out_p
+
+
 def get_predictor_scale(adpcm, sample: int) -> int:
     """GcAdpcmDecoder.GetPredictorScale (GcAdpcmDecoder.cs:56-59): metadata lookup, no arithmetic."""
     return int(adpcm[sample // SAMPLES_PER_FRAME * BYTES_PER_FRAME])
