@@ -1,6 +1,6 @@
 // bindings/csharp/Containers.B200.cs — P/Invoke declarations and replacement bodies for the container layer either side of
 // the codec path (include/vgaudio_b200.h, "Containers either side of the codec path"): WaveReader, DspWriter / DspReader,
-// AdxWriter (+ CriAdxEncryption), HcaWriter (+ CriHcaEncryption) and the CLI's batch job.
+// AdxWriter (+ CriAdxEncryption), HcaWriter / HcaReader (+ CriHcaEncryption) and the CLI's batch job.
 // NOT compiled in this repository (no .NET toolchain in the build image); this is the file a VGAudio maintainer adds.
 using System;
 using System.Collections.Generic;
@@ -73,6 +73,9 @@ namespace VGAudio.Native
         public static extern int vgb_hca_write_batch(VgbHcaInfo* info, int nFiles, byte** frames, int keyType, ulong keyCode, byte** comment, float* volume, byte** filesOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_dsp_to_wave_batch(byte** files, long* lengths, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_hca_parse(byte* file, long length, VgbHcaInfo* info, int* encryptionType);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_convert_hca_to_wave_batch(byte** files, long* lengths, int nFiles, ulong* keyCode, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_wave_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, long* outSizes,
             byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
@@ -162,6 +165,55 @@ namespace VGAudio.Cli
                     if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); continue; }   // Batch.cs:39-43
                     Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
                     File.WriteAllBytes(outPaths[i], outputs[i]);
+                }
+            }
+            finally
+            {
+                foreach (var h in inPins) h.Free();
+                foreach (var h in outPins) h.Free();
+            }
+        }
+
+        // The decode direction for a chunk of .hca files (`-b --out-format wav`): HcaReader -> ToPcm16 -> WaveWriter per file
+        // in one native call per pass.  keyCode is the type-56 key (CriHcaKey(ulong)); the native library carries no list of
+        // known keys, so a caller that wants HcaReader.FindKey's search runs CriHcaEncryption.FindKey on the file and passes
+        // the code it finds.  A file whose frames the decoder refuses (a wrong key, a bad frame) fails in the second pass alone.
+        public static unsafe void ConvertHcaToWave(string[] inPaths, string[] outPaths, ulong? keyCode, Action<string> log, Action<int> reportAdd)
+        {
+            int n = inPaths.Length;
+            byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
+            var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            var outPins = new List<GCHandle>();
+            try
+            {
+                byte** inPtr = stackalloc byte*[n];
+                byte** outPtr = stackalloc byte*[n];
+                long* len = stackalloc long[n];
+                long* outSize = stackalloc long[n];
+                int* status = stackalloc int[n];
+                ulong code = keyCode ?? 0;
+                ulong* codePtr = keyCode.HasValue ? &code : null;
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
+                VgAudioB200.Check(VgAudioB200Containers.vgb_convert_hca_to_wave_batch(inPtr, len, n, codePtr, outSize, null, status));
+                var outputs = new byte[n][];
+                for (int i = 0; i < n; i++)
+                {
+                    outPtr[i] = null;
+                    if (status[i] != VgAudioB200.Ok) continue;
+                    outputs[i] = new byte[outSize[i]];
+                    outPins.Add(GCHandle.Alloc(outputs[i], GCHandleType.Pinned));
+                    outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
+                }
+                VgAudioB200.Check(VgAudioB200Containers.vgb_convert_hca_to_wave_batch(inPtr, len, n, codePtr, outSize, outPtr, status));
+                for (int i = 0; i < n; i++)
+                {
+                    if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); }   // Batch.cs:39-43
+                    else
+                    {
+                        Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
+                        File.WriteAllBytes(outPaths[i], outputs[i]);
+                    }
+                    reportAdd(1);
                 }
             }
             finally

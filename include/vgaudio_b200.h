@@ -402,6 +402,20 @@ int32_t vgb_imdct128_batch(const double *in, int32_t n_sequences, int32_t n_bloc
 int32_t vgb_hca_decode_batch(const uint8_t *const *frames, const vgb_hca_info *info, int32_t n_streams,
                              int16_t *const *pcm_out);
 
+/* Device-resident variant of vgb_hca_decode_batch (asynchronous on `cuda_stream`), with the same rules for info (at most
+ * 65535 streams): the frames of stream s are frame_count * frame_size bytes at d_frames + frames_offset[s]; channel c of
+ * its PCM is written to sample_count samples at d_pcm + pcm_offset[s] + c * channel_stride[s] (channel_stride >=
+ * sample_count).  Samples no frame covers (sample_count > frame_count * 1024 - inserted_samples) are not written: clear
+ * the buffer first for the reference's fresh short[].  The workspace holds the stream table, the status words, the parse
+ * records and the seam addends; vgb_hca_decode_workspace_bytes sizes it from the same info.  The per-stream status of
+ * the decoder stays in the workspace: vgb_hca_decode_dev_status synchronises the stream and maps it to VGB_E_DATA with
+ * vgb_hca_decode_batch's messages. */
+uint64_t vgb_hca_decode_workspace_bytes(const vgb_hca_info *info, int32_t n_streams);
+int32_t vgb_hca_decode_dev(const uint8_t *d_frames, const int64_t *frames_offset, const vgb_hca_info *info, int32_t n_streams,
+                           int16_t *d_pcm, const int64_t *pcm_offset, const int64_t *channel_stride,
+                           void *d_workspace, uint64_t workspace_bytes, void *cuda_stream);
+int32_t vgb_hca_decode_dev_status(const void *d_workspace, int32_t n_streams, void *cuda_stream);
+
 
 /* =====================================================================================================================
  * Containers either side of the codec path (SURVEY.md 8f rank 2-4): the WAVE front end, the DSP / ADX / HCA writers, the
@@ -483,6 +497,15 @@ int32_t vgb_adx_write_batch(const vgb_adx_desc *files, int32_t n_files, const ui
 int32_t vgb_adx_crypt_batch(uint8_t *const *audio, int32_t n_channels, int32_t length, const vgb_adx_key *key,
                             int32_t encryption_type, int32_t frame_size);
 
+/* HcaReader.ReadHcaHeader (Containers/Hca/HcaReader.cs:59-121) on a file image, host only: the chunk walk over
+ * header_size bytes ("fmt", "comp", "dec", "loop", "ath", "ciph", "rva", "vbr", "comm", "pad"; every id byte masked with
+ * 0x7f, so the ids of encrypted files read the same; a later chunk overwrites what an earlier one set), UseAthCurve for
+ * an "ath" chunk of type 1 and for version < 0x0200 files without one, track_count at least 1, HcaInfo.CalculateHfrValues
+ * when bands_per_hfr_group > 0, sample_count = min(sample_count, LoopEndSample) for looping files.  The "ciph" value goes
+ * to *encryption_type_out (0 without the chunk; may be NULL).  VGB_E_DATA for a bad signature, an unknown chunk
+ * ("Chunk X is not supported."), a read past `length`, and an image shorter than header_size + frame_count * frame_size
+ * (where ReadHcaData, :123-138, would hand short frames to the decoder).  CRCs are not checked, as in the reference. */
+int32_t vgb_hca_parse(const uint8_t *file, int64_t length, vgb_hca_info *info_out, int32_t *encryption_type_out);
 /* CriHcaKey (Codecs/CriHca/CriHcaKey.cs): key_type 0, 1 or 56 (key_code used by 56 only); 256-byte substitution tables. */
 int32_t vgb_hca_key_tables(int32_t key_type, uint64_t key_code, uint8_t *decrypt_out, uint8_t *encrypt_out);
 /* CriHcaEncryption.Crypt (CriHcaEncryption.cs:12-33) for a batch of streams, in place: substitution over the first
@@ -531,6 +554,23 @@ int32_t vgb_convert_wave_batch(const uint8_t *const *files, const int64_t *lengt
  * samples).  A frame header that selects a predictor outside 0..7 fails the whole call (VGB_E_DATA). */
 int32_t vgb_convert_dsp_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, int64_t *out_sizes,
                                       uint8_t *const *files_out, int32_t *status_out);
+/* The decode direction of the batch job for .hca file images: HcaReader.ReadFile -> ToAudioStream (Containers/Hca/HcaReader.cs:20-49)
+ * -> CriHcaFormat.ToPcm16 (Formats/CriHca/CriHcaFormat.cs:25-32) -> WaveWriter, with vgb_convert_dsp_to_wave_batch's
+ * two-pass protocol and sharding (files weigh frame_count * channel_count).  Decryption follows HcaReader.FindKey
+ * (:238-252): "ciph" 1 uses the built-in type-1 table, 56 the table of *key_code, any other value none.  The reference's
+ * list of known keys is not carried: a type-56 file without key_code fails with "Cannot find key to decrypt HCA file.",
+ * and the given code is not tested against the frames.  Per file, on the device: the frames are copied in, decrypted in
+ * place, decoded (vgb_hca_decode_dev, one launch per group of files that share a codec configuration) and joined behind
+ * the WAVE header (smpl when looping, extensible fmt above two channels).
+ * Per-file errors, each failing that file only (Batch.cs:39-43): a parse error, more than 8 channels or a layout the
+ * decoder cannot take, sample_count < 0, 2 GiB of PCM or more, loop points WithLoop rejects (AudioFormatBaseBuilder.cs:23-50),
+ * a missing key - all known in the sizing pass - and a decoder status word on the device ("Invalid frame header" ...),
+ * known only in the fill pass: such a file gets its status_out entry, out_sizes[i] = 0 and its buffer is not written.
+ * Unlike the .dsp direction, where one bad predictor fails the call, a bad frame fails its file alone: a wrong key shows
+ * up exactly this way, and one such file must not cost the batch.  With status_out NULL, such a file fails the call
+ * (VGB_E_DATA) after every other file has been written. */
+int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files,
+                                      const uint64_t *key_code, int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
 /* Measurement tap: device time of the most recent vgb_convert_wave_batch summed over its (first 32) batches per device,
  * over every device that converted part of it, out[0..3] = WAVE split, encode, loop-context decode, file assembly (ms,
  * CUDA events on the kernel streams); returns the number of batches timed on all devices together. */

@@ -179,6 +179,10 @@ SIGNATURES = {
     "vgb_hca_query": (C.c_int32, [C.c_void_p, C.c_void_p]),
     "vgb_hca_encode_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_hca_decode_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "vgb_hca_decode_workspace_bytes": (C.c_uint64, [C.c_void_p, C.c_int32]),
+    "vgb_hca_decode_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_uint64, C.c_void_p]),
+    "vgb_hca_decode_dev_status": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
     "vgb_gcadpcm_seek_entry_count": (C.c_int32, [C.c_int32, C.c_int32]),
     "vgb_gcadpcm_seek_context_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "vgb_gcadpcm_alignment": (C.c_int32, [C.c_void_p, C.c_void_p]),
@@ -208,11 +212,13 @@ SIGNATURES = {
     "vgb_adx_file_size": (C.c_int64, [C.c_void_p]),
     "vgb_adx_write_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_adx_crypt_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32]),
+    "vgb_hca_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "vgb_hca_key_tables": (C.c_int32, [C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
     "vgb_hca_crypt_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int32]),
     "vgb_hca_write_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_debug_stage_ms": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_convert_dsp_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_convert_hca_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),
 }

@@ -5,10 +5,11 @@
 // WaveReader -> encoder -> writer chain of a chunk of files runs as ONE coalesced call on the device
 // (vgb_convert_wave_batch).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
-//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
+//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp and .hca inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--adxtype Linear|Fixed|Exp|ExpEnc...]
 //                 [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
+// With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey; there is no list of known keys).
 // --devices 0,1,2,3 binds those CUDA devices (vgb_init_devices): every chunk of files is then sharded over them, one
 // worker and one copy / kernel pipeline per device.  A device may be listed more than once.  The default is device 0.
 #include <sys/stat.h>
@@ -36,6 +37,13 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
     f.seekg(0);
     out.resize((size_t)n);
     return n == 0 || (bool)f.read(reinterpret_cast<char *>(out.data()), n);
+}
+
+static bool is_hca(const fs::path &p)
+{
+    std::string ext = p.extension().string();
+    std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
+    return ext == ".hca";
 }
 
 static int usage()
@@ -98,7 +106,7 @@ int main(int argc, char **argv)
         } else return usage();
     }
     if (in_dir.empty() || out_dir.empty()) return usage();
-    const bool to_wave = fmt == "wav";  // the decode direction: .dsp files in, 16-bit WAVE files out
+    const bool to_wave = fmt == "wav";  // the decode direction: .dsp and .hca files in, 16-bit WAVE files out
     if (fmt == "dsp") opt.out_type = VGB_CONTAINER_DSP;
     else if (fmt == "adx") opt.out_type = VGB_CONTAINER_ADX;
     else if (fmt == "hca") opt.out_type = VGB_CONTAINER_HCA;
@@ -112,14 +120,14 @@ int main(int argc, char **argv)
     }
     if (opt.out_type == VGB_CONTAINER_HCA && have_code) { opt.hca_key_type = 56; opt.hca_key_code = key_code; }
 
-    // Batch.cs:16-19: the files of the input directory (here: the WAVE ones; the other containers are not read)
+    // Batch.cs:16-19: the files of the input directory (here: the WAVE ones, or the .dsp and .hca ones when decoding)
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
         if (!e.is_regular_file()) return;
         std::string ext = e.path().extension().string();
         std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
-        if (to_wave ? ext == ".dsp" : (ext == ".wav" || ext == ".wave")) files.push_back(e.path());
+        if (to_wave ? (ext == ".dsp" || ext == ".hca") : (ext == ".wav" || ext == ".wave")) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -146,9 +154,26 @@ int main(int argc, char **argv)
         std::vector<int64_t> len(n), out_size(n);
         std::vector<int32_t> status(n);
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
-        auto convert = [&](uint8_t *const *outs) {
-            return to_wave ? vgb_convert_dsp_to_wave_batch(ptr.data(), len.data(), n, out_size.data(), outs, status.data())
-                           : vgb_convert_wave_batch(ptr.data(), len.data(), n, &opt, out_size.data(), outs, status.data(), nullptr, nullptr);
+        // decoding: the chunk's .dsp and .hca files go to their own converters, each on its rows of the chunk's tables
+        std::vector<int32_t> rows[2];
+        for (int k = 0; k < n; k++) rows[to_wave && is_hca(files[first + k])].push_back(k);
+        auto convert = [&](uint8_t *const *outs) -> int32_t {
+            if (!to_wave) return vgb_convert_wave_batch(ptr.data(), len.data(), n, &opt, out_size.data(), outs, status.data(), nullptr, nullptr);
+            for (int h = 0; h < 2; h++) {
+                const std::vector<int32_t> &r = rows[h];
+                if (r.empty()) continue;
+                std::vector<const uint8_t *> p;
+                std::vector<int64_t> l, sz(r.size());
+                std::vector<uint8_t *> o;
+                std::vector<int32_t> st(r.size());
+                for (int32_t k : r) { p.push_back(ptr[k]); l.push_back(len[k]); o.push_back(outs ? outs[k] : nullptr); }
+                const int32_t m = (int32_t)r.size();
+                const int32_t s = h ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), outs ? o.data() : nullptr, st.data())
+                                    : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), outs ? o.data() : nullptr, st.data());
+                if (s != VGB_OK) return s;
+                for (int32_t j = 0; j < m; j++) { out_size[r[j]] = sz[j]; status[r[j]] = st[j]; }
+            }
+            return VGB_OK;
         };
         if (convert(nullptr) != VGB_OK) {
             std::fprintf(stderr, "%s\n", vgb_last_error());

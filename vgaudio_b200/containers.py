@@ -208,6 +208,14 @@ def hca_crypt_batch(frames: Sequence[np.ndarray], frame_size: int, key_type: int
     return rows
 
 
+def hca_parse(file) -> Tuple[N.VgbHcaInfo, int]:
+    """HcaReader.ReadHcaHeader on a file image: (HcaInfo, the "ciph" encryption type); raises VgbError(VGB_E_DATA)."""
+    f = _bytes_arr(file)
+    info, ciph = N.VgbHcaInfo(), C.c_int32(0)
+    N.check(N.lib.vgb_hca_parse(f.ctypes.data, f.size, C.byref(info), C.byref(ciph)))
+    return info, int(ciph.value)
+
+
 def hca_write_batch(infos: Sequence[N.VgbHcaInfo], frames: Sequence[np.ndarray], key_type: int = -1, key_code: int = 0,
                     comments: Optional[Sequence[Optional[str]]] = None, volumes: Optional[Sequence[float]] = None) -> List[np.ndarray]:
     n = len(infos)
@@ -262,3 +270,12 @@ def convert_wave_batch(files: Sequence, options: N.VgbConvertOptions, progress=N
 def convert_dsp_to_wave_batch(files: Sequence) -> Tuple[List[Optional[np.ndarray]], List[int]]:
     """The decode direction of the batch job: .dsp images in, 16-bit WAVE images out (DspReader -> ToPcm16 -> WaveWriter)."""
     return _convert(N.lib.vgb_convert_dsp_to_wave_batch, files)
+
+
+def convert_hca_to_wave_batch(files: Sequence, key_code: Optional[int] = None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """The decode direction of the batch job for .hca images: HcaReader -> decrypt -> ToPcm16 -> WaveWriter.  key_code is
+    the type-56 key of keyed files (None: such files fail); a file whose frames the decoder refuses fails alone."""
+    code = C.c_uint64(key_code) if key_code is not None else None
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_hca_to_wave_batch(
+        ftab, lens, n, C.byref(code) if code is not None else None, sizes, otab, st), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames

@@ -114,6 +114,12 @@ extern thread_local Context *t_ctx;                     // the context this thre
 
 int32_t ensure_ready_locked();
 void hca_tables_release_locked();  // abi_hca.cu
+// abi_hca.cu, the HCA decoder's rules, shared by vgb_hca_decode_batch / _dev and the .hca -> WAVE converter:
+bool hca_same_config(const vgb_hca_info &a, const vgb_hca_info &b);  // one decode launch can take both streams
+int32_t hca_decode_check(const vgb_hca_info *info, int32_t n_streams);  // VGB_E_ARG unless one launch can decode all (n >= 1)
+int32_t hca_decode_fault(int32_t status, const char *what, int index);  // a decoder status word as the reference's exception
+// synchronises `st` and copies the status words of the last vgb_hca_decode_dev on `d_workspace` to status[0..n)
+int32_t hca_decode_words(const void *d_workspace, int32_t n_streams, int32_t *status, cudaStream_t st);
 void tick(int slot, bool begin, cudaStream_t stream);
 
 // hooks of containers.cu, which keeps its own slabs and streams per context (Context::containers)

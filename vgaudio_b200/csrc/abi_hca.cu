@@ -358,7 +358,74 @@ int32_t hca_tables_ready_locked()
     return VGB_OK;
 }
 
+// Byte offsets in a decode workspace (vgb_hca_decode_dev): stream table, status words, seam addends (2 x 128 doubles
+// per channel-frame), parse records
+struct HcaDecodeLayout {
+    size_t o_status, o_edge, o_parsed, bytes;
+    HcaDecodeLayout(const HcaConfig &cfg, int n_streams, int64_t total_frames)
+    {
+        const size_t n = (size_t)std::max(n_streams, 1);
+        o_status = align_up(n * sizeof(HcaStream), 256);
+        o_edge = align_up(o_status + n * 4, 256);
+        o_parsed = align_up(o_edge + (size_t)total_frames * cfg.channel_count * 2 * 128 * sizeof(double), 256);
+        bytes = align_up(o_parsed + hca_decode_parsed_bytes(cfg, total_frames), 256);
+    }
+};
+
 }  // namespace
+
+bool vgb::hca_same_config(const vgb_hca_info &a, const vgb_hca_info &b)
+{
+    return a.channel_count == b.channel_count && a.frame_size == b.frame_size && a.base_band_count == b.base_band_count &&
+           a.stereo_band_count == b.stereo_band_count && a.total_band_count == b.total_band_count && a.hfr_band_count == b.hfr_band_count &&
+           a.bands_per_hfr_group == b.bands_per_hfr_group && a.hfr_group_count == b.hfr_group_count && a.track_count == b.track_count &&
+           a.channel_config == b.channel_config && (a.use_ath_curve != 0) == (b.use_ath_curve != 0) &&
+           (!a.use_ath_curve || a.sample_rate == b.sample_rate);
+}
+
+int32_t vgb::hca_decode_check(const vgb_hca_info *info, int32_t n_streams)
+{
+    const vgb_hca_info &h0 = info[0];
+    if (h0.channel_count < 1 || h0.channel_count > 8) return fail(VGB_E_ARG, "channel_count must be 1..8");
+    for (int s = 0; s < n_streams; s++) {
+        const vgb_hca_info &b = info[s];
+        if (!hca_same_config(h0, b)) {
+            vgb_hca_info c = b;  // b with h0's ATH fields: differs only when the band layout or frame size does
+            c.use_ath_curve = h0.use_ath_curve;
+            c.sample_rate = h0.sample_rate;
+            if (!hca_same_config(h0, c)) return fail(VGB_E_ARG, "stream %d: all streams of one call must share the band layout and frame size", s);
+            return fail(VGB_E_ARG, "stream %d: all streams of one call must share UseAthCurve (and then the sample rate)", s);
+        }
+        if (b.sample_count < 0 || b.frame_count < 0 || b.inserted_samples < 0) return fail(VGB_E_ARG, "stream %d: negative count", s);
+    }
+    if (h0.frame_size < 8 || h0.frame_size > 0xffff) return fail(VGB_E_ARG, "frame_size out of range");
+    if (h0.base_band_count < 0 || h0.stereo_band_count < 0 || h0.base_band_count + h0.stereo_band_count > 128 ||
+        h0.total_band_count > 128 || h0.hfr_group_count < 0 || h0.hfr_group_count > 8 ||
+        (h0.hfr_group_count > 0 && h0.bands_per_hfr_group <= 0))
+        return fail(VGB_E_ARG, "band layout out of range");
+    if (h0.hfr_group_count > 0) {  // ReconstructHighFrequency mirrors bands around base+stereo: keep both sides in 0..127
+        const int start = h0.base_band_count + h0.stereo_band_count;
+        const int hfr_bands = std::min(h0.hfr_band_count, std::min(h0.total_band_count, 127) - h0.hfr_band_count);
+        if (hfr_bands > start || start + hfr_bands > 128) return fail(VGB_E_ARG, "high-frequency band layout out of range");
+    }
+    return VGB_OK;
+}
+
+int32_t vgb::hca_decode_fault(int32_t status, const char *what, int index)
+{
+    if (status == VGB_HCA_BAD_SYNC) return fail(VGB_E_DATA, "%s %d: Invalid frame header", what, index);
+    if (status == VGB_HCA_BAD_DELTA) return fail(VGB_E_DATA, "%s %d: scale factor delta out of range", what, index);
+    if (status == VGB_HCA_BAD_INDEX) return fail(VGB_E_DATA, "%s %d: intensity index out of range", what, index);
+    return VGB_OK;
+}
+
+int32_t vgb::hca_decode_words(const void *d_workspace, int32_t n_streams, int32_t *status, cudaStream_t st)
+{
+    const size_t o_status = align_up((size_t)std::max(n_streams, 1) * sizeof(HcaStream), 256);
+    CUDA_TRY(cudaMemcpyAsync(status, static_cast<const char *>(d_workspace) + o_status, (size_t)n_streams * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return VGB_OK;
+}
 
 extern "C" {
 
@@ -567,30 +634,9 @@ static int32_t hca_decode_one(const uint8_t *const *frames, const vgb_hca_info *
     if (n_streams < 0) return fail(VGB_E_ARG, "n_streams is negative");
     if (n_streams == 0) return VGB_OK;
     if (!frames || !info || !pcm_out) return fail(VGB_E_ARG, "NULL argument");
+    VGB_TRY(hca_decode_check(info, n_streams));
     const vgb_hca_info &h0 = info[0];
     const int nch = h0.channel_count;
-    if (nch < 1 || nch > 8) return fail(VGB_E_ARG, "channel_count must be 1..8");
-    for (int s = 0; s < n_streams; s++) {
-        const vgb_hca_info &b = info[s];
-        if (b.channel_count != nch || b.frame_size != h0.frame_size || b.base_band_count != h0.base_band_count ||
-            b.stereo_band_count != h0.stereo_band_count || b.total_band_count != h0.total_band_count ||
-            b.hfr_band_count != h0.hfr_band_count || b.bands_per_hfr_group != h0.bands_per_hfr_group ||
-            b.hfr_group_count != h0.hfr_group_count || b.track_count != h0.track_count || b.channel_config != h0.channel_config)
-            return fail(VGB_E_ARG, "stream %d: all streams of one call must share the band layout and frame size", s);
-        if ((b.use_ath_curve != 0) != (h0.use_ath_curve != 0) || (b.use_ath_curve && b.sample_rate != h0.sample_rate))
-            return fail(VGB_E_ARG, "stream %d: all streams of one call must share UseAthCurve (and then the sample rate)", s);
-        if (b.sample_count < 0 || b.frame_count < 0 || b.inserted_samples < 0) return fail(VGB_E_ARG, "stream %d: negative count", s);
-    }
-    if (h0.frame_size < 8 || h0.frame_size > 0xffff) return fail(VGB_E_ARG, "frame_size out of range");
-    if (h0.base_band_count < 0 || h0.stereo_band_count < 0 || h0.base_band_count + h0.stereo_band_count > 128 ||
-        h0.total_band_count > 128 || h0.hfr_group_count < 0 || h0.hfr_group_count > 8 ||
-        (h0.hfr_group_count > 0 && h0.bands_per_hfr_group <= 0))
-        return fail(VGB_E_ARG, "band layout out of range");
-    if (h0.hfr_group_count > 0) {  // ReconstructHighFrequency mirrors bands around base+stereo: keep both sides in 0..127
-        const int start = h0.base_band_count + h0.stereo_band_count;
-        const int hfr_bands = std::min(h0.hfr_band_count, std::min(h0.total_band_count, 127) - h0.hfr_band_count);
-        if (hfr_bands > start || start + hfr_bands > 128) return fail(VGB_E_ARG, "high-frequency band layout out of range");
-    }
     const HcaConfig cfg = hca_config(h0);
 
     std::vector<HcaStream> streams(n_streams);
@@ -683,11 +729,7 @@ static int32_t hca_decode_one(const uint8_t *const *frames, const vgb_hca_info *
         return copy_units(cudaMemcpyDeviceToHost, g_ctx.pcm.c(), out_off.data(), pcm_out, out_len.data(), s0 * nch, n * nch, g_ctx.s_out);
     };
     VGB_TRY(run_group_pipeline(n_groups, h2d, one_phase(kern), d2h, no_done));
-    for (int s = 0; s < n_streams; s++) {
-        if (status[s] == VGB_HCA_BAD_SYNC) return fail(VGB_E_DATA, "stream %d: Invalid frame header", s);
-        if (status[s] == VGB_HCA_BAD_DELTA) return fail(VGB_E_DATA, "stream %d: scale factor delta out of range", s);
-        if (status[s] == VGB_HCA_BAD_INDEX) return fail(VGB_E_DATA, "stream %d: intensity index out of range", s);
-    }
+    for (int s = 0; s < n_streams; s++) VGB_TRY(hca_decode_fault(status[s], "stream", s));
     return VGB_OK;
 }
 
@@ -702,6 +744,76 @@ int32_t vgb_hca_decode_batch(const uint8_t *const *frames, const vgb_hca_info *i
         auto s_out = pick_rows(pcm_out, u, nch);
         return hca_decode_one(s_in.data(), s_info.data(), (int)u.size(), s_out.data());
     });
+}
+
+/* ---- device-resident HCA decode (see the header) ---- */
+uint64_t vgb_hca_decode_workspace_bytes(const vgb_hca_info *info, int32_t n_streams)
+{
+    if (n_streams < 0 || (n_streams > 0 && !info)) return 0;
+    int64_t frames = 0;
+    for (int s = 0; s < n_streams; s++) frames += std::max(info[s].frame_count, 0);
+    HcaConfig cfg{};
+    cfg.channel_count = n_streams > 0 ? hca_clampi(info[0].channel_count, 1, 8) : 1;
+    return HcaDecodeLayout(cfg, n_streams, frames).bytes;
+}
+
+int32_t vgb_hca_decode_dev(const uint8_t *d_frames, const int64_t *frames_offset, const vgb_hca_info *info, int32_t n_streams,
+                           int16_t *d_pcm, const int64_t *pcm_offset, const int64_t *channel_stride,
+                           void *d_workspace, uint64_t workspace_bytes, void *cuda_stream)
+{
+    if (n_streams < 0) return fail(VGB_E_ARG, "n_streams is negative");
+    if (n_streams == 0) return VGB_OK;
+    if (!d_frames || !frames_offset || !info || !d_pcm || !pcm_offset || !channel_stride || !d_workspace) return fail(VGB_E_ARG, "NULL argument");
+    if (n_streams > 65535) return fail(VGB_E_ARG, "n_streams %d: at most 65535 streams per call", n_streams);  // grid y / z of the frame kernels
+    VGB_TRY(hca_decode_check(info, n_streams));
+    const uint64_t need = vgb_hca_decode_workspace_bytes(info, n_streams);
+    if (need > workspace_bytes) return fail(VGB_E_ARG, "workspace too small: need %llu bytes", (unsigned long long)need);
+    const HcaConfig cfg = hca_config(info[0]);
+    std::vector<HcaStream> streams(n_streams);
+    int64_t total_frames = 0;
+    int max_frames = 0;
+    for (int s = 0; s < n_streams; s++) {
+        const vgb_hca_info &h = info[s];
+        if (frames_offset[s] < 0 || pcm_offset[s] < 0 || channel_stride[s] < h.sample_count)
+            return fail(VGB_E_ARG, "stream %d: bad offsets (channel_stride must cover sample_count)", s);
+        HcaStream &t = streams[s];
+        t.pcm_off = pcm_offset[s];
+        t.channel_stride = channel_stride[s];
+        t.frames_off = frames_offset[s];
+        t.dct_off = total_frames;  // the parse records and seam addends are indexed by the call-wide frame number
+        t.sample_count = h.sample_count;
+        t.frame_count = h.frame_count;
+        t.inserted_samples = h.inserted_samples;
+        total_frames += h.frame_count;
+        max_frames = std::max(max_frames, h.frame_count);
+    }
+    const HcaDecodeLayout L(cfg, n_streams, total_frames);
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    VGB_TRY(ensure_ready_locked());
+    VGB_TRY(hca_tables_ready_locked());
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    char *ws = static_cast<char *>(d_workspace);
+    CUDA_TRY(cudaMemcpyAsync(ws, streams.data(), streams.size() * sizeof(HcaStream), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemsetAsync(ws + L.o_status, 0, (size_t)n_streams * 4, st));
+    tick(7, true, st);
+    CUDA_TRY(launch_hca_decode(d_frames, reinterpret_cast<const HcaStream *>(ws), n_streams, max_frames, total_frames, cfg, g_hca_tables.view,
+                               reinterpret_cast<uint8_t *>(ws + L.o_parsed), reinterpret_cast<double *>(ws + L.o_edge), d_pcm,
+                               reinterpret_cast<int32_t *>(ws + L.o_status), st));
+    tick(7, false, st);
+    g_ctx.launches += 3;
+    return VGB_OK;
+}
+
+/* Synchronises `cuda_stream` and maps the per-stream status words the last vgb_hca_decode_dev on this workspace left
+ * (the reference's InvalidDataException "Invalid frame header", ...). */
+int32_t vgb_hca_decode_dev_status(const void *d_workspace, int32_t n_streams, void *cuda_stream)
+{
+    if (n_streams <= 0) return VGB_OK;
+    if (!d_workspace) return fail(VGB_E_ARG, "NULL argument");
+    std::vector<int32_t> status(n_streams, 0);
+    VGB_TRY(hca_decode_words(d_workspace, n_streams, status.data(), static_cast<cudaStream_t>(cuda_stream)));
+    for (int s = 0; s < n_streams; s++) VGB_TRY(hca_decode_fault(status[s], "stream", s));
+    return VGB_OK;
 }
 
 }  // extern "C"
