@@ -1,6 +1,6 @@
 // bindings/csharp/Containers.B200.cs — P/Invoke declarations and replacement bodies for the container layer either side of
 // the codec path (include/vgaudio_b200.h, "Containers either side of the codec path"): WaveReader, DspWriter / DspReader,
-// AdxWriter (+ CriAdxEncryption), HcaWriter / HcaReader (+ CriHcaEncryption) and the CLI's batch job.
+// AdxWriter / AdxReader (+ CriAdxEncryption), HcaWriter / HcaReader (+ CriHcaEncryption) and the CLI's batch job.
 // NOT compiled in this repository (no .NET toolchain in the build image); this is the file a VGAudio maintainer adds.
 using System;
 using System.Collections.Generic;
@@ -33,6 +33,17 @@ namespace VGAudio.Native
 
     [StructLayout(LayoutKind.Sequential)]
     internal struct VgbAdxKey { public int Seed, Mult, Inc; }
+
+    [StructLayout(LayoutKind.Sequential)]
+    internal unsafe struct VgbAdxFileInfo   // AdxStructure (Containers/Adx/AdxStructure.cs) + where the audio sits
+    {
+        public int HeaderSize, Type, FrameSize, BitDepth, ChannelCount, SampleRate, SampleCount, HighpassFrequency;
+        public int Version, Revision, InsertedSamples, LoopCount, Looping, LoopType;
+        public int LoopStartSample, LoopStartByte, LoopEndSample, LoopEndByte;
+        public int SamplesPerFrame, Reserved;
+        public long AudioOffset, AudioSize;
+        public fixed short History[255 * 2];
+    }
 
     [StructLayout(LayoutKind.Sequential)]
     internal struct VgbConvertOptions
@@ -74,6 +85,9 @@ namespace VGAudio.Native
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_dsp_to_wave_batch(byte** files, long* lengths, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_hca_parse(byte* file, long length, VgbHcaInfo* info, int* encryptionType);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_adx_parse(byte* file, long length, VgbAdxFileInfo* info);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_convert_adx_to_wave_batch(byte** files, long* lengths, int nFiles, VgbAdxKey* key, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_hca_to_wave_batch(byte** files, long* lengths, int nFiles, ulong* keyCode, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
@@ -205,6 +219,56 @@ namespace VGAudio.Cli
                     outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
                 }
                 VgAudioB200.Check(VgAudioB200Containers.vgb_convert_hca_to_wave_batch(inPtr, len, n, codePtr, outSize, outPtr, status));
+                for (int i = 0; i < n; i++)
+                {
+                    if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); }   // Batch.cs:39-43
+                    else
+                    {
+                        Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
+                        File.WriteAllBytes(outPaths[i], outputs[i]);
+                    }
+                    reportAdd(1);
+                }
+            }
+            finally
+            {
+                foreach (var h in inPins) h.Free();
+                foreach (var h in outPins) h.Free();
+            }
+        }
+
+        // The decode direction for a chunk of .adx files (`-b --out-format wav`): AdxReader -> ToPcm16 -> WaveWriter per file
+        // in one native call per pass.  key (CriAdxKey from --keystring / --keycode, as vgb_adx_key_from_string / _code make it)
+        // decrypts files of revision 8 and 9; the native library carries no list of known keys, so a caller that wants
+        // CriAdxEncryption.FindKey's search runs it on the file and passes the key it finds.  A file whose frames select a
+        // filter the reference cannot index fails in the second pass alone.
+        public static unsafe void ConvertAdxToWave(string[] inPaths, string[] outPaths, VgbAdxKey? key, Action<string> log, Action<int> reportAdd)
+        {
+            int n = inPaths.Length;
+            byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
+            var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            var outPins = new List<GCHandle>();
+            try
+            {
+                byte** inPtr = stackalloc byte*[n];
+                byte** outPtr = stackalloc byte*[n];
+                long* len = stackalloc long[n];
+                long* outSize = stackalloc long[n];
+                int* status = stackalloc int[n];
+                VgbAdxKey k = key ?? default;
+                VgbAdxKey* keyPtr = key.HasValue ? &k : null;
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
+                VgAudioB200.Check(VgAudioB200Containers.vgb_convert_adx_to_wave_batch(inPtr, len, n, keyPtr, outSize, null, status));
+                var outputs = new byte[n][];
+                for (int i = 0; i < n; i++)
+                {
+                    outPtr[i] = null;
+                    if (status[i] != VgAudioB200.Ok) continue;
+                    outputs[i] = new byte[outSize[i]];
+                    outPins.Add(GCHandle.Alloc(outputs[i], GCHandleType.Pinned));
+                    outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
+                }
+                VgAudioB200.Check(VgAudioB200Containers.vgb_convert_adx_to_wave_batch(inPtr, len, n, keyPtr, outSize, outPtr, status));
                 for (int i = 0; i < n; i++)
                 {
                     if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); }   // Batch.cs:39-43

@@ -57,6 +57,19 @@ namespace VGAudio.Native
             int nChannels, short** pcmOut);
 
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern ulong vgb_adx_decode_workspace_bytes(int* sampleCount, VgbAdxParams* parameters, int nChannels);
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_adx_decode_dev(byte* dAdpcm, long* adpcmOffset, int* nBytes, int* sampleCount, VgbAdxParams* parameters,
+            int nChannels, short* dPcm, long* pcmOffset, void* dWorkspace, ulong workspaceBytes, IntPtr cudaStream);
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_adx_decode_dev_status(void* dWorkspace, int nChannels, IntPtr cudaStream);
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_adx_debug_decode_stats(ulong* output, int n);
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_hca_query(VgbHcaParams* parameters, VgbHcaInfo* infoOut);
 
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]

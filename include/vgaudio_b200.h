@@ -333,6 +333,31 @@ int32_t vgb_adx_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, cons
 int32_t vgb_adx_decode_batch(const uint8_t *const *adpcm, const int32_t *n_bytes, const int32_t *sample_count,
                              const vgb_adx_params *params, int32_t n_channels, int16_t *const *pcm_out);
 
+/* Device-resident, time-parallel variant of vgb_adx_decode_batch (same rules for params, sample_count and n_bytes, except
+ * that any sample rate is taken, as CriAdxCodec.Decode takes it; asynchronous on `cuda_stream`): channel c reads n_bytes[c] bytes at d_adpcm + adpcm_offset[c] and writes
+ * sample_count[c] samples to d_pcm + pcm_offset[c], zeros included where the padding logic produces none.  Each
+ * channel's frames are cut into segments decoded concurrently and spliced where a frame-end history pair matches
+ * (adx.cu; the segment count follows the SM and channel counts, VGB_ADX_DEC_SEGMENTS / VGB_ADX_DEC_MIN_SEG_FRAMES in the
+ * environment force it / the shortest segment).  18-byte frames whose row starts at a 16-byte aligned address take the
+ * fast path, and the output store width follows the address of each row; any base pointer and offset and any frame size
+ * 3..255 decode bit-exactly.  d_pcm must be 2-byte aligned and d_workspace 8-byte aligned (VGB_E_ARG otherwise).  A frame
+ * that yields no sample (the head frame when sample_count <= padding % samples per frame) never indexes the coefficient
+ * table, so its filter number is not checked, as in the reference.  The workspace (vgb_adx_decode_workspace_bytes from
+ * the same sample counts and params) holds the channel table, per-channel status words and the splice bookkeeping:
+ * vgb_adx_decode_dev_status synchronises the stream and returns VGB_E_DATA for the lowest channel whose Fixed-type
+ * frame selects a filter 4..7, with vgb_adx_decode_batch's message. */
+uint64_t vgb_adx_decode_workspace_bytes(const int32_t *sample_count, const vgb_adx_params *params, int32_t n_channels);
+int32_t vgb_adx_decode_dev(const uint8_t *d_adpcm, const int64_t *adpcm_offset, const int32_t *n_bytes, const int32_t *sample_count,
+                           const vgb_adx_params *params, int32_t n_channels, int16_t *d_pcm, const int64_t *pcm_offset,
+                           void *d_workspace, uint64_t workspace_bytes, void *cuda_stream);
+int32_t vgb_adx_decode_dev_status(const void *d_workspace, int32_t n_channels, void *cuda_stream);
+/* Bookkeeping of the most recent vgb_adx_decode_dev on this thread's context (its workspace must still be allocated;
+ * criadx.decode_dev returns it for that reason):
+ * out[0] segments per channel, out[1] frames decoded by the boundary run-ons, out[2] frames decoded by the serial
+ * cascade (boundaries whose run-on did not lock inside its segment), out[3] boundaries the cascade repaired, out[4] the
+ * longest run-on in frames.  n = how many words to fill (up to 5).  Synchronises the device. */
+int32_t vgb_adx_debug_decode_stats(uint64_t *out, int32_t n);
+
 /* ---------------------------------------------------------------------------------------------------------
  * CRI HCA encode (Codecs/CriHca/CriHcaEncoder.cs), host buffers.  One call replaces CriHcaFormat.EncodeFromPcm16
  * (Formats/CriHca/CriHcaFormat.cs:34-84, single-threaded in the reference) for a batch of streams.
@@ -497,6 +522,28 @@ int32_t vgb_adx_write_batch(const vgb_adx_desc *files, int32_t n_files, const ui
 int32_t vgb_adx_crypt_batch(uint8_t *const *audio, int32_t n_channels, int32_t length, const vgb_adx_key *key,
                             int32_t encryption_type, int32_t frame_size);
 
+/* AdxStructure (Containers/Adx/AdxStructure.cs) as AdxReader.ReadHeader / ReadData (Containers/Adx/AdxReader.cs:14-124)
+ * leave it, plus where the audio sits: audio_size bytes at audio_offset = header_size + 4, frame-interleaved over the
+ * channels.  history[c] is the header's pair of channel c (version >= 4 only), for reporting: ToPcm16 never uses it. */
+#define VGB_ADX_MAX_CHANNELS 255
+typedef struct vgb_adx_file_info {
+    int32_t header_size, type, frame_size, bit_depth, channel_count, sample_rate, sample_count, highpass_frequency;
+    int32_t version, revision, inserted_samples, loop_count, looping, loop_type;
+    int32_t loop_start_sample, loop_start_byte, loop_end_sample, loop_end_byte;
+    int32_t samples_per_frame, reserved;
+    int64_t audio_offset, audio_size;
+    int16_t history[VGB_ADX_MAX_CHANNELS][2];
+} vgb_adx_file_info;
+/* AdxReader.ReadFile's header and data reads on a file image, host only: big-endian, HeaderSize and InsertedSamples
+ * signed 16-bit; version >= 4 skips 4 bytes and reads two shorts per channel (4 more bytes skipped for mono); nothing
+ * past the history when Position + 24 > HeaderSize; the loop fields only when LoopCount > 0.  VGB_E_DATA, naming the
+ * file, wherever the reference throws: the signature ("File doesn't have ADX signature (0x80 0x00)"), a read past the
+ * image, a frame size or channel count of 0 (division by zero), a negative header offset or audio length, and an audio
+ * region shorter than AudioDataLength (Interleave.cs:118-128, "Specified length is greater than the number of bytes
+ * remaining in the Stream").  On purpose, where the reference would not throw but no decode can run: frame sizes 1 and 2
+ * (no whole sample per frame) and InsertedSamples <= -samples_per_frame (ToPcm16 would index before the audio). */
+int32_t vgb_adx_parse(const uint8_t *file, int64_t length, vgb_adx_file_info *info_out);
+
 /* HcaReader.ReadHcaHeader (Containers/Hca/HcaReader.cs:59-121) on a file image, host only: the chunk walk over
  * header_size bytes ("fmt", "comp", "dec", "loop", "ath", "ciph", "rva", "vbr", "comm", "pad"; every id byte masked with
  * 0x7f, so the ids of encrypted files read the same; a later chunk overwrites what an earlier one set), UseAthCurve for
@@ -571,6 +618,26 @@ int32_t vgb_convert_dsp_to_wave_batch(const uint8_t *const *files, const int64_t
  * (VGB_E_DATA) after every other file has been written. */
 int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files,
                                       const uint64_t *key_code, int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* The decode direction of the batch job for .adx file images: AdxReader -> ToAudioStream (Containers/Adx/AdxReader.cs:14-58)
+ * -> CriAdxFormat.ToPcm16 (Formats/CriAdx/CriAdxFormat.cs:35-55) -> WaveWriter, with vgb_convert_hca_to_wave_batch's
+ * two-pass protocol, per-file status and sharding (files weigh frames * channels).  Per group of files, on the device:
+ * the audio regions are copied in, de-interleaved into channel rows, decrypted in place where needed, decoded by the
+ * time-parallel decoder (vgb_adx_decode_dev) and joined behind the WAVE header.  The reference's rules kept:
+ * ToPcm16 decodes sample_count - inserted_samples samples with padding = inserted_samples, the header's frame size,
+ * high-pass, type and version and history 0 (the header's history is never handed to the decoder); the WAVE loop points
+ * are the loop samples minus inserted_samples, checked by WithLoop's rules (AudioFormatBaseBuilder.cs:23-50).
+ * Keys (*key from vgb_adx_key_from_code / _from_string, or NULL): revision 8 or 9 is decrypted with *key, and fails with
+ * "encrypted ADX file (type N) and no key" without one; any other revision is not decrypted.  Two differences on
+ * purpose: AdxReader.EncryptionKey would also "decrypt" files of other revisions, but a directory mixes files, so the key
+ * goes to types 8 and 9 only; and the reference's built-in key list (CriAdxEncryption.FindKey) is not carried - there is
+ * no key search.  A sample rate <= 0 decodes as in the reference (CalculateCoefficients' double math; a rate of 0 gives
+ * NaN, which C#'s (int) makes int.MinValue and (short) 0).  Per-file errors, each failing that file only: a parse error, a missing key, bad loop points, a negative
+ * unaligned sample count, decoded frames past a channel's audio (IndexOutOfRangeException), 2 GiB of PCM or more, too many
+ * channels for the WAVE join - all known in the sizing pass - and a Fixed-type frame with a filter 4..7, found on the
+ * device in the fill pass: that file gets its status_out entry, out_sizes[i] = 0 and its buffer is not written.  With
+ * status_out NULL such a file fails the call (VGB_E_DATA) after every other file has been written. */
+int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_adx_key *key,
+                                      int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
 /* Measurement tap: device time of the most recent vgb_convert_wave_batch summed over its (first 32) batches per device,
  * over every device that converted part of it, out[0..3] = WAVE split, encode, loop-context decode, file assembly (ms,
  * CUDA events on the kernel streams); returns the number of batches timed on all devices together. */

@@ -104,6 +104,19 @@ class VgbAdxKey(C.Structure):
     _fields_ = [("seed", C.c_int32), ("mult", C.c_int32), ("inc", C.c_int32)]
 
 
+VGB_ADX_MAX_CHANNELS = 255
+
+
+class VgbAdxFileInfo(C.Structure):
+    """AdxStructure as AdxReader leaves it (Containers/Adx/AdxStructure.cs), plus where the audio sits."""
+
+    _fields_ = [(n, C.c_int32) for n in ("header_size", "type", "frame_size", "bit_depth", "channel_count", "sample_rate",
+                                         "sample_count", "highpass_frequency", "version", "revision", "inserted_samples",
+                                         "loop_count", "looping", "loop_type", "loop_start_sample", "loop_start_byte",
+                                         "loop_end_sample", "loop_end_byte", "samples_per_frame", "reserved")] + [
+        ("audio_offset", C.c_int64), ("audio_size", C.c_int64), ("history", (C.c_int16 * 2) * VGB_ADX_MAX_CHANNELS)]
+
+
 class VgbConvertOptions(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("out_type", "no_trim", "dsp_samples_per_interleave", "dsp_loop_point_alignment",
                                          "adx_version", "adx_frame_size", "adx_type", "adx_filter_plus1",
@@ -167,6 +180,11 @@ SIGNATURES = {
                                          C.c_void_p, C.c_void_p]),
     "vgb_adx_calculate_coefficients": (C.c_int32, [C.c_int32, C.c_int32, C.c_void_p]),
     "vgb_adx_decode_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "vgb_adx_decode_workspace_bytes": (C.c_uint64, [C.c_void_p, C.c_void_p, C.c_int32]),
+    "vgb_adx_decode_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_uint64, C.c_void_p]),
+    "vgb_adx_decode_dev_status": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "vgb_adx_debug_decode_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_adx_workspace_bytes": (C.c_uint64, [C.c_int64, C.c_int32]),
     "vgb_adx_encode_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -212,6 +230,7 @@ SIGNATURES = {
     "vgb_adx_file_size": (C.c_int64, [C.c_void_p]),
     "vgb_adx_write_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_adx_crypt_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32]),
+    "vgb_adx_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
     "vgb_hca_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "vgb_hca_key_tables": (C.c_int32, [C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
     "vgb_hca_crypt_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int32]),
@@ -219,6 +238,7 @@ SIGNATURES = {
     "vgb_convert_debug_stage_ms": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_convert_dsp_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_hca_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_convert_adx_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),
 }

@@ -5,11 +5,12 @@
 // WaveReader -> encoder -> writer chain of a chunk of files runs as ONE coalesced call on the device
 // (vgb_convert_wave_batch).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
-//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp and .hca inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
+//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp, .hca and .adx inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--adxtype Linear|Fixed|Exp|ExpEnc...]
 //                 [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
-// With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey; there is no list of known keys).
+// With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
+// --keycode N, the CriAdxKey of type-8 / type-9 .adx files; there is no list of known keys.
 // --devices 0,1,2,3 binds those CUDA devices (vgb_init_devices): every chunk of files is then sharded over them, one
 // worker and one copy / kernel pipeline per device.  A device may be listed more than once.  The default is device 0.
 #include <sys/stat.h>
@@ -39,11 +40,12 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
     return n == 0 || (bool)f.read(reinterpret_cast<char *>(out.data()), n);
 }
 
-static bool is_hca(const fs::path &p)
+// which decoder takes an input of the decode direction: 0 .dsp, 1 .hca, 2 .adx
+static int decoder_of(const fs::path &p)
 {
     std::string ext = p.extension().string();
     std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
-    return ext == ".hca";
+    return ext == ".hca" ? 1 : ext == ".adx" ? 2 : 0;
 }
 
 static int usage()
@@ -106,28 +108,31 @@ int main(int argc, char **argv)
         } else return usage();
     }
     if (in_dir.empty() || out_dir.empty()) return usage();
-    const bool to_wave = fmt == "wav";  // the decode direction: .dsp and .hca files in, 16-bit WAVE files out
+    const bool to_wave = fmt == "wav";  // the decode direction: .dsp, .hca and .adx files in, 16-bit WAVE files out
     if (fmt == "dsp") opt.out_type = VGB_CONTAINER_DSP;
     else if (fmt == "adx") opt.out_type = VGB_CONTAINER_ADX;
     else if (fmt == "hca") opt.out_type = VGB_CONTAINER_HCA;
     else if (!to_wave) return usage();
-    if (opt.out_type == VGB_CONTAINER_ADX && (have_code || !key_string.empty())) {
-        vgb_adx_key k{};
-        const int32_t s = !key_string.empty() ? vgb_adx_key_from_string(key_string.c_str(), &k) : vgb_adx_key_from_code(key_code, &k);
+    vgb_adx_key adx_key{};  // the CriAdxKey of --keystring / --keycode, for writing .adx files or reading keyed ones
+    const bool have_adx_key = have_code || !key_string.empty();
+    if ((opt.out_type == VGB_CONTAINER_ADX || to_wave) && have_adx_key) {
+        const int32_t s = !key_string.empty() ? vgb_adx_key_from_string(key_string.c_str(), &adx_key) : vgb_adx_key_from_code(key_code, &adx_key);
         if (s != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
-        opt.adx_has_key = 1; opt.adx_key_seed = k.seed; opt.adx_key_mult = k.mult; opt.adx_key_inc = k.inc;
+    }
+    if (opt.out_type == VGB_CONTAINER_ADX && have_adx_key) {
+        opt.adx_has_key = 1; opt.adx_key_seed = adx_key.seed; opt.adx_key_mult = adx_key.mult; opt.adx_key_inc = adx_key.inc;
         opt.adx_encryption_type = !key_string.empty() ? 8 : 9;  // CreateConfiguration.cs:126-135: key strings are type 8, key codes type 9
     }
     if (opt.out_type == VGB_CONTAINER_HCA && have_code) { opt.hca_key_type = 56; opt.hca_key_code = key_code; }
 
-    // Batch.cs:16-19: the files of the input directory (here: the WAVE ones, or the .dsp and .hca ones when decoding)
+    // Batch.cs:16-19: the files of the input directory (here: the WAVE ones, or the .dsp, .hca and .adx ones when decoding)
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
         if (!e.is_regular_file()) return;
         std::string ext = e.path().extension().string();
         std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
-        if (to_wave ? (ext == ".dsp" || ext == ".hca") : (ext == ".wav" || ext == ".wave")) files.push_back(e.path());
+        if (to_wave ? (ext == ".dsp" || ext == ".hca" || ext == ".adx") : (ext == ".wav" || ext == ".wave")) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -154,12 +159,12 @@ int main(int argc, char **argv)
         std::vector<int64_t> len(n), out_size(n);
         std::vector<int32_t> status(n);
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
-        // decoding: the chunk's .dsp and .hca files go to their own converters, each on its rows of the chunk's tables
-        std::vector<int32_t> rows[2];
-        for (int k = 0; k < n; k++) rows[to_wave && is_hca(files[first + k])].push_back(k);
+        // decoding: the chunk's .dsp, .hca and .adx files go to their own converters, each on its rows of the chunk's tables
+        std::vector<int32_t> rows[3];
+        for (int k = 0; k < n; k++) rows[to_wave ? decoder_of(files[first + k]) : 0].push_back(k);
         auto convert = [&](uint8_t *const *outs) -> int32_t {
             if (!to_wave) return vgb_convert_wave_batch(ptr.data(), len.data(), n, &opt, out_size.data(), outs, status.data(), nullptr, nullptr);
-            for (int h = 0; h < 2; h++) {
+            for (int h = 0; h < 3; h++) {
                 const std::vector<int32_t> &r = rows[h];
                 if (r.empty()) continue;
                 std::vector<const uint8_t *> p;
@@ -168,8 +173,10 @@ int main(int argc, char **argv)
                 std::vector<int32_t> st(r.size());
                 for (int32_t k : r) { p.push_back(ptr[k]); l.push_back(len[k]); o.push_back(outs ? outs[k] : nullptr); }
                 const int32_t m = (int32_t)r.size();
-                const int32_t s = h ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), outs ? o.data() : nullptr, st.data())
-                                    : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), outs ? o.data() : nullptr, st.data());
+                uint8_t *const *ot = outs ? o.data() : nullptr;
+                const int32_t s = h == 2 ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, have_adx_key ? &adx_key : nullptr, sz.data(), ot, st.data())
+                                : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
+                                         : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());
                 if (s != VGB_OK) return s;
                 for (int32_t j = 0; j < m; j++) { out_size[r[j]] = sz[j]; status[r[j]] = st[j]; }
             }

@@ -194,6 +194,14 @@ def adx_crypt(audio: Sequence[np.ndarray], key: N.VgbAdxKey, encryption_type: in
 
 
 # ---- CRI HCA (Containers/Hca/HcaWriter.cs, Codecs/CriHca/CriHcaEncryption.cs, CriHcaKey.cs) -----------------------------
+def adx_parse(file) -> N.VgbAdxFileInfo:
+    """AdxReader.ReadFile's header and data reads on a file image; raises VgbError(VGB_E_DATA)."""
+    f = _bytes_arr(file)
+    info = N.VgbAdxFileInfo()
+    N.check(N.lib.vgb_adx_parse(f.ctypes.data, f.size, C.byref(info)))
+    return info
+
+
 def hca_key_tables(key_type: int, key_code: int = 0) -> Tuple[np.ndarray, np.ndarray]:
     dec, enc = np.zeros(256, np.uint8), np.zeros(256, np.uint8)
     N.check(N.lib.vgb_hca_key_tables(key_type, key_code, dec.ctypes.data, enc.ctypes.data))
@@ -278,4 +286,12 @@ def convert_hca_to_wave_batch(files: Sequence, key_code: Optional[int] = None) -
     code = C.c_uint64(key_code) if key_code is not None else None
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_hca_to_wave_batch(
         ftab, lens, n, C.byref(code) if code is not None else None, sizes, otab, st), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def convert_adx_to_wave_batch(files: Sequence, key: Optional[N.VgbAdxKey] = None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """The decode direction of the batch job for .adx images: AdxReader -> decrypt -> ToPcm16 -> WaveWriter.  key (from
+    adx_key) decrypts files of revision 8 and 9 (None: such files fail); a file with a bad Fixed-type filter fails alone."""
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_adx_to_wave_batch(
+        ftab, lens, n, C.byref(key) if key is not None else None, sizes, otab, st), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames

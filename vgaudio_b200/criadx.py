@@ -97,3 +97,30 @@ def decode_batch(adpcm, sample_counts, configs) -> List[np.ndarray]:
 def decode(adpcm, sample_count: int, config: Optional[CriAdxParameters] = None) -> np.ndarray:
     """CriAdxCodec.Decode(byte[] adpcm, int sampleCount, CriAdxParameters config = null)."""
     return decode_batch([adpcm], [sample_count], [config or CriAdxParameters()])[0]
+
+
+def decode_dev(d_adpcm, adpcm_offset, n_bytes, sample_counts, configs, d_pcm, pcm_offset, stream=None, workspace=None):
+    """CriAdxCodec.Decode for every channel on device buffers (vgb_adx_decode_dev, the time-parallel decoder): d_adpcm is
+    a uint8 and d_pcm an int16 CUDA tensor (views at any element offset are fine); channel c reads n_bytes[c] bytes at
+    adpcm_offset[c] and writes sample_counts[c] samples at pcm_offset[c].  Runs on `stream` (a torch.cuda.Stream, default
+    the current one) and waits for it; raises VgbError(VGB_E_DATA) for a Fixed-type frame with a filter outside 0..3.
+    `workspace` (a uint8 CUDA tensor of at least vgb_adx_decode_workspace_bytes) is allocated when None.  Returns the
+    workspace: vgb_adx_debug_decode_stats reads the last decode's bookkeeping from it, so keep it while the tap is read."""
+    import torch
+
+    n = len(sample_counts)
+    if isinstance(configs, CriAdxParameters):
+        configs = [configs] * n
+    counts = np.ascontiguousarray(sample_counts, dtype=np.int32)
+    nb = np.ascontiguousarray(n_bytes, dtype=np.int32)
+    a_off = np.ascontiguousarray(adpcm_offset, dtype=np.int64)
+    p_off = np.ascontiguousarray(pcm_offset, dtype=np.int64)
+    params = _params_array(configs)
+    ws_bytes = N.lib.vgb_adx_decode_workspace_bytes(counts.ctypes.data, C.cast(params, C.c_void_p), n)
+    if workspace is None:
+        workspace = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=d_pcm.device)
+    st = (stream or torch.cuda.current_stream(d_pcm.device)).cuda_stream
+    N.check(N.lib.vgb_adx_decode_dev(d_adpcm.data_ptr(), a_off.ctypes.data, nb.ctypes.data, counts.ctypes.data, C.cast(params, C.c_void_p), n,
+                                     d_pcm.data_ptr(), p_off.ctypes.data, workspace.data_ptr(), workspace.numel(), st))
+    N.check(N.lib.vgb_adx_decode_dev_status(workspace.data_ptr(), n, st))
+    return workspace

@@ -103,6 +103,7 @@ struct Context {
     bool ev_used[kTimers] = {};
     std::atomic<int64_t> launches{0};
     GcSegArgs last_seg{};            // bookkeeping of the most recent encode launch (vgb_gcadpcm_debug_splice_stats)
+    AdxDecSegArgs last_adx_dec{};    // the same for the most recent time-parallel ADX decode (vgb_adx_debug_decode_stats)
     HcaTableStore hca_tables;
     std::atomic<ContainerState *> containers{nullptr};  // created on first use, released by containers_release
 };
@@ -120,6 +121,9 @@ int32_t hca_decode_check(const vgb_hca_info *info, int32_t n_streams);  // VGB_E
 int32_t hca_decode_fault(int32_t status, const char *what, int index);  // a decoder status word as the reference's exception
 // synchronises `st` and copies the status words of the last vgb_hca_decode_dev on `d_workspace` to status[0..n)
 int32_t hca_decode_words(const void *d_workspace, int32_t n_streams, int32_t *status, cudaStream_t st);
+// abi_adx.cu: synchronises `st` and copies the per-channel status words of the last vgb_adx_decode_dev on `d_workspace`
+// (bit 0: a Fixed-type frame selects a filter 4..7, bit 1: a frame of another type a filter 1..7) to status[0..n)
+int32_t adx_decode_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st);
 void tick(int slot, bool begin, cudaStream_t stream);
 
 // hooks of containers.cu, which keeps its own slabs and streams per context (Context::containers)

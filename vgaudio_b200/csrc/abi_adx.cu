@@ -1,5 +1,5 @@
 // abi_adx.cu — the CRI ADX entry points of the C ABI: host-pointer batch calls (pipelined over channel groups, sharded
-// over the bound devices) and the device-resident encode.
+// over the bound devices), the device-resident encode and the device-resident, time-parallel decode.
 #include <climits>
 #include <cmath>
 
@@ -22,25 +22,30 @@ int32_t vgb_adx_encoded_byte_count(int32_t pcm_length, int32_t padding, int32_t 
 
 namespace {
 
+// (int)double on x64 (cvttsd2si): NaN and values outside int32 give int.MinValue
+int32_t cast_double_to_int_x64(double v) { return (v > -2147483649.0 && v < 2147483648.0) ? (int32_t)v : INT32_MIN; }
+
 // CriAdxCodec.CalculateCoefficients (CriAdxCodec.cs:173-184): host double math, once per distinct (freq, rate).
-// (short)(double) goes through (int) truncation like the oracle.
+// (short)(double) goes through (int) truncation like the oracle; a rate of 0 makes the pair NaN, which C# casts to 0.
 void adx_calc_coefs(int highpass, int rate, int16_t &c0, int16_t &c1)
 {
     const double sqrt2 = std::sqrt(2.0);
     const double a = sqrt2 - std::cos(2.0 * 3.14159265358979323846 * highpass / rate);
     const double b = sqrt2 - 1;
     const double c = (a - std::sqrt((a + b) * (a - b))) / b;
-    c0 = (int16_t)(int32_t)(c * 8192);
-    c1 = (int16_t)(int32_t)(c * c * -4096);
+    c0 = (int16_t)cast_double_to_int_x64(c * 8192);
+    c1 = (int16_t)cast_double_to_int_x64(c * c * -4096);
 }
 
-int32_t adx_validate(const vgb_adx_params &p, int c)
+// any_rate: the decode-side entry points take every sample rate the reference decodes (CalculateCoefficients is defined
+// for all of them); the host batch calls keep their positive-rate rule
+int32_t adx_validate(const vgb_adx_params &p, int c, bool any_rate = false)
 {
     if (p.frame_size < 3 || p.frame_size > 255) return fail(VGB_E_ARG, "channel %d: frame_size %d outside 3..255", c, p.frame_size);
     if (p.type != 2 && p.type != 3 && p.type != 4) return fail(VGB_E_ARG, "channel %d: unknown CriAdxType %d", c, p.type);
     if (p.type == 2 && (p.filter < 0 || p.filter > 3)) return fail(VGB_E_ARG, "channel %d: filter %d outside 0..3", c, p.filter);
     if (p.padding < 0) return fail(VGB_E_ARG, "channel %d: negative padding", c);
-    if (p.sample_rate <= 0) return fail(VGB_E_ARG, "channel %d: sample_rate must be positive", c);
+    if (p.sample_rate <= 0 && !any_rate) return fail(VGB_E_ARG, "channel %d: sample_rate must be positive", c);
     return VGB_OK;
 }
 
@@ -335,6 +340,140 @@ int32_t vgb_adx_decode_batch(const uint8_t *const *adpcm, const int32_t *n_bytes
         auto s_out = pick_rows(pcm_out, u);
         return adx_decode_one(s_in.data(), s_nb.data(), s_sc.data(), s_par.data(), (int)u.size(), s_out.data());
     });
+}
+
+}  // extern "C"
+
+namespace {
+
+// Byte offsets in a workspace of the time-parallel decode (vgb_adx_decode_dev): channel table, status words, run-on
+// start pairs, stats, the trace (one word per body frame)
+struct AdxDecodeLayout {
+    size_t o_status, o_used, o_stats, o_trace, bytes;
+    AdxDecodeLayout(int n_channels, int64_t body_frames)
+    {
+        const size_t n = (size_t)std::max(n_channels, 1);
+        o_status = align_up(n * sizeof(AdxDecChannel), 256);
+        o_used = o_status + align_up(n * 4, 256);
+        o_stats = o_used + align_up(n * kAdxDecMaxSegments * 4, 256);
+        o_trace = o_stats + 256;
+        bytes = o_trace + align_up((size_t)(body_frames + 1) * 4, 256);
+    }
+};
+
+int64_t adx_body_frames(const int32_t *sample_count, const vgb_adx_params *params, int32_t n_channels)
+{
+    int64_t frames = 0;
+    for (int c = 0; c < n_channels; c++) {
+        const vgb_adx_params &p = params[c];
+        if (p.frame_size < 3 || p.frame_size > 255 || p.padding < 0 || sample_count[c] < 0) continue;  // refused by the call
+        frames += adx_dec_geom(sample_count[c], p.frame_size, p.padding).body;
+    }
+    return frames;
+}
+
+}  // namespace
+
+int32_t vgb::adx_decode_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st)
+{
+    const AdxDecodeLayout L(n_channels, 0);
+    CUDA_TRY(cudaMemcpyAsync(status, static_cast<const char *>(d_workspace) + L.o_status, (size_t)n_channels * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return VGB_OK;
+}
+
+extern "C" {
+
+/* ---- device-resident, time-parallel ADX decode (see the header) ---- */
+uint64_t vgb_adx_decode_workspace_bytes(const int32_t *sample_count, const vgb_adx_params *params, int32_t n_channels)
+{
+    if (n_channels < 0 || (n_channels > 0 && (!sample_count || !params))) return 0;
+    return AdxDecodeLayout(n_channels, adx_body_frames(sample_count, params, n_channels)).bytes;
+}
+
+int32_t vgb_adx_decode_dev(const uint8_t *d_adpcm, const int64_t *adpcm_offset, const int32_t *n_bytes, const int32_t *sample_count,
+                           const vgb_adx_params *params, int32_t n_channels, int16_t *d_pcm, const int64_t *pcm_offset,
+                           void *d_workspace, uint64_t workspace_bytes, void *cuda_stream)
+{
+    if (n_channels < 0) return fail(VGB_E_ARG, "n_channels is negative");
+    if (n_channels == 0) return VGB_OK;
+    if (!d_adpcm || !adpcm_offset || !n_bytes || !sample_count || !params || !d_pcm || !pcm_offset || !d_workspace)
+        return fail(VGB_E_ARG, "NULL argument");
+    if ((reinterpret_cast<uintptr_t>(d_pcm) & 1) || (reinterpret_cast<uintptr_t>(d_workspace) & 7))
+        return fail(VGB_E_ARG, "d_pcm must be 2-byte and d_workspace 8-byte aligned");
+    std::vector<AdxDecChannel> tab(n_channels);
+    int64_t frames = 0;
+    int max_body = 0;
+    for (int c = 0; c < n_channels; c++) {
+        const vgb_adx_params &p = params[c];
+        VGB_TRY(adx_validate(p, c, /*any_rate=*/true));
+        if (sample_count[c] < 0 || n_bytes[c] < 0) return fail(VGB_E_ARG, "channel %d: negative length", c);
+        if (adpcm_offset[c] < 0 || pcm_offset[c] < 0) return fail(VGB_E_ARG, "channel %d: negative offset", c);
+        const AdxDecGeom g = adx_dec_geom(sample_count[c], p.frame_size, p.padding);
+        // the frames Decode walks must lie inside the row: the reference would index past its array
+        const int64_t need = g.in0 + (int64_t)g.frames * p.frame_size;
+        if (sample_count[c] > 0 && n_bytes[c] < need)
+            return fail(VGB_E_ARG, "channel %d: %d bytes of ADX data, %lld needed for %d samples", c, n_bytes[c], (long long)need, sample_count[c]);
+        AdxDecChannel &t = tab[c];
+        t.pcm_off = pcm_offset[c]; t.adpcm_off = adpcm_offset[c]; t.trace_off = frames;
+        t.n_samples = sample_count[c]; t.frame_size = p.frame_size; t.version = p.version; t.padding = p.padding; t.type = p.type;
+        t.history = (int16_t)p.history;
+        if (p.type == 2) { t.coef0 = 0; t.coef1 = 0; }
+        else adx_calc_coefs(p.highpass_frequency, p.sample_rate, t.coef0, t.coef1);
+        frames += g.body;
+        max_body = std::max(max_body, g.body);
+    }
+    const AdxDecodeLayout L(n_channels, frames);
+    if (L.bytes > workspace_bytes) return fail(VGB_E_ARG, "workspace too small: need %llu bytes", (unsigned long long)L.bytes);
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    VGB_TRY(ensure_ready_locked());
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    char *ws = static_cast<char *>(d_workspace);
+    AdxDecSegArgs sa{};
+    sa.trace = reinterpret_cast<uint32_t *>(ws + L.o_trace);
+    sa.used_start = reinterpret_cast<uint32_t *>(ws + L.o_used);
+    sa.stats = reinterpret_cast<unsigned long long *>(ws + L.o_stats);
+    sa.status = reinterpret_cast<int32_t *>(ws + L.o_status);
+    sa.seg_count = adx_decode_pick_segments(n_channels, max_body, &sa.min_seg_frames);
+    CUDA_TRY(cudaMemcpyAsync(ws, tab.data(), tab.size() * sizeof(AdxDecChannel), cudaMemcpyHostToDevice, st));  // pageable: staged before return
+    CUDA_TRY(cudaMemsetAsync(ws + L.o_status, 0, (size_t)n_channels * 4, st));
+    CUDA_TRY(cudaMemsetAsync(ws + L.o_stats, 0, kAdxDecStatWords * sizeof(unsigned long long), st));
+    tick(5, true, st);
+    launch_adx_decode_seg(d_adpcm, reinterpret_cast<const AdxDecChannel *>(ws), n_channels, d_pcm, sa, st);
+    tick(5, false, st);
+    g_ctx.launches += sa.seg_count > 1 ? 3 : 1;
+    g_ctx.last_adx_dec = sa;
+    CUDA_TRY(cudaGetLastError());
+    return VGB_OK;
+}
+
+/* Synchronises `cuda_stream` and maps the status words the last vgb_adx_decode_dev on this workspace left: the lowest
+ * channel whose Fixed-type frame selects a filter 4..7 (IndexOutOfRangeException at CriAdxCodec.Coefs, :186-191). */
+int32_t vgb_adx_decode_dev_status(const void *d_workspace, int32_t n_channels, void *cuda_stream)
+{
+    if (n_channels <= 0) return VGB_OK;
+    if (!d_workspace) return fail(VGB_E_ARG, "NULL argument");
+    std::vector<int32_t> status(n_channels, 0);
+    VGB_TRY(adx_decode_words(d_workspace, n_channels, status.data(), static_cast<cudaStream_t>(cuda_stream)));
+    for (int c = 0; c < n_channels; c++)
+        if (status[c] & 1) return fail(VGB_E_DATA, "channel %d: a Fixed-type frame selects a filter outside 0..3", c);
+    return VGB_OK;
+}
+
+/* Bookkeeping of the most recent time-parallel ADX decode on this thread's context (see the header).  Synchronises
+ * the device. */
+int32_t vgb_adx_debug_decode_stats(uint64_t *out, int32_t n)
+{
+    if (!out || n < 0) return fail(VGB_E_ARG, "bad arguments");
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    for (int i = 0; i < n; i++) out[i] = 0;
+    if (!g_ctx.ready || !g_ctx.last_adx_dec.stats) return VGB_OK;
+    unsigned long long st[kAdxDecStatWords] = {};
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(st, g_ctx.last_adx_dec.stats, sizeof st, cudaMemcpyDeviceToHost));
+    if (n > 0) out[0] = (uint64_t)g_ctx.last_adx_dec.seg_count;
+    for (int i = 1; i < n && i <= kAdxDecStatWords; i++) out[i] = st[i - 1];
+    return VGB_OK;
 }
 
 }  // extern "C"

@@ -494,6 +494,293 @@ adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restric
     for (; current < sample_count; current++) dst[current] = 0;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// TIME-PARALLEL DECODING.  adx_decode_kernel runs one thread through a whole channel: right for many-channel batches,
+// ~100x too serial for one long stereo track.  The decoder is a state machine on (hist1, hist2), so the encoder's three
+// phases carry over with the frame-end pair as the only thing compared (AdxDecGeom names the frames):
+//   kAdxChain    thread = (channel, segment) over body frames: segment 0 decodes the head frame from the channel's history
+//                and runs on, the others start from (0, 0); output and every body frame's end pair (`trace`) are written
+//   kAdxRunOn    thread = (channel, boundary): from the previous segment's recorded end pair, decode on inside the segment
+//                until a frame-end pair equals the recorded one (from there the recorded output IS the true one)
+//   kAdxCascade  thread = channel: repairs, in order, every boundary whose start pair changed after its run-on read it
+//                (a run-on that never locked: digital silence keeps a wrong nonzero pair fixed under the >> 12), across
+//                segment ends if need be, then decodes the tail frame and zero-fills what no frame reaches
+// Exact by construction: a matching pair at the same frame means identical output from there on.  18-byte frames of a
+// row at a 16-byte aligned address read groups of 8 frames (144 B, 8-frame aligned in the row) through the cp.async ring;
+// the head, unaligned leftovers, other frame sizes and the tail take the per-byte loop, which reads only the bytes
+// CriAdxCodec.Decode reads.
+// ---------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void adx_fixed_coefs(uint32_t b0, int32_t &c0, int32_t &c1)  // CriAdxCodec.Coefs (:186-191)
+{
+    const int k = ((int)((b0 >> 4) & 0xF) >> 1) & 3;
+    c0 = k == 0 ? 0 : (k == 1 ? 0x0F00 : (k == 2 ? 0x1CC0 : 0x1880));
+    c1 = k == 0 ? 0 : (k == 1 ? 0 : (k == 2 ? (int16_t)0xF300 : (int16_t)0xF240));
+}
+
+// The filter number of a frame header (:26) indexes CriAdxCodec.Coefs, four rows, for the Fixed type and a one-row table
+// of the computed pair for every other type: status bit 0 for a Fixed filter 4..7, bit 1 for another type's filter 1..7
+// (both IndexOutOfRangeException in the reference)
+__device__ __forceinline__ uint32_t adx_filter_fault(uint32_t b0, int type)
+{
+    return type == 2 ? (b0 >> 7) & 1u : ((b0 & 0xE0u) ? 2u : 0u);
+}
+
+// One frame by the reference's loop (:24-51): header at byte fb of src, samples s in [start, to_read) to dst[0..).  A frame
+// that yields no sample never indexes the coefficient table, so its filter number is not checked.
+__device__ __forceinline__ void adx_dec_frame_general(const AdxDecChannel &c, const uint8_t *__restrict__ src, int64_t fb, int start,
+                                                      int to_read, int16_t *__restrict__ dst, int32_t &hist1, int32_t &hist2,
+                                                      uint32_t &bad_filter)
+{
+    const uint32_t b0 = src[fb], b1 = src[fb + 1];
+    int32_t c0 = c.coef0, c1 = c.coef1;
+    if (c.type == 2) adx_fixed_coefs(b0, c0, c1);
+    if (to_read > start) bad_filter |= adx_filter_fault(b0, c.type);  // coefs[filterNum] is indexed in the sample loop only
+    int32_t scale = (int16_t)(((b0 << 8) | b1) & 0x1FFF);
+    scale = (int16_t)(c.type == 4 ? (1 << ((12 - scale) & 31)) : scale + 1);
+    const bool v4 = c.version == 4;
+    for (int s = start; s < to_read; s++) {
+        const uint32_t byte = src[fb + 2 + s / 2];
+        int32_t sample = (s & 1) == 0 ? ((int32_t)(byte << 24) >> 28) : ((int32_t)(byte << 28) >> 28);
+        if (v4) sample = wadd(wmul(scale, sample), wadd(wmul(hist1, c0), wmul(hist2, c1)) >> 12);
+        else sample = wadd(wadd(wmul(scale, sample), wmul(hist1, c0) >> 12), wmul(hist2, c1) >> 12);
+        const int32_t out = clamp16(sample);
+        hist2 = hist1;
+        hist1 = out;
+        dst[s - start] = (int16_t)out;
+    }
+}
+
+// One 18-byte frame at byte `base` of an 8-frame group w[] (the arithmetic of adx_decode_kernel's fast path); o[]
+// receives the 32 samples as halfword pairs.
+template <bool kV4>
+__device__ __forceinline__ void adx_dec_frame_std(const uint32_t (&w)[36], int base, int32_t coef0, int32_t coef1, int type,
+                                                  int32_t &hist1, int32_t &hist2, uint32_t &bad_filter, uint32_t (&o)[16])
+{
+    auto byte_at = [&](int k) -> uint32_t { return (w[(base + k) >> 2] >> (((base + k) & 3) * 8)) & 0xFFu; };
+    const uint32_t b0 = byte_at(0), b1 = byte_at(1);
+    int32_t c0 = coef0, c1 = coef1;
+    if (type == 2) adx_fixed_coefs(b0, c0, c1);
+    bad_filter |= adx_filter_fault(b0, type);
+    int32_t scale = (int16_t)(((b0 << 8) | b1) & 0x1FFF);
+    scale = (int16_t)(type == 4 ? (1 << ((12 - scale) & 31)) : scale + 1);
+    const int32_t bias0 = wmul(-32768, c0), bias1 = wmul(-32768, c1);  // history biased by +32768: Clamp16 is one VIMNMX
+    int32_t hb1 = hist1 + 32768, hb2 = hist2 + 32768;
+#pragma unroll
+    for (int s2 = 0; s2 < 32; s2++) {
+        const int byte = base + 2 + (s2 >> 1);
+        const int lo_bit = (byte & 3) * 8 + ((s2 & 1) ? 0 : 4);
+        const int32_t q = (int32_t)(w[byte >> 2] << (28 - lo_bit)) >> 28;
+        const int32_t sq = adx_imad(scale, q, 32768);
+        int32_t biased;
+        if (kV4) {
+            const int32_t t = adx_imad(c1, hb2, wadd(bias0, bias1));
+            biased = wadd(adx_imad(c0, hb1, t) >> 12, sq);
+        } else {
+            const int32_t t = wadd(adx_imad(c1, hb2, bias1) >> 12, sq);
+            biased = wadd(adx_imad(c0, hb1, bias0) >> 12, t);
+        }
+        const int32_t ob = __viaddmin_s32_relu(biased, 0, 65535);
+        hb2 = hb1;
+        hb1 = ob;
+        if (s2 & 1) o[s2 >> 1] |= (uint32_t)ob << 16; else o[s2 >> 1] = (uint32_t)ob;
+    }
+#pragma unroll
+    for (int j = 0; j < 16; j++) o[j] ^= 0x80008000u;
+    hist1 = hb1 - 32768;
+    hist2 = hb2 - 32768;
+}
+
+__host__ __device__ __forceinline__ int adx_dec_seg_len(int body, int seg_count, int min_seg)
+{
+    const int per = (body + seg_count - 1) / seg_count;
+    return ((per > min_seg ? per : min_seg) + 7) & ~7;  // a multiple of 8: interior boundaries fall on 8-frame groups
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(kAdxThreads)
+adx_decode_seg_kernel(const uint8_t *__restrict__ adpcm, const AdxDecChannel *__restrict__ tab, int n_channels, int16_t *__restrict__ pcm,
+                      AdxDecSegArgs sa)
+{
+    __shared__ __align__(16) uint4 ring[kAdxStages][9][kAdxThreads];  // [stage][16-byte chunk of the group][thread]
+    const int ch = blockIdx.x * blockDim.x + threadIdx.x;
+    if (ch >= n_channels) return;
+    const AdxDecChannel c = tab[ch];
+    const uint8_t *src = adpcm + c.adpcm_off;
+    int16_t *dst = pcm + c.pcm_off;
+    const AdxDecGeom g = adx_dec_geom(c.n_samples, c.frame_size, c.padding);
+    const int seg_len = adx_dec_seg_len(g.body, sa.seg_count, sa.min_seg_frames);
+    const int a1 = (int)(g.in0 / c.frame_size) + 1;  // row frame of body frame 0
+    // boundary s >= 1 sits at body frame s * seg_len - (a1 & 7): a multiple of 8 in the row; the last segment runs to the end
+    auto seg_lo = [&](int s) { return s == 0 ? 0 : (s >= sa.seg_count ? g.body : min(g.body, s * seg_len - (a1 & 7))); };
+    // both paths are chosen from absolute addresses: the caller's base pointers need not be aligned beyond their type
+    const bool fast = c.frame_size == 18 && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
+    const int64_t out_pos = (int64_t)c.pcm_off + g.k0;  // body frame j writes samples out_pos + 32 j..
+    const uintptr_t out_addr = reinterpret_cast<uintptr_t>(pcm + out_pos);  // + 64 j keeps its alignment
+    const int store = (out_addr & 15) == 0 ? 16 : ((out_addr & 3) == 0 ? 4 : 2);  // widest store the output's alignment allows
+    uint32_t *trace = sa.trace + c.trace_off;
+    uint32_t bad_filter = 0;
+
+    // body frames [lo, hi) from (h1, h2); splice: stop after the first frame whose end pair equals the recorded one.
+    // Returns the number of frames decoded.
+    auto run = [&](int lo, int hi, int32_t &h1, int32_t &h2, bool splice) -> int {
+        int j = lo, done = 0;
+        auto finish = [&](int jj) -> bool {  // frame jj decoded: record its pair or stop at the recorded one
+            const uint32_t pair = ((uint32_t)h1 & 0xFFFFu) | ((uint32_t)h2 << 16);
+            done++;
+            if (splice && trace[jj] == pair) return true;
+            trace[jj] = pair;
+            return false;
+        };
+        auto general = [&](int jj) -> bool {
+            adx_dec_frame_general(c, src, g.in0 + (int64_t)(1 + jj) * c.frame_size, 0, g.spf, dst + g.k0 + (int64_t)jj * g.spf, h1, h2, bad_filter);
+            return finish(jj);
+        };
+        if (fast) {
+            const int jg = min(hi, lo + ((8 - ((a1 + lo) & 7)) & 7));  // first body frame at a multiple of 8 in the row
+            for (; j < jg; j++) if (general(j)) return done;
+            const int groups = (hi - j) / kAdxDecGroup;
+            const uint4 *vin = reinterpret_cast<const uint4 *>(src + (int64_t)(a1 + j) * 18);
+            auto issue = [&](int q) {
+                if (q < groups) {
+#pragma unroll
+                    for (int k = 0; k < 9; k++) cp_async16(&ring[q % kAdxStages][k][threadIdx.x], vin + (int64_t)q * 9 + k);
+                }
+                asm volatile("cp.async.commit_group;" ::: "memory");
+            };
+#pragma unroll
+            for (int q = 0; q < kAdxStages - 1; q++) issue(q);
+            bool stop = false;
+            for (int q = 0; q < groups && !stop; q++) {
+                issue(q + kAdxStages - 1);
+                asm volatile("cp.async.wait_group %0;" ::"n"(kAdxStages - 1) : "memory");
+                uint32_t w[36];
+#pragma unroll
+                for (int k = 0; k < 9; k++) {
+                    const uint4 v = ring[q % kAdxStages][k][threadIdx.x];
+                    w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+                }
+#pragma unroll
+                for (int fr = 0; fr < kAdxDecGroup; fr++) {
+                    uint32_t o[16];
+                    if (c.version == 4) adx_dec_frame_std<true>(w, 18 * fr, c.coef0, c.coef1, c.type, h1, h2, bad_filter, o);
+                    else adx_dec_frame_std<false>(w, 18 * fr, c.coef0, c.coef1, c.type, h1, h2, bad_filter, o);
+                    const int64_t at = out_pos + (int64_t)(j + fr) * 32;
+                    if (store == 16) {
+                        uint4 *v = reinterpret_cast<uint4 *>(pcm + at);
+#pragma unroll
+                        for (int k = 0; k < 4; k++) v[k] = make_uint4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
+                    } else if (store == 4) {
+                        uint32_t *v = reinterpret_cast<uint32_t *>(pcm + at);
+#pragma unroll
+                        for (int k = 0; k < 16; k++) v[k] = o[k];
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < 16; k++) { pcm[at + 2 * k] = (int16_t)(o[k] & 0xFFFFu); pcm[at + 2 * k + 1] = (int16_t)(o[k] >> 16); }
+                    }
+                    if (finish(j + fr)) { stop = true; break; }
+                }
+                j += kAdxDecGroup;
+            }
+            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            if (stop) return done;
+        }
+        for (; j < hi; j++) if (general(j)) return done;
+        return done;
+    };
+    // the tail frame from the true pair after the last body frame, then zeros where no frame reaches (:14,:31-33)
+    auto tail = [&](int32_t h1, int32_t h2) {
+        int64_t produced = g.k0 + (int64_t)g.body * g.spf;
+        if (g.frames > 1 + g.body) {
+            const int to_read = min(g.spf, c.n_samples - (int)produced);
+            adx_dec_frame_general(c, src, g.in0 + (int64_t)(1 + g.body) * c.frame_size, 0, to_read, dst + produced, h1, h2, bad_filter);
+            produced += max(to_read, 0);
+        }
+        for (int64_t s = produced; s < c.n_samples; s++) dst[s] = 0;
+    };
+    auto report = [&]() { if (bad_filter) atomicOr(&sa.status[ch], (int)bad_filter); };
+
+    if (kMode == kAdxChain) {
+        const int s = blockIdx.y;
+        const int lo = seg_lo(s), hi = seg_lo(s + 1);
+        if (s > 0 && lo >= hi) return;
+        int32_t h1 = 0, h2 = 0;  // a guess, for every segment but the first
+        if (s == 0) {
+            h1 = h2 = c.history;
+            if (g.frames > 0) adx_dec_frame_general(c, src, g.in0, g.start, min(g.spf, c.n_samples), dst, h1, h2, bad_filter);
+        }
+        run(lo, hi, h1, h2, false);
+        if (s == 0 && (sa.seg_count == 1 || g.body == 0)) tail(h1, h2);  // else the cascade decodes the tail from the true pair
+        report();
+        return;
+    }
+    if (kMode == kAdxRunOn) {
+        const int s = blockIdx.y + 1;
+        const int lo = seg_lo(s), hi = seg_lo(s + 1);
+        if (lo >= hi) return;
+        const uint32_t start = trace[lo - 1];
+        sa.used_start[(int64_t)ch * kAdxDecMaxSegments + s] = start;
+        int32_t h1 = (int32_t)(int16_t)(start & 0xFFFFu), h2 = (int32_t)(int16_t)(start >> 16);
+        const int done = run(lo, hi, h1, h2, true);
+        atomicAdd(&sa.stats[0], (unsigned long long)done);
+        atomicMax(&sa.stats[3], (unsigned long long)done);
+        return;
+    }
+    // cascade: one thread per channel walks the boundaries in order
+    int truth_upto = 0;
+    for (int s = 1; s < sa.seg_count; s++) {
+        const int lo = seg_lo(s);
+        if (lo >= g.body) break;
+        if (lo < truth_upto) continue;
+        const uint32_t start = trace[lo - 1];
+        if (start == sa.used_start[(int64_t)ch * kAdxDecMaxSegments + s]) continue;
+        int32_t h1 = (int32_t)(int16_t)(start & 0xFFFFu), h2 = (int32_t)(int16_t)(start >> 16);
+        const int done = run(lo, g.body, h1, h2, true);
+        truth_upto = lo + done;
+        atomicAdd(&sa.stats[1], (unsigned long long)done);
+        atomicAdd(&sa.stats[2], 1ull);
+    }
+    if (g.body == 0) return;  // segment 0's chain decoded the whole channel
+    const uint32_t last = trace[g.body - 1];
+    tail((int32_t)(int16_t)(last & 0xFFFFu), (int32_t)(int16_t)(last >> 16));
+    report();
+}
+
+// Segments per channel of the time-parallel ADX decode: about four waves of threads over the SMs, no segment shorter
+// than the minimum (VGB_ADX_DEC_SEGMENTS / VGB_ADX_DEC_MIN_SEG_FRAMES override both).
+int adx_decode_pick_segments(int n_channels, int max_body_frames, int *min_seg_out)
+{
+    int min_seg = kAdxDecMinSegFrames;
+    if (const char *env = std::getenv("VGB_ADX_DEC_MIN_SEG_FRAMES")) {
+        const int v = std::atoi(env);
+        if (v >= 1) min_seg = v;
+    }
+    if (min_seg_out) *min_seg_out = min_seg;
+    if (const char *env = std::getenv("VGB_ADX_DEC_SEGMENTS")) {
+        const int v = std::atoi(env);
+        if (v >= 1) return std::min(v, kAdxDecMaxSegments);
+    }
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) {
+        (void)cudaGetLastError();
+        sms = 132;  // H100 SXM
+    }
+    const long long want = (4ll * sms * 512 + n_channels - 1) / std::max(n_channels, 1);
+    const int max_s = std::max(1, std::min(kAdxDecMaxSegments, max_body_frames / min_seg));
+    return (int)std::max<long long>(1, std::min<long long>(want, max_s));
+}
+
+void launch_adx_decode_seg(const uint8_t *adpcm, const AdxDecChannel *tab, int n_channels, int16_t *pcm, AdxDecSegArgs sa, cudaStream_t stream)
+{
+    if (n_channels <= 0) return;
+    const int blocks = (n_channels + kAdxThreads - 1) / kAdxThreads;
+    adx_decode_seg_kernel<kAdxChain><<<dim3(blocks, sa.seg_count), kAdxThreads, 0, stream>>>(adpcm, tab, n_channels, pcm, sa);
+    if (sa.seg_count > 1) {
+        adx_decode_seg_kernel<kAdxRunOn><<<dim3(blocks, sa.seg_count - 1), kAdxThreads, 0, stream>>>(adpcm, tab, n_channels, pcm, sa);
+        adx_decode_seg_kernel<kAdxCascade><<<dim3(blocks, 1), kAdxThreads, 0, stream>>>(adpcm, tab, n_channels, pcm, sa);
+    }
+}
+
 // Segments per channel of the time-parallel ADX encode: thread-per-item kernels want every SM full of threads
 // (~512 resident per SM at this register count), the run-on at a boundary is a handful of frames.
 // Shortest segment in frames.  Measured with the oracle on the synthetic set: a chain started from raw history meets the

@@ -107,6 +107,48 @@ struct AdxSegArgs {
     int32_t min_seg_frames;
 };
 
+// Time-parallel ADX decoding (adx.cu, the adx_decode_seg_kernel family).  CriAdxCodec.Decode (:9-54) walks frames
+// 0..frames-1 from byte (padding / spf) * frame_size: the HEAD frame 0 yields samples start..min(spf, n)-1 of its frame
+// (k0 of them), every BODY frame after it all spf samples, and at most one TAIL frame the rest; samples no frame reaches
+// stay 0.  Only body frames are cut into segments.
+struct AdxDecGeom {
+    int32_t spf, start, frames, k0, body;
+    int64_t in0;  // byte of the head frame in the channel's row
+};
+__host__ __device__ __forceinline__ AdxDecGeom adx_dec_geom(int32_t n, int32_t frame_size, int32_t padding)
+{
+    AdxDecGeom g;
+    g.spf = (frame_size - 2) * 2;
+    g.start = padding > 0 ? padding % g.spf : 0;                                      // :21
+    g.in0 = (int64_t)(padding / g.spf) * frame_size;                                  // :22
+    g.frames = n > 0 ? div_round_up(n, g.spf) : 0;                                    // :19
+    const int32_t k0 = (n < g.spf ? n : g.spf) - g.start;
+    g.k0 = g.frames > 0 && k0 > 0 ? k0 : 0;
+    const int32_t full = 1 + (n - g.k0) / g.spf;                                      // head + whole frames after it
+    g.body = g.frames > 0 ? (full < g.frames ? full : g.frames) - 1 : 0;
+    return g;
+}
+struct AdxDecChannel {
+    int64_t pcm_off;     // sample offset of the channel's output
+    int64_t adpcm_off;   // byte offset of the channel's row (the fast path wants a multiple of 16)
+    int64_t trace_off;   // first word of the channel in the trace slab (one word per body frame)
+    int32_t n_samples, frame_size, version, padding, type;
+    int32_t history;     // initial hist1 = hist2 (:16-17)
+    int16_t coef0, coef1;  // CalculateCoefficients (Linear / Exponential; Fixed frames pick their own)
+};
+constexpr int kAdxDecMinSegFrames = 512;  // run-ons measured at p99 62 / max 101 frames; VGB_ADX_DEC_MIN_SEG_FRAMES overrides
+constexpr int kAdxDecMaxSegments = 256;
+constexpr int kAdxDecStatWords = 4;
+struct AdxDecSegArgs {
+    uint32_t *trace;             // [trace_off[ch] + body frame] the pair (hist1 & 0xffff) | hist2 << 16 after the frame
+    uint32_t *used_start;        // [ch][kAdxDecMaxSegments] the pair a boundary's run-on started from
+    unsigned long long *stats;   // [0] frames decoded by run-ons, [1] by the cascade, [2] boundaries the cascade repaired,
+                                 // [3] longest run-on
+    int32_t *status;             // [ch] bit 0: a Fixed-type frame selects a filter 4..7, bit 1: another type's frame a filter 1..7
+    int32_t seg_count;
+    int32_t min_seg_frames;
+};
+
 // ---- CRI HCA ------------------------------------------------------------------------------------------------
 // per-stream status codes the encoder kernel can raise (mapped to the reference's exceptions by the C ABI)
 constexpr int32_t VGB_HCA_BITRATE_TOO_LOW = 1;   // InvalidDataException("Bitrate is set too low.") CriHcaEncoder.cs:469-472

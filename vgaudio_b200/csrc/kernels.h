@@ -51,6 +51,10 @@ void launch_adx_encode(const int16_t *pcm, const AdxChannel *tab, int n_channels
                        AdxSegArgs seg, cudaStream_t stream);  // seg.trace == nullptr: one segment (plain serial encode)
 void launch_adx_decode(const uint8_t *adpcm, const AdxChannel *tab, int n_channels, int16_t *pcm, int32_t *status,
                        cudaStream_t stream);  // status: lowest channel with a fixed-filter number 4..7 (atomicMin), may be null
+// the time-parallel decode (chain / run-on / cascade); seg.status, seg.stats and the trace live in the caller's workspace
+int adx_decode_pick_segments(int n_channels, int max_body_frames, int *min_seg_out);
+void launch_adx_decode_seg(const uint8_t *adpcm, const AdxDecChannel *tab, int n_channels, int16_t *pcm, AdxDecSegArgs seg,
+                           cudaStream_t stream);
 
 // hca.cu — CriHcaEncoder.EncodeFrame + CriHcaPacking.PackFrame (Codecs/CriHca/CriHcaEncoder.cs:271-286)
 size_t hca_encode_smem_bytes(const HcaConfig &cfg);
