@@ -93,6 +93,9 @@ namespace VGAudio.Native
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_wave_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, long* outSizes,
             byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_transcode_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
+            VgbAdxKey* inAdxKey, ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
     }
 }
 
@@ -278,6 +281,61 @@ namespace VGAudio.Cli
                         File.WriteAllBytes(outPaths[i], outputs[i]);
                     }
                     reportAdd(1);
+                }
+            }
+            finally
+            {
+                foreach (var h in inPins) h.Free();
+                foreach (var h in outPins) h.Free();
+            }
+        }
+
+        // Coded files in, another codec out (`-b -i adx/ --out-format hca` and the like): per file the source's reader,
+        // ToPcm16 and the target's encoder and writer from the options (Convert.ConvertFile with KeepConfiguration false),
+        // decoded and re-encoded on the device in one native call per pass.  inTypes[i] is VGB_CONTAINER_DSP / _ADX / _HCA
+        // (1 / 2 / 3) for file i; a file already in options.OutType's codec fails alone (no rewrite is performed).
+        // inAdxKey decrypts revision 8 / 9 .adx sources and inHcaKeyCode "ciph" 56 .hca sources; the output's key is in
+        // options.  A file whose frames the decoder refuses fails in the second pass alone.
+        public static unsafe void Transcode(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
+            ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd)
+        {
+            int n = inPaths.Length;
+            byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
+            var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            var outPins = new List<GCHandle>();
+            try
+            {
+                byte** inPtr = stackalloc byte*[n];
+                byte** outPtr = stackalloc byte*[n];
+                long* len = stackalloc long[n];
+                long* outSize = stackalloc long[n];
+                int* status = stackalloc int[n];
+                VgbAdxKey k = inAdxKey ?? default;
+                VgbAdxKey* keyPtr = inAdxKey.HasValue ? &k : null;
+                ulong code = inHcaKeyCode ?? 0;
+                ulong* codePtr = inHcaKeyCode.HasValue ? &code : null;
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
+                fixed (int* types = inTypes)
+                {
+                    VgAudioB200.Check(VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero));
+                    var outputs = new byte[n][];
+                    for (int i = 0; i < n; i++)
+                    {
+                        outPtr[i] = null;
+                        if (status[i] != VgAudioB200.Ok) continue;
+                        outputs[i] = new byte[outSize[i]];
+                        outPins.Add(GCHandle.Alloc(outputs[i], GCHandleType.Pinned));
+                        outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
+                    }
+                    VgbProgress cb = (user, delta) => reportAdd((int)delta);   // progress.ReportAdd(1) per file (Batch.cs:45)
+                    VgAudioB200.Check(VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero));
+                    GC.KeepAlive(cb);
+                    for (int i = 0; i < n; i++)
+                    {
+                        if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); continue; }   // Batch.cs:39-43
+                        Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
+                        File.WriteAllBytes(outPaths[i], outputs[i]);
+                    }
                 }
             }
             finally

@@ -638,6 +638,27 @@ int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t
  * status_out NULL such a file fails the call (VGB_E_DATA) after every other file has been written. */
 int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_adx_key *key,
                                       int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* Transcoding in the batch job: .dsp, .adx and .hca file images in, another of the three out (Convert.ConvertFile with a
+ * coded source: the source's reader, a fresh configuration from the options, source.ToPcm16() -> EncodeFromPcm16).
+ * in_type[i] (VGB_CONTAINER_*) names file i's codec: a .dsp file has no signature.  options->out_type, its options and
+ * its key describe the output exactly as for vgb_convert_wave_batch; options->group_bytes counts DECODED PCM bytes per
+ * GPU batch (0: an eighth of the job's PCM, 64..512 MiB; a batch holds at most 4096 files).  The sources are read as by vgb_convert_{dsp,adx,hca}_to_wave_batch:
+ * the PCM, loop points and rate their ToPcm16 yields (.adx: sample_count - inserted_samples samples, loop points shifted;
+ * .hca: trimmed at the loop end; .dsp: from the header's start history), and their keys: *in_adx_key decrypts revision 8
+ * and 9 .adx files, *in_hca_key_code "ciph" 56 .hca files, "ciph" 1 uses the built-in table; a keyed source without its
+ * key fails alone, keys are never applied to other revisions and there is no key search.  No PCM leaves the device:
+ * per batch one H2D of the coded regions, the source's decode straight into the encoder's channel rows, encode and file
+ * assembly, one D2H of the finished files.  Same two-pass protocol, per-file status, progress and sharding (files weigh
+ * sample_count * channel_count + 1024) as vgb_convert_wave_batch.
+ * Per-file errors of the sizing pass, each failing that file only: in_type not DSP / ADX / HCA, or equal to out_type
+ * (a rewrite in the source's own codec is not performed), the source's parse and planning errors (as its -> WAVE
+ * converter, without the WAVE writer's limits), and the target's planning errors (as vgb_convert_wave_batch).
+ * In the fill pass, an ADX frame with a filter the reference cannot index or an HCA frame the decoder refuses fails that
+ * file alone (status_out entry, out_sizes[i] = 0, buffer not written; without status_out the call fails with VGB_E_DATA
+ * after the other files are written), a GC-ADPCM predictor outside 0..7 fails the call (VGB_E_DATA). */
+int32_t vgb_transcode_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                            const vgb_convert_options *options, const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code,
+                            int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
 /* Measurement tap: device time of the most recent vgb_convert_wave_batch summed over its (first 32) batches per device,
  * over every device that converted part of it, out[0..3] = WAVE split, encode, loop-context decode, file assembly (ms,
  * CUDA events on the kernel streams); returns the number of batches timed on all devices together. */

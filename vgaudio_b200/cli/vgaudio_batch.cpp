@@ -1,14 +1,20 @@
-// vgaudio_batch — batch conversion of a directory of WAVE files to .dsp / .adx / .hca on the GPU.
+// vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
+// .dsp / .adx / .hca, and .dsp, .adx and .hca files to WAVE.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
-// WaveReader -> encoder -> writer chain of a chunk of files runs as ONE coalesced call on the device
-// (vgb_convert_wave_batch).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
+// reader -> encoder -> writer chain of a chunk of files runs as ONE coalesced call on the device per kind of input
+// (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch for coded files, vgb_convert_*_to_wave_batch for
+// --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp, .hca and .adx inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
-//                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--adxtype Linear|Fixed|Exp|ExpEnc...]
-//                 [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
+//                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
+//                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
+// With --out-format dsp|adx|hca the inputs are the .wav / .wave files and the .dsp, .adx and .hca files in another codec
+// than the output's (a file already in the output's codec is not listed: the same codec would be a rewrite).
+// --keycode / --keystring are the output's key; --in-keycode N is the key of type-56 .hca inputs, and --in-keystring S,
+// or else --in-keycode N, the CriAdxKey of type-8 / type-9 .adx inputs.
 // With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
 // --keycode N, the CriAdxKey of type-8 / type-9 .adx files; there is no list of known keys.
 // --devices 0,1,2,3 binds those CUDA devices (vgb_init_devices): every chunk of files is then sharded over them, one
@@ -40,19 +46,20 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
     return n == 0 || (bool)f.read(reinterpret_cast<char *>(out.data()), n);
 }
 
-// which decoder takes an input of the decode direction: 0 .dsp, 1 .hca, 2 .adx
-static int decoder_of(const fs::path &p)
+// the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, -1 none of them
+static int kind_of(const fs::path &p)
 {
     std::string ext = p.extension().string();
     std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
-    return ext == ".hca" ? 1 : ext == ".adx" ? 2 : 0;
+    return ext == ".dsp" ? 0 : ext == ".hca" ? 1 : ext == ".adx" ? 2 : (ext == ".wav" || ext == ".wave") ? 3 : -1;
 }
+static const int32_t kContainerOfKind[3] = {VGB_CONTAINER_DSP, VGB_CONTAINER_HCA, VGB_CONTAINER_ADX};
 
 static int usage()
 {
     std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
-                         "                     [--limit-bitrate] [--keycode N] [--keystring S] [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4]\n"
-                         "                     [--chunk-mb N] [--devices LIST]\n");
+                         "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
+                         "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n");
     return 2;
 }
 
@@ -74,9 +81,9 @@ static bool parse_devices(const std::string &list, std::vector<int32_t> &out)
 
 int main(int argc, char **argv)
 {
-    std::string in_dir, out_dir, fmt, key_string;
-    bool recurse = false, have_code = false;
-    uint64_t key_code = 0;
+    std::string in_dir, out_dir, fmt, key_string, in_key_string;
+    bool recurse = false, have_code = false, have_in_code = false;
+    uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
     std::vector<int32_t> devices;  // empty: device 0 through vgb_init
     vgb_convert_options opt{};
@@ -93,6 +100,8 @@ int main(int argc, char **argv)
         else if (a == "--limit-bitrate") opt.hca_limit_bitrate = 1;
         else if (a == "--keycode") { key_code = std::strtoull(next(), nullptr, 0); have_code = true; }
         else if (a == "--keystring") key_string = next();
+        else if (a == "--in-keycode") { in_key_code = std::strtoull(next(), nullptr, 0); have_in_code = true; }
+        else if (a == "--in-keystring") in_key_string = next();
         else if (a == "--framesize") opt.adx_frame_size = std::atoi(next());
         else if (a == "--version") opt.adx_version = std::atoi(next());
         else if (a == "--chunk-mb") chunk_mb = (size_t)std::atoll(next());
@@ -124,15 +133,23 @@ int main(int argc, char **argv)
         opt.adx_encryption_type = !key_string.empty() ? 8 : 9;  // CreateConfiguration.cs:126-135: key strings are type 8, key codes type 9
     }
     if (opt.out_type == VGB_CONTAINER_HCA && have_code) { opt.hca_key_type = 56; opt.hca_key_code = key_code; }
+    // the keys of coded inputs that are transcoded: --in-keystring, or else --in-keycode, for .adx; --in-keycode for .hca
+    vgb_adx_key in_adx_key{};
+    const bool have_in_adx_key = !to_wave && (have_in_code || !in_key_string.empty());
+    if (have_in_adx_key) {
+        const int32_t s = !in_key_string.empty() ? vgb_adx_key_from_string(in_key_string.c_str(), &in_adx_key) : vgb_adx_key_from_code(in_key_code, &in_adx_key);
+        if (s != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
+    }
 
-    // Batch.cs:16-19: the files of the input directory (here: the WAVE ones, or the .dsp, .hca and .adx ones when decoding)
+    // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca and .adx ones when decoding; else the WAVE
+    // ones and the coded ones in another codec than the output's)
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
         if (!e.is_regular_file()) return;
-        std::string ext = e.path().extension().string();
-        std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
-        if (to_wave ? (ext == ".dsp" || ext == ".hca" || ext == ".adx") : (ext == ".wav" || ext == ".wave")) files.push_back(e.path());
+        const int kind = kind_of(e.path());
+        if (kind < 0) return;
+        if (to_wave ? kind < 3 : (kind == 3 || kContainerOfKind[kind] != opt.out_type)) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -159,24 +176,35 @@ int main(int argc, char **argv)
         std::vector<int64_t> len(n), out_size(n);
         std::vector<int32_t> status(n);
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
-        // decoding: the chunk's .dsp, .hca and .adx files go to their own converters, each on its rows of the chunk's tables
-        std::vector<int32_t> rows[3];
-        for (int k = 0; k < n; k++) rows[to_wave ? decoder_of(files[first + k]) : 0].push_back(k);
+        // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
+        // codec; encoding, the WAVE converter for WAVE files and one transcode call for the coded ones
+        std::vector<int32_t> rows[4];
+        for (int k = 0; k < n; k++) {
+            const int kind = kind_of(files[first + k]);
+            rows[to_wave ? kind : (kind == 3 ? 3 : 0)].push_back(k);
+        }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
-            if (!to_wave) return vgb_convert_wave_batch(ptr.data(), len.data(), n, &opt, out_size.data(), outs, status.data(), nullptr, nullptr);
-            for (int h = 0; h < 3; h++) {
+            for (int h = 0; h < 4; h++) {
                 const std::vector<int32_t> &r = rows[h];
                 if (r.empty()) continue;
                 std::vector<const uint8_t *> p;
                 std::vector<int64_t> l, sz(r.size());
                 std::vector<uint8_t *> o;
-                std::vector<int32_t> st(r.size());
-                for (int32_t k : r) { p.push_back(ptr[k]); l.push_back(len[k]); o.push_back(outs ? outs[k] : nullptr); }
+                std::vector<int32_t> st(r.size()), types;
+                for (int32_t k : r) {
+                    p.push_back(ptr[k]); l.push_back(len[k]); o.push_back(outs ? outs[k] : nullptr);
+                    const int kind = kind_of(files[first + k]);
+                    if (kind < 3) types.push_back(kContainerOfKind[kind]);
+                }
                 const int32_t m = (int32_t)r.size();
                 uint8_t *const *ot = outs ? o.data() : nullptr;
-                const int32_t s = h == 2 ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, have_adx_key ? &adx_key : nullptr, sz.data(), ot, st.data())
-                                : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
-                                         : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());
+                int32_t s;
+                if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
+                else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, have_in_adx_key ? &in_adx_key : nullptr,
+                                                           have_in_code ? &in_key_code : nullptr, sz.data(), ot, st.data(), nullptr, nullptr);
+                else s = h == 2 ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, have_adx_key ? &adx_key : nullptr, sz.data(), ot, st.data())
+                       : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
+                                : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());
                 if (s != VGB_OK) return s;
                 for (int32_t j = 0; j < m; j++) { out_size[r[j]] = sz[j]; status[r[j]] = st[j]; }
             }

@@ -295,3 +295,17 @@ def convert_adx_to_wave_batch(files: Sequence, key: Optional[N.VgbAdxKey] = None
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_adx_to_wave_batch(
         ftab, lens, n, C.byref(key) if key is not None else None, sizes, otab, st), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def transcode_batch(files: Sequence, in_types: Sequence[int], options: N.VgbConvertOptions, adx_key: Optional[N.VgbAdxKey] = None,
+                    hca_key_code: Optional[int] = None, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """.dsp / .adx / .hca images in (in_types: CONTAINER_* per file), options.out_type out, decoded and re-encoded on the
+    device: ([output file bytes or None], [per-file status]).  adx_key (from adx_key) decrypts revision 8 / 9 .adx
+    sources, hca_key_code "ciph" 56 .hca sources; the output's key is in options."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    code = C.c_uint64(hca_key_code) if hca_key_code is not None else None
+    cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_transcode_batch(
+        ftab, lens, types, n, C.byref(options), C.byref(adx_key) if adx_key is not None else None,
+        C.byref(code) if code is not None else None, sizes, otab, st, cb if otab is not None else None, None), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames

@@ -121,6 +121,10 @@ int32_t hca_decode_check(const vgb_hca_info *info, int32_t n_streams);  // VGB_E
 int32_t hca_decode_fault(int32_t status, const char *what, int index);  // a decoder status word as the reference's exception
 // synchronises `st` and copies the status words of the last vgb_hca_decode_dev on `d_workspace` to status[0..n)
 int32_t hca_decode_words(const void *d_workspace, int32_t n_streams, int32_t *status, cudaStream_t st);
+// the same for the encoder's status words of the last vgb_hca_encode_dev on `d_workspace`, and one such word as the
+// reference's exception ("<what> <index>: Bitrate is set too low." ...)
+int32_t hca_encode_words(const void *d_workspace, int32_t n_streams, int32_t *status, cudaStream_t st);
+int32_t hca_encode_fault(int32_t status, const char *what, int index);
 // abi_adx.cu: synchronises `st` and copies the per-channel status words of the last vgb_adx_decode_dev on `d_workspace`
 // (bit 0: a Fixed-type frame selects a filter 4..7, bit 1: a frame of another type a filter 1..7) to status[0..n)
 int32_t adx_decode_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st);

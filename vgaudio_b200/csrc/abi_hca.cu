@@ -237,18 +237,35 @@ HcaStream hca_encode_stream(const vgb_hca_info &h, const HcaVirtual &v, int64_t 
     return t;
 }
 
+}  // namespace
+
+int32_t vgb::hca_encode_fault(int32_t status, const char *what, int index)
+{
+    if (status == VGB_HCA_BITRATE_TOO_LOW) return fail(VGB_E_DATA, "%s %d: Bitrate is set too low.", what, index);
+    if (status == VGB_HCA_NOT_IMPLEMENTED) return fail(VGB_E_STATE, "%s %d: evaluation boundary search failed (NotImplementedException in the reference)", what, index);
+    if (status == VGB_HCA_BIT_OVERFLOW) return fail(VGB_E_STATE, "%s %d: Not enough bits left in output buffer", what, index);
+    return VGB_OK;
+}
+
+namespace {
+
 // The encoder's per-stream status words as the reference's exceptions
 int32_t hca_encode_status(const std::vector<int32_t> &status)
 {
-    for (int s = 0; s < (int)status.size(); s++) {
-        if (status[s] == VGB_HCA_BITRATE_TOO_LOW) return fail(VGB_E_DATA, "stream %d: Bitrate is set too low.", s);
-        if (status[s] == VGB_HCA_NOT_IMPLEMENTED) return fail(VGB_E_STATE, "stream %d: evaluation boundary search failed (NotImplementedException in the reference)", s);
-        if (status[s] == VGB_HCA_BIT_OVERFLOW) return fail(VGB_E_STATE, "stream %d: Not enough bits left in output buffer", s);
-    }
+    for (int s = 0; s < (int)status.size(); s++) VGB_TRY(hca_encode_fault(status[s], "stream", s));
     return VGB_OK;
 }
 
 }  // namespace
+
+int32_t vgb::hca_encode_words(const void *d_workspace, int32_t n_streams, int32_t *status, cudaStream_t st)
+{
+    const size_t o_status = align_up((size_t)n_streams * sizeof(HcaStream), 256);
+    CUDA_TRY(cudaMemcpyAsync(status, static_cast<const char *>(d_workspace) + o_status, (size_t)n_streams * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return VGB_OK;
+}
+
 
 // One-time upload of the codec tables (per process/device).  Trig tables: Mdct.GenerateTrigTables (Mdct.cs:183-195)
 // with the host libm, exactly as the oracle builds them; dead zones: CriHcaTables.QuantizerDeadZoneFunction (:68-78).
@@ -594,10 +611,7 @@ int32_t vgb_hca_encode_dev_status(const void *d_workspace, int32_t n_streams, vo
     if (n_streams <= 0) return VGB_OK;
     if (!d_workspace) return fail(VGB_E_ARG, "NULL argument");
     std::vector<int32_t> status(n_streams, 0);
-    const size_t o_status = align_up((size_t)n_streams * sizeof(HcaStream), 256);
-    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    CUDA_TRY(cudaMemcpyAsync(status.data(), static_cast<const char *>(d_workspace) + o_status, (size_t)n_streams * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    VGB_TRY(hca_encode_words(d_workspace, n_streams, status.data(), static_cast<cudaStream_t>(cuda_stream)));
     return hca_encode_status(status);
 }
 

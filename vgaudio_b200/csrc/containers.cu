@@ -15,6 +15,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstdio>
+#include <deque>
 
 #include "abi.cuh"
 
@@ -351,6 +352,24 @@ __global__ void __launch_bounds__(256) adx_assemble_kernel(const AdxFile *__rest
     }
 }
 
+// AdxWriter's version-4 history block (AdxWriter.cs:99-100): each channel's History, big-endian and twice, taken from the
+// encoder's write-back (CriAdxCodec.cs:69-74) on the device; runs behind adx_assemble_kernel and patches the finished
+// headers.  Thread = channel row.
+struct AdxHistPatch {
+    int64_t at;     // byte offset of the row's pair in the output slab
+    int32_t bytes;  // how many of its 4 bytes the header keeps: the "(c)CRI" at header_size - 2 overwrites the rest, and
+                    // a non-looping file's 36-byte header has no room for more than two channels' pairs (0: version 3)
+    int32_t pad;
+};
+__global__ void adx_history_kernel(const AdxHistPatch *__restrict__ patch, const int16_t *__restrict__ history, int n_rows, uint8_t *__restrict__ out)
+{
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_rows) return;
+    const AdxHistPatch p = patch[r];
+    const uint32_t h = (uint16_t)history[r];
+    for (int j = 0; j < p.bytes; j++) out[p.at + j] = (uint8_t)((j & 1) ? h : h >> 8);
+}
+
 // in-place EncryptDecrypt over channel rows (CriAdxEncryption.cs:8-44): thread = (frame, channel)
 __global__ void adx_crypt_kernel(uint8_t *__restrict__ adpcm, const int64_t *__restrict__ row_off, int channels, int frames, int frame_size,
                                  int row_len, int seed, int mult, int inc, int enc_type)
@@ -467,6 +486,9 @@ struct ContainerState {
     cudaEvent_t ev_in[kWays] = {}, ev_split[kWays] = {}, ev_k[kWays] = {}, ev_out[kWays] = {};
     // working set 0 doubles as the single-shot entry points' and the .dsp -> WAVE converter's
     DevBuf in[kWays], out[kWays], tab[kWays], pcms[kWays], encs[kWays], decs[kWays], coefss[kWays], wss[kWays];
+    // vgb_transcode_batch's source side: de-interleaved coded rows and the decoder's workspace, whose status words are
+    // read after the next group is enqueued, so no encoder may reuse it before then
+    DevBuf srcs[kWays], dws[kWays];
     // stage timers of the batch converter: per group 5 events (start, split done, encode done, context done, assembled)
     static constexpr int kTimedGroups = 32, kStageEvents = 5;
     cudaEvent_t stage[kTimedGroups][kStageEvents] = {};
@@ -750,6 +772,7 @@ void containers_release(Context &c)  // vgb_shutdown, once per bound context
             for (int i = 0; i < kWays; i++) {
                 s->in[i].release(); s->out[i].release(); s->tab[i].release();
                 s->pcms[i].release(); s->encs[i].release(); s->decs[i].release(); s->coefss[i].release(); s->wss[i].release();
+                s->srcs[i].release(); s->dws[i].release();
                 cudaEventDestroy(s->ev_in[i]); cudaEventDestroy(s->ev_split[i]); cudaEventDestroy(s->ev_k[i]); cudaEventDestroy(s->ev_out[i]);
                 cudaStreamDestroy(s->s_kern[i]);
             }
