@@ -137,8 +137,9 @@ int32_t vgb_gcadpcm_encode_batch(const int16_t *const *pcm, const int32_t *n_sam
  * -> GcAdpcmDecoder.Decode, GcAdpcmDecoder.cs:10-54).  n_bytes[c] is the length of adpcm[c]; params[c].sample_count
  * == -1 decodes ByteCountToSampleCount(n_bytes[c]) samples.  pcm_out[c] receives sample_count samples.
  * VGB_E_DATA: a frame header selects a predictor outside 0..7 (IndexOutOfRangeException at GcAdpcmDecoder.cs:31-32);
- * the message names the lowest such channel.  The device-resident variant below cannot report it without a
- * synchronisation: there the lookup wraps (predictor & 7). */
+ * the message names the lowest such channel.  The device-resident variant below decodes such a frame with the lookup
+ * wrapped (predictor & 7) and leaves the lowest such channel in its workspace, where vgb_gcadpcm_decode_dev_status
+ * reports it. */
 int32_t vgb_gcadpcm_decode_batch(const uint8_t *const *adpcm, const int32_t *n_bytes, const int16_t *coefs,
                                  const vgb_gc_params *params, int32_t n_channels, int16_t *const *pcm_out);
 
@@ -156,6 +157,9 @@ int32_t vgb_gcadpcm_encode_frames(int16_t *pcm_in_out, const int32_t *sample_cou
  * The offset/length tables are HOST arrays (they are tiny and are uploaded on `stream`); both slabs must be
  * padded so that each channel's region is readable/writable up to the next multiple of 16 bytes.
  * vgb_gcadpcm_workspace_bytes() tells how much scratch HBM the call needs for the given total frame count.
+ * Base pointers: d_pcm, d_adpcm and d_workspace must be 16-byte aligned, d_coefs_in / d_coefs_out / d_coefs 2-byte
+ * aligned (the kernels read and write them with 16-byte vector and cp.async accesses); VGB_E_ARG otherwise, before any
+ * device work.
  * ------------------------------------------------------------------------------------------------------- */
 uint64_t vgb_gcadpcm_workspace_bytes(int64_t total_frames, int32_t n_channels);
 
@@ -271,8 +275,9 @@ int32_t vgb_debug_last_coefs_done(float *ms_out, int32_t n);
  * boundary does not re-lock inside its segment), out[3] boundaries the cascade had to repair, out[4] the longest
  * run-on in frames, out[5 + b] the number of run-ons of 2^b .. 2^(b+1)-1 frames (b = 0..13, the last one open).  n = how
  * many words to fill (up to 19).  bench.py reports (out[1] + out[2]) / frames as `fallback_frames_frac`.  Synchronises
- * the device.  VGB_GC_SEGMENTS=<n> in the environment forces the segment count (1 = the plain serial loop of
- * GcAdpcmEncoder.cs:30-43). */
+ * the device.  The words live in the workspace of that launch: after a vgb_gcadpcm_encode_dev the caller's workspace
+ * must still be allocated (and not yet reused) when this is called.  VGB_GC_SEGMENTS=<n> in the environment forces the
+ * segment count (1 = the plain serial loop of GcAdpcmEncoder.cs:30-43). */
 int32_t vgb_gcadpcm_debug_splice_stats(uint64_t *out, int32_t n);
 
 /* Debug/test taps (tests/ only): run coefficient phase 1 and return, per frame, the direct-form pair and the
@@ -320,8 +325,9 @@ int32_t vgb_adx_encode_batch(const int16_t *const *pcm, const int32_t *n_samples
 /* Device-resident variant of vgb_adx_encode_batch (same semantics, asynchronous on `cuda_stream`): d_pcm / d_adpcm are HBM
  * slabs, channel c at pcm_offset[c] samples (a multiple of 8) / adpcm_offset[c] bytes (even); d_history_out ([n] shorts)
  * may be NULL; d_workspace holds the channel table and the bookkeeping of the time-parallel encoder (one word per
- * 32-sample frame; vgb_adx_workspace_bytes(total samples, channels)).  The multi-GPU batch path and bench.py's
- * device-resident figures use it. */
+ * 32-sample frame; vgb_adx_workspace_bytes(total samples, channels)).  d_pcm must be 16-byte aligned (the encoder
+ * copies it with cp.async), d_adpcm and d_history_out 2-byte aligned, d_workspace 8-byte aligned; VGB_E_ARG otherwise.
+ * The multi-GPU batch path and bench.py's device-resident figures use it. */
 uint64_t vgb_adx_workspace_bytes(int64_t total_samples, int32_t n_channels);
 int32_t vgb_adx_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, const int32_t *n_samples, const vgb_adx_params *params,
                            int32_t n_channels, int16_t *d_history_out, uint8_t *d_adpcm, const int64_t *adpcm_offset,
@@ -401,7 +407,8 @@ int32_t vgb_hca_encode_batch(const int16_t *const *pcm, const vgb_hca_params *pa
 /* Device-resident variant of vgb_hca_encode_batch (asynchronous on `cuda_stream`): channel c of stream s starts at
  * pcm_offset[s] + c * channel_stride[s] samples of d_pcm; its frames go to d_frames + frames_offset[s]
  * (info.frame_count * info.frame_size bytes, from vgb_hca_query).  The per-stream status of the encoder (the reference's
- * "Bitrate is set too low." ...) stays in the workspace: vgb_hca_encode_dev_status synchronises the stream and maps it. */
+ * "Bitrate is set too low." ...) stays in the workspace: vgb_hca_encode_dev_status synchronises the stream and maps it.
+ * d_pcm must be 2-byte and d_workspace 8-byte aligned (VGB_E_ARG otherwise); d_frames and the offsets may be odd. */
 uint64_t vgb_hca_workspace_bytes(int32_t n_streams);
 int32_t vgb_hca_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, const int64_t *channel_stride, const vgb_hca_params *params,
                            int32_t n_streams, vgb_hca_info *info_out, uint8_t *d_frames, const int64_t *frames_offset,
@@ -434,7 +441,8 @@ int32_t vgb_hca_decode_batch(const uint8_t *const *frames, const vgb_hca_info *i
  * the buffer first for the reference's fresh short[].  The workspace holds the stream table, the status words, the parse
  * records and the seam addends; vgb_hca_decode_workspace_bytes sizes it from the same info.  The per-stream status of
  * the decoder stays in the workspace: vgb_hca_decode_dev_status synchronises the stream and maps it to VGB_E_DATA with
- * vgb_hca_decode_batch's messages. */
+ * vgb_hca_decode_batch's messages.  d_pcm must be 2-byte aligned and d_workspace 8-byte aligned (the stream table's
+ * int64 fields, the fp64 seam addends); VGB_E_ARG otherwise. */
 uint64_t vgb_hca_decode_workspace_bytes(const vgb_hca_info *info, int32_t n_streams);
 int32_t vgb_hca_decode_dev(const uint8_t *d_frames, const int64_t *frames_offset, const vgb_hca_info *info, int32_t n_streams,
                            int16_t *d_pcm, const int64_t *pcm_offset, const int64_t *channel_stride,

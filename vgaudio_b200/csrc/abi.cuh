@@ -39,6 +39,15 @@ int32_t fail(int32_t code, const char *fmt, ...);    // sets g_err, returns `cod
 
 inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// VGB_E_ARG unless the caller's device pointer `p` (argument `name`) is `a`-byte aligned (a power of two; NULL passes).
+// The _dev entry points check their base pointers with it before any device work: the kernels behind them read and
+// write with vector loads, cp.async copies and 8-byte fields that would fault the context on a misaligned address.
+inline int32_t check_aligned(const void *p, size_t a, const char *name)
+{
+    if (reinterpret_cast<uintptr_t>(p) & (a - 1)) return fail(VGB_E_ARG, "%s=%p must be %zu-byte aligned", name, p, a);
+    return VGB_OK;
+}
+
 // Grow-only device buffer.
 struct DevBuf {
     void *p = nullptr;

@@ -221,6 +221,10 @@ int32_t vgb_adx_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, cons
     if (n_channels < 0) return fail(VGB_E_ARG, "n_channels is negative");
     if (n_channels == 0) return VGB_OK;
     if (!d_pcm || !pcm_offset || !n_samples || !params || !d_adpcm || !adpcm_offset || !d_workspace) return fail(VGB_E_ARG, "NULL argument");
+    VGB_TRY(check_aligned(d_pcm, 16, "d_pcm"));  // the encoder's cp.async
+    VGB_TRY(check_aligned(d_history_out, 2, "d_history_out"));
+    VGB_TRY(check_aligned(d_adpcm, 2, "d_adpcm"));  // uint16_t stores
+    VGB_TRY(check_aligned(d_workspace, 8, "d_workspace"));  // AdxChannel's int64 fields
     {
         int64_t total = 0;
         for (int c = 0; c < n_channels; c++) total += n_samples[c] > 0 ? n_samples[c] : 0;

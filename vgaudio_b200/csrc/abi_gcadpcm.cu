@@ -875,6 +875,11 @@ int32_t vgb_gcadpcm_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, 
     VGB_TRY(dev_layout(lay, pcm_offset, adpcm_offset, n_samples, params, n_channels, false, true));
     if (n_channels == 0) return VGB_OK;
     if (!d_pcm || !d_coefs_out || !d_adpcm || !d_workspace) return fail(VGB_E_ARG, "NULL device pointer");
+    VGB_TRY(check_aligned(d_pcm, 16, "d_pcm"));  // gc_coef_frames_kernel's uint4 loads, the encoder's cp.async
+    VGB_TRY(check_aligned(d_coefs_in, 2, "d_coefs_in"));
+    VGB_TRY(check_aligned(d_coefs_out, 2, "d_coefs_out"));
+    VGB_TRY(check_aligned(d_adpcm, 16, "d_adpcm"));  // the encoder's uint4 stores
+    VGB_TRY(check_aligned(d_workspace, 16, "d_workspace"));  // double2 records
     const GcWorkspace w = carve(lay.rec_total, n_channels);
     if (w.total > workspace_bytes)
         return fail(VGB_E_ARG, "workspace too small: need %zu bytes, got %llu", w.total, (unsigned long long)workspace_bytes);
@@ -891,6 +896,9 @@ int32_t vgb_gcadpcm_coefs_dev(const int16_t *d_pcm, const int64_t *pcm_offset, c
     VGB_TRY(dev_layout(lay, pcm_offset, nullptr, n_samples, nullptr, n_channels, false, false));
     if (n_channels == 0) return VGB_OK;
     if (!d_pcm || !d_coefs_out || !d_workspace) return fail(VGB_E_ARG, "NULL device pointer");
+    VGB_TRY(check_aligned(d_pcm, 16, "d_pcm"));
+    VGB_TRY(check_aligned(d_coefs_out, 2, "d_coefs_out"));
+    VGB_TRY(check_aligned(d_workspace, 16, "d_workspace"));
     const GcWorkspace w = carve(lay.rec_total, n_channels);
     if (w.total > workspace_bytes)
         return fail(VGB_E_ARG, "workspace too small: need %zu bytes, got %llu", w.total, (unsigned long long)workspace_bytes);
@@ -914,6 +922,10 @@ int32_t vgb_gcadpcm_decode_dev(const uint8_t *d_adpcm, const int64_t *adpcm_offs
     GcLayout lay;
     VGB_TRY(dev_layout(lay, pcm_offset, adpcm_offset, counts.data(), params, n_channels, true, true));
     if (!d_pcm || !d_coefs || !d_adpcm || !d_workspace) return fail(VGB_E_ARG, "NULL device pointer");
+    VGB_TRY(check_aligned(d_adpcm, 16, "d_adpcm"));  // gc_decode_kernel's cp.async
+    VGB_TRY(check_aligned(d_coefs, 2, "d_coefs"));
+    VGB_TRY(check_aligned(d_pcm, 16, "d_pcm"));  // its uint4 stores
+    VGB_TRY(check_aligned(d_workspace, 16, "d_workspace"));
     const GcWorkspace w = carve(32, n_channels);
     if (w.total > workspace_bytes)
         return fail(VGB_E_ARG, "workspace too small: need %zu bytes, got %llu", w.total, (unsigned long long)workspace_bytes);

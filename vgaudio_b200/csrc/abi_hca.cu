@@ -573,6 +573,8 @@ int32_t vgb_hca_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, cons
     if (n_streams < 0) return fail(VGB_E_ARG, "n_streams is negative");
     if (n_streams == 0) return VGB_OK;
     if (!d_pcm || !pcm_offset || !channel_stride || !params || !d_frames || !frames_offset || !d_workspace) return fail(VGB_E_ARG, "NULL argument");
+    VGB_TRY(check_aligned(d_pcm, 2, "d_pcm"));
+    VGB_TRY(check_aligned(d_workspace, 8, "d_workspace"));  // HcaStream's int64 fields
     if (vgb_hca_workspace_bytes(n_streams) > workspace_bytes)
         return fail(VGB_E_ARG, "workspace too small: need %llu bytes", (unsigned long long)vgb_hca_workspace_bytes(n_streams));
     std::vector<vgb_hca_info> infos;
@@ -778,6 +780,8 @@ int32_t vgb_hca_decode_dev(const uint8_t *d_frames, const int64_t *frames_offset
     if (n_streams < 0) return fail(VGB_E_ARG, "n_streams is negative");
     if (n_streams == 0) return VGB_OK;
     if (!d_frames || !frames_offset || !info || !d_pcm || !pcm_offset || !channel_stride || !d_workspace) return fail(VGB_E_ARG, "NULL argument");
+    VGB_TRY(check_aligned(d_pcm, 2, "d_pcm"));
+    VGB_TRY(check_aligned(d_workspace, 8, "d_workspace"));  // HcaStream's int64 fields, the fp64 seam addends
     if (n_streams > 65535) return fail(VGB_E_ARG, "n_streams %d: at most 65535 streams per call", n_streams);  // grid y / z of the frame kernels
     VGB_TRY(hca_decode_check(info, n_streams));
     const uint64_t need = vgb_hca_decode_workspace_bytes(info, n_streams);
