@@ -1,6 +1,7 @@
 // bindings/csharp/Containers.B200.cs — P/Invoke declarations and replacement bodies for the container layer either side of
 // the codec path (include/vgaudio_b200.h, "Containers either side of the codec path"): WaveReader, DspWriter / DspReader,
-// AdxWriter / AdxReader (+ CriAdxEncryption), HcaWriter / HcaReader (+ CriHcaEncryption) and the CLI's batch job.
+// AdxWriter / AdxReader (+ CriAdxEncryption), HcaWriter / HcaReader (+ CriHcaEncryption), BrstmReader / BCFstmReader and the
+// CLI's batch job.
 // NOT compiled in this repository (no .NET toolchain in the build image); this is the file a VGAudio maintainer adds.
 using System;
 using System.Collections.Generic;
@@ -43,6 +44,20 @@ namespace VGAudio.Native
         public int SamplesPerFrame, Reserved;
         public long AudioOffset, AudioSize;
         public fixed short History[255 * 2];
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    internal unsafe struct VgbNwInfo   // BxstmStructure (Containers/NintendoWare/BxstmStructure.cs), what decoding needs
+    {
+        public int Codec, Looping, ChannelCount, SampleRate, LoopStart, SampleCount;
+        public int InterleaveSize, BigEndian;
+        public uint Version;
+        public int SeekTable, RegionCount, TrackCount, AdpcmChannelCount, SamplesPerSeekEntry;
+        public int LoopStartUnaligned, LoopEndUnaligned, OutputSize, Reserved;
+        public long AudioOffset, AudioLength;
+        public fixed short Coefs[255 * 16];
+        public fixed short Gain[255];
+        public fixed short StartContext[255 * 3], LoopContext[255 * 3];
     }
 
     [StructLayout(LayoutKind.Sequential)]
@@ -90,6 +105,11 @@ namespace VGAudio.Native
         public static extern int vgb_convert_adx_to_wave_batch(byte** files, long* lengths, int nFiles, VgbAdxKey* key, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_hca_to_wave_batch(byte** files, long* lengths, int nFiles, ulong* keyCode, long* outSizes, byte** filesOut, int* statusOut);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_brstm_parse(byte* file, long length, VgbNwInfo* info);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_bcfstm_parse(byte* file, long length, VgbNwInfo* info);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_convert_nw_to_wave_batch(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_gcadpcm_debug_decode_stats(ulong* output, int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_wave_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, long* outSizes,
             byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
@@ -281,6 +301,56 @@ namespace VGAudio.Cli
                         File.WriteAllBytes(outPaths[i], outputs[i]);
                     }
                     reportAdd(1);
+                }
+            }
+            finally
+            {
+                foreach (var h in inPins) h.Free();
+                foreach (var h in outPins) h.Free();
+            }
+        }
+
+        // The decode direction for a chunk of NintendoWare streams (`-b --out-format wav` over .brstm / .bcstm / .bfstm): the
+        // reader the extension names (ContainerTypes.cs: BrstmReader for .brstm, BCFstmReader for .bcstm and .bfstm) ->
+        // ToPcm16 -> WaveWriter per file in one native call per pass.  inTypes[i] is VGB_CONTAINER_BRSTM / _BCSTM / _BFSTM
+        // (4 / 5 / 6).  A file whose GC-ADPCM frames select a predictor outside 0..7 fails in the second pass alone.
+        public static unsafe void ConvertNwToWave(string[] inPaths, int[] inTypes, string[] outPaths, Action<string> log, Action<int> reportAdd)
+        {
+            int n = inPaths.Length;
+            byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
+            var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            var outPins = new List<GCHandle>();
+            try
+            {
+                byte** inPtr = stackalloc byte*[n];
+                byte** outPtr = stackalloc byte*[n];
+                long* len = stackalloc long[n];
+                long* outSize = stackalloc long[n];
+                int* status = stackalloc int[n];
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
+                fixed (int* types = inTypes)
+                {
+                    VgAudioB200.Check(VgAudioB200Containers.vgb_convert_nw_to_wave_batch(inPtr, len, types, n, outSize, null, status));
+                    var outputs = new byte[n][];
+                    for (int i = 0; i < n; i++)
+                    {
+                        outPtr[i] = null;
+                        if (status[i] != VgAudioB200.Ok) continue;
+                        outputs[i] = new byte[outSize[i]];
+                        outPins.Add(GCHandle.Alloc(outputs[i], GCHandleType.Pinned));
+                        outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
+                    }
+                    VgAudioB200.Check(VgAudioB200Containers.vgb_convert_nw_to_wave_batch(inPtr, len, types, n, outSize, outPtr, status));
+                    for (int i = 0; i < n; i++)
+                    {
+                        if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); }   // Batch.cs:39-43
+                        else
+                        {
+                            Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
+                            File.WriteAllBytes(outPaths[i], outputs[i]);
+                        }
+                        reportAdd(1);
+                    }
                 }
             }
             finally

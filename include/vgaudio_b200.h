@@ -552,6 +552,42 @@ typedef struct vgb_adx_file_info {
  * (no whole sample per frame) and InsertedSamples <= -samples_per_frame (ToPcm16 would index before the audio). */
 int32_t vgb_adx_parse(const uint8_t *file, int64_t length, vgb_adx_file_info *info_out);
 
+/* BxstmStructure (Containers/NintendoWare/BxstmStructure.cs) as BrstmReader.ReadFile (BrstmReader.cs:12-185) or
+ * BCFstmReader.ReadFile (BCFstmReader.cs:14-288) leaves it, reduced to what decoding needs: StreamInfo's codec
+ * (NwCodec.cs: 0 PCM8, 1 PCM16, 2 GC-ADPCM), looping, channel count, rate, loop start and sample count, the interleave
+ * size and the byte order of the file (BRSTM: always big-endian), the region Stream.DeInterleave reads (audio_length
+ * bytes at audio_offset, each reader's ReadDataBlock) and its per-channel output size (Common.SamplesToBytes), and per
+ * channel with GC-ADPCM info (Structures/ChannelInfo.cs) the coefficients, gain (BRSTM only) and start / loop contexts
+ * (PredScale, Hist1, Hist2).  version is NwVersion.Version; seek_table: 0 none read, 1 read (BRSTM: the standard size),
+ * 2 the shortened BRSTM size; region_count / track_count: entries read from REGN / the track info.  The unaligned loop
+ * fields (version-dependent, Common.cs:118-157) are read and reported but, as in the reference, not used. */
+#define VGB_NW_MAX_CHANNELS 255
+typedef struct vgb_nw_info {
+    int32_t codec, looping, channel_count, sample_rate, loop_start, sample_count;
+    int32_t interleave_size, big_endian;
+    uint32_t version;
+    int32_t seek_table, region_count, track_count, adpcm_channel_count, samples_per_seek_entry;
+    int32_t loop_start_unaligned, loop_end_unaligned, output_size, reserved;
+    int64_t audio_offset, audio_length;
+    int16_t coefs[VGB_NW_MAX_CHANNELS][16];
+    int16_t gain[VGB_NW_MAX_CHANNELS];
+    int16_t start_context[VGB_NW_MAX_CHANNELS][3], loop_context[VGB_NW_MAX_CHANNELS][3];
+} vgb_nw_info;
+/* The two readers on a file image, host only.  Every read and check runs in the reference's order and fails with
+ * VGB_E_DATA and the reference's message: the signature ("File has no RSTM header", "File has no CSTM or FSTM header")
+ * and byte-order mark, "Actual file length is less than stated length", each block's id and size against the main
+ * header (HEAD / ADPC / DATA, INFO / SEEK / REGN / DATA), "Could not read stream/track/channel info.", a read past the
+ * image, a negative position, the ADPC / SEEK seek table (BRSTM: the standard and shortened sizes are read, another size
+ * is skipped; a zero samples-per-entry divides by zero), the REGN regions (a REGN block in a version without region
+ * info dereferences null), the track info, and Stream.DeInterleave's checks (Utilities/Interleave.cs:118-133: the
+ * region stays in the image and splits evenly over the channels).  Refused on purpose, where the reference would fail
+ * later or read something these readers do not carry: codec 3 (IMA; ToAudioStream returns null) and any codec above
+ * it, a GC-ADPCM stream with fewer channel infos than channels, and CWAV / FWAV / CSTP / FSTP images, wave info blocks
+ * and prefetch / wave data blocks (BCFstmReader accepts them; "... are not read").  vgb_bcfstm_parse accepts CSTM and
+ * FSTM alike. */
+int32_t vgb_brstm_parse(const uint8_t *file, int64_t length, vgb_nw_info *info_out);
+int32_t vgb_bcfstm_parse(const uint8_t *file, int64_t length, vgb_nw_info *info_out);
+
 /* HcaReader.ReadHcaHeader (Containers/Hca/HcaReader.cs:59-121) on a file image, host only: the chunk walk over
  * header_size bytes ("fmt", "comp", "dec", "loop", "ath", "ciph", "rva", "vbr", "comm", "pad"; every id byte masked with
  * 0x7f, so the ids of encrypted files read the same; a later chunk overwrites what an earlier one set), UseAthCurve for
@@ -581,6 +617,9 @@ int32_t vgb_hca_write_batch(const vgb_hca_info *info, int32_t n_files, const uin
 #define VGB_CONTAINER_DSP 1
 #define VGB_CONTAINER_ADX 2
 #define VGB_CONTAINER_HCA 3
+#define VGB_CONTAINER_BRSTM 4 /* NintendoWare streams: readers only (vgb_convert_nw_to_wave_batch) */
+#define VGB_CONTAINER_BCSTM 5
+#define VGB_CONTAINER_BFSTM 6
 typedef struct vgb_convert_options {
     int32_t out_type;                   /* VGB_CONTAINER_* */
     int32_t no_trim;                    /* Configuration.TrimFile = !no_trim */
@@ -646,6 +685,33 @@ int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t
  * status_out NULL such a file fails the call (VGB_E_DATA) after every other file has been written. */
 int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_adx_key *key,
                                       int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* The decode direction of the batch job for NintendoWare streams: .brstm, .bcstm and .bfstm file images in, 16-bit
+ * WAVE images out - BrstmReader / BCFstmReader (vgb_brstm_parse / vgb_bcfstm_parse) -> Common.ToAudioStream
+ * (Containers/NintendoWare/Common.cs:45-116) -> ToPcm16 -> WaveWriter.  in_type[i] (VGB_CONTAINER_BRSTM, _BCSTM or
+ * _BFSTM) names the reader, as the reference picks one by file extension: BRSTM uses BrstmReader, BCSTM and BFSTM both
+ * use BCFstmReader, which accepts either magic; the magic is not sniffed, so a .bcstm image passed as BRSTM fails as in
+ * the reference.  Same two-pass protocol, per-file status and sharding as vgb_convert_adx_to_wave_batch (files weigh
+ * sample_count * channel_count).  Per group of files, on the device: one H2D of the DATA regions, the existing
+ * de-interleave (Stream.DeInterleave: a shorter last block, rows of SamplesToBytes(sample_count) bytes zero-filled or
+ * truncated; an interleave size <= 0 copies nothing, so the rows are zeros), then the GC-ADPCM rows through the
+ * time-parallel decoder (from each channel's start context; VGB_GC_DEC_SEGMENTS / VGB_GC_DEC_MIN_SEG_FRAMES force the
+ * segment count and the shortest segment, read at each call) and the PCM rows through nw_pcm_kernel (PCM16 byte-swapped
+ * when the file is big-endian, PCM8 by Pcm8Codec.DecodeSigned), then the WAVE join behind the host-built header (smpl
+ * when looping, extensible fmt above two channels), one D2H of the finished files.  Gain, tracks, regions and seek
+ * tables do not change the output and are not read by the decode.  Loop points follow WithLoop(Looping, LoopStart,
+ * SampleCount) (AudioFormatBaseBuilder.cs:23-50; VGB_E_ARG with its messages).  Per-file errors, each failing that
+ * file only: in_type not one of the three, a parse error, bad loop points, a negative sample count (refused on purpose:
+ * the reference allocates from it), 2 GiB of PCM or more, too many channels for the WAVE join - all known in the sizing
+ * pass - and, found on the device in the fill pass, a GC-ADPCM frame header that selects a predictor 8..15 (the
+ * reference indexes coefficients[predictor * 2] and throws): that file gets its status_out entry, out_sizes[i] = 0 and
+ * its buffer is not written.  With status_out NULL such a file fails the call (VGB_E_DATA) after every other file has
+ * been written. */
+int32_t vgb_convert_nw_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                                     int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* Bookkeeping of the most recent time-parallel GC-ADPCM decode of vgb_convert_nw_to_wave_batch on this thread's
+ * context (its last group of files): out[0] segments per channel, [1] frames decoded by run-ons, [2] frames decoded by
+ * the cascade, [3] boundaries the cascade repaired, [4] longest run-on in frames.  Synchronises the device. */
+int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n);
 /* Transcoding in the batch job: .dsp, .adx and .hca file images in, another of the three out (Convert.ConvertFile with a
  * coded source: the source's reader, a fresh configuration from the options, source.ToPcm16() -> EncodeFromPcm16).
  * in_type[i] (VGB_CONTAINER_*) names file i's codec: a .dsp file has no signature.  options->out_type, its options and

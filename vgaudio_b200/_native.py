@@ -117,6 +117,21 @@ class VgbAdxFileInfo(C.Structure):
         ("audio_offset", C.c_int64), ("audio_size", C.c_int64), ("history", (C.c_int16 * 2) * VGB_ADX_MAX_CHANNELS)]
 
 
+VGB_NW_MAX_CHANNELS = 255
+
+
+class VgbNwInfo(C.Structure):
+    """BxstmStructure as BrstmReader / BCFstmReader leave it, reduced to what decoding needs (see the header)."""
+
+    _fields_ = [(n, C.c_int32) for n in ("codec", "looping", "channel_count", "sample_rate", "loop_start", "sample_count",
+                                         "interleave_size", "big_endian")] + [("version", C.c_uint32)] + [
+        (n, C.c_int32) for n in ("seek_table", "region_count", "track_count", "adpcm_channel_count", "samples_per_seek_entry",
+                                 "loop_start_unaligned", "loop_end_unaligned", "output_size", "reserved")] + [
+        ("audio_offset", C.c_int64), ("audio_length", C.c_int64),
+        ("coefs", (C.c_int16 * 16) * VGB_NW_MAX_CHANNELS), ("gain", C.c_int16 * VGB_NW_MAX_CHANNELS),
+        ("start_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS), ("loop_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS)]
+
+
 class VgbConvertOptions(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("out_type", "no_trim", "dsp_samples_per_interleave", "dsp_loop_point_alignment",
                                          "adx_version", "adx_frame_size", "adx_type", "adx_filter_plus1",
@@ -239,6 +254,10 @@ SIGNATURES = {
     "vgb_convert_dsp_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_hca_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_adx_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_brstm_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "vgb_bcfstm_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "vgb_convert_nw_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_gcadpcm_debug_decode_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_convert_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),
     "vgb_transcode_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

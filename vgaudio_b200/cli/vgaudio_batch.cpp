@@ -1,5 +1,5 @@
 // vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
-// .dsp / .adx / .hca, and .dsp, .adx and .hca files to WAVE.
+// .dsp / .adx / .hca, and .dsp, .adx, .hca, .brstm, .bcstm and .bfstm files to WAVE.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
@@ -7,7 +7,7 @@
 // (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch for coded files, vgb_convert_*_to_wave_batch for
 // --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
-//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp, .hca and .adx inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
+//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm and .bfstm inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
@@ -46,12 +46,15 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
     return n == 0 || (bool)f.read(reinterpret_cast<char *>(out.data()), n);
 }
 
-// the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, -1 none of them
+// the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, 4 .brstm, 5 .bcstm, 6 .bfstm, -1 none of them.  The
+// extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs): the NintendoWare streams are
+// read (decoded to WAVE), not written.
 static int kind_of(const fs::path &p)
 {
     std::string ext = p.extension().string();
     std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
-    return ext == ".dsp" ? 0 : ext == ".hca" ? 1 : ext == ".adx" ? 2 : (ext == ".wav" || ext == ".wave") ? 3 : -1;
+    return ext == ".dsp" ? 0 : ext == ".hca" ? 1 : ext == ".adx" ? 2 : (ext == ".wav" || ext == ".wave") ? 3
+         : ext == ".brstm" ? 4 : ext == ".bcstm" ? 5 : ext == ".bfstm" ? 6 : -1;
 }
 static const int32_t kContainerOfKind[3] = {VGB_CONTAINER_DSP, VGB_CONTAINER_HCA, VGB_CONTAINER_ADX};
 
@@ -141,7 +144,7 @@ int main(int argc, char **argv)
         if (s != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
     }
 
-    // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca and .adx ones when decoding; else the WAVE
+    // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca, .adx and NintendoWare ones when decoding; else the WAVE
     // ones and the coded ones in another codec than the output's)
     std::vector<fs::path> files;
     std::error_code ec;
@@ -149,7 +152,7 @@ int main(int argc, char **argv)
         if (!e.is_regular_file()) return;
         const int kind = kind_of(e.path());
         if (kind < 0) return;
-        if (to_wave ? kind < 3 : (kind == 3 || kContainerOfKind[kind] != opt.out_type)) files.push_back(e.path());
+        if (to_wave ? kind != 3 : (kind == 3 || (kind < 3 && kContainerOfKind[kind] != opt.out_type))) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -177,14 +180,15 @@ int main(int argc, char **argv)
         std::vector<int32_t> status(n);
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
         // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
-        // codec; encoding, the WAVE converter for WAVE files and one transcode call for the coded ones
-        std::vector<int32_t> rows[4];
+        // codec (one for the three NintendoWare streams); encoding, the WAVE converter for WAVE files and one transcode
+        // call for the coded ones
+        std::vector<int32_t> rows[5];
         for (int k = 0; k < n; k++) {
             const int kind = kind_of(files[first + k]);
-            rows[to_wave ? kind : (kind == 3 ? 3 : 0)].push_back(k);
+            rows[to_wave ? std::min(kind, 4) : (kind == 3 ? 3 : 0)].push_back(k);
         }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
-            for (int h = 0; h < 4; h++) {
+            for (int h = 0; h < 5; h++) {
                 const std::vector<int32_t> &r = rows[h];
                 if (r.empty()) continue;
                 std::vector<const uint8_t *> p;
@@ -195,6 +199,7 @@ int main(int argc, char **argv)
                     p.push_back(ptr[k]); l.push_back(len[k]); o.push_back(outs ? outs[k] : nullptr);
                     const int kind = kind_of(files[first + k]);
                     if (kind < 3) types.push_back(kContainerOfKind[kind]);
+                    else if (kind > 3) types.push_back(VGB_CONTAINER_BRSTM + (kind - 4));
                 }
                 const int32_t m = (int32_t)r.size();
                 uint8_t *const *ot = outs ? o.data() : nullptr;
@@ -202,6 +207,7 @@ int main(int argc, char **argv)
                 if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
                 else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, have_in_adx_key ? &in_adx_key : nullptr,
                                                            have_in_code ? &in_key_code : nullptr, sz.data(), ot, st.data(), nullptr, nullptr);
+                else if (h == 4) s = vgb_convert_nw_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
                 else s = h == 2 ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, have_adx_key ? &adx_key : nullptr, sz.data(), ot, st.data())
                        : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
                                 : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());

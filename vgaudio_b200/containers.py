@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's container layer either side of the codec path (SURVEY.md 8f rank 2-4) over the
 C ABI: WaveReader, DspWriter / DspReader, AdxWriter (+ CriAdxEncryption / CriAdxKey), HcaWriter (+ CriHcaEncryption /
-CriHcaKey) and the CLI's batch conversion (src/VGAudio.Cli/Batch.cs).  No arithmetic here: parsing, byte movement and
+CriHcaKey), BrstmReader / BCFstmReader and the CLI's batch conversion (src/VGAudio.Cli/Batch.cs).  No arithmetic here: parsing, byte movement and
 key streams run in libvgaudio_b200.so.
 """
 from __future__ import annotations
@@ -14,6 +14,7 @@ import numpy as np
 from . import _native as N
 
 CONTAINER_DSP, CONTAINER_ADX, CONTAINER_HCA = 1, 2, 3
+CONTAINER_BRSTM, CONTAINER_BCSTM, CONTAINER_BFSTM = 4, 5, 6   # readers only: convert_nw_to_wave_batch
 
 
 def _bytes_arr(b) -> np.ndarray:
@@ -294,6 +295,32 @@ def convert_adx_to_wave_batch(files: Sequence, key: Optional[N.VgbAdxKey] = None
     adx_key) decrypts files of revision 8 and 9 (None: such files fail); a file with a bad Fixed-type filter fails alone."""
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_adx_to_wave_batch(
         ftab, lens, n, C.byref(key) if key is not None else None, sizes, otab, st), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def brstm_parse(file) -> N.VgbNwInfo:
+    """BrstmReader.ReadFile on a file image, reduced to what decoding needs; raises VgbError(VGB_E_DATA)."""
+    f = _bytes_arr(file)
+    info = N.VgbNwInfo()
+    N.check(N.lib.vgb_brstm_parse(f.ctypes.data, f.size, C.byref(info)))
+    return info
+
+
+def bcfstm_parse(file) -> N.VgbNwInfo:
+    """BCFstmReader.ReadFile (CSTM or FSTM) on a file image; raises VgbError(VGB_E_DATA)."""
+    f = _bytes_arr(file)
+    info = N.VgbNwInfo()
+    N.check(N.lib.vgb_bcfstm_parse(f.ctypes.data, f.size, C.byref(info)))
+    return info
+
+
+def convert_nw_to_wave_batch(files: Sequence, in_types: Sequence[int]) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """The decode direction of the batch job for .brstm / .bcstm / .bfstm images (in_types: CONTAINER_BRSTM, _BCSTM or
+    _BFSTM per file, naming the reader): ([WAVE bytes or None], [per-file status]); a file whose GC-ADPCM frames select a
+    predictor outside 0..7 fails alone."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_nw_to_wave_batch(
+        ftab, lens, types, n, sizes, otab, st), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
 
 

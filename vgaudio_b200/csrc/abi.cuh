@@ -113,6 +113,7 @@ struct Context {
     std::atomic<int64_t> launches{0};
     GcSegArgs last_seg{};            // bookkeeping of the most recent encode launch (vgb_gcadpcm_debug_splice_stats)
     AdxDecSegArgs last_adx_dec{};    // the same for the most recent time-parallel ADX decode (vgb_adx_debug_decode_stats)
+    GcDecSegArgs last_gc_dec{};      // and GC-ADPCM decode (vgb_gcadpcm_debug_decode_stats)
     HcaTableStore hca_tables;
     std::atomic<ContainerState *> containers{nullptr};  // created on first use, released by containers_release
 };
@@ -137,6 +138,12 @@ int32_t hca_encode_fault(int32_t status, const char *what, int index);
 // abi_adx.cu: synchronises `st` and copies the per-channel status words of the last vgb_adx_decode_dev on `d_workspace`
 // (bit 0: a Fixed-type frame selects a filter 4..7, bit 1: a frame of another type a filter 1..7) to status[0..n)
 int32_t adx_decode_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st);
+// abi_gcadpcm.cu, the time-parallel GC-ADPCM decode of the NintendoWare -> WAVE converter: workspace bytes for
+// n_channels channels holding full_frames full frames in all, the asynchronous decode (tab: host table; trace_off is
+// filled here), and the per-channel status words (bit 0: a predictor 8..15), which synchronise `st`
+uint64_t gc_decode_seg_workspace_bytes(int32_t n_channels, int64_t full_frames);
+int32_t gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &tab, int16_t *d_pcm, void *d_workspace, cudaStream_t st);
+int32_t gc_decode_seg_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st);
 void tick(int slot, bool begin, cudaStream_t stream);
 
 // hooks of containers.cu, which keeps its own slabs and streams per context (Context::containers)

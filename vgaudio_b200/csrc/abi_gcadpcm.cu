@@ -524,9 +524,87 @@ int32_t align_one(const uint8_t *const *adpcm, const int32_t *n_bytes, const int
     return VGB_OK;
 }
 
+// Byte offsets in a workspace of the time-parallel decode: channel table, status words, run-on start pairs, stats, the
+// trace (one word per full frame)
+struct GcSegDecodeLayout {
+    size_t o_status, o_used, o_stats, o_trace, bytes;
+    GcSegDecodeLayout(int n_channels, int64_t full_frames)
+    {
+        const size_t n = (size_t)std::max(n_channels, 1);
+        o_status = align_up(n * sizeof(GcDecChannel), 256);
+        o_used = o_status + align_up(n * 4, 256);
+        o_stats = o_used + align_up(n * kGcDecMaxSegments * 4, 256);
+        o_trace = o_stats + 256;
+        bytes = o_trace + align_up((size_t)(full_frames + 1) * 4, 256);
+    }
+};
+
 }  // namespace
 
+uint64_t vgb::gc_decode_seg_workspace_bytes(int32_t n_channels, int64_t full_frames)
+{
+    return GcSegDecodeLayout(n_channels, full_frames).bytes;
+}
+
+int32_t vgb::gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &tab, int16_t *d_pcm, void *d_workspace, cudaStream_t st)
+{
+    const int n_channels = (int)tab.size();
+    if (n_channels == 0) return VGB_OK;
+    int64_t frames = 0;
+    int max_full = 0;
+    for (GcDecChannel &c : tab) {
+        const int full = c.n_samples / kGcFrameSamples;
+        c.trace_off = frames;
+        frames += full;
+        max_full = std::max(max_full, full);
+    }
+    const GcSegDecodeLayout L(n_channels, frames);
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    VGB_TRY(ensure_ready_locked());
+    char *ws = static_cast<char *>(d_workspace);
+    GcDecSegArgs sa{};
+    sa.trace = reinterpret_cast<uint32_t *>(ws + L.o_trace);
+    sa.used_start = reinterpret_cast<uint32_t *>(ws + L.o_used);
+    sa.stats = reinterpret_cast<unsigned long long *>(ws + L.o_stats);
+    sa.status = reinterpret_cast<int32_t *>(ws + L.o_status);
+    sa.seg_count = gc_decode_pick_segments(n_channels, max_full, &sa.min_seg_frames);
+    CUDA_TRY(cudaMemcpyAsync(ws, tab.data(), tab.size() * sizeof(GcDecChannel), cudaMemcpyHostToDevice, st));  // pageable: staged before return
+    CUDA_TRY(cudaMemsetAsync(ws + L.o_status, 0, (size_t)n_channels * 4, st));
+    CUDA_TRY(cudaMemsetAsync(ws + L.o_stats, 0, kGcDecStatWords * sizeof(unsigned long long), st));
+    tick(3, true, st);
+    launch_gc_decode_seg(d_adpcm, reinterpret_cast<const GcDecChannel *>(ws), n_channels, d_pcm, sa, st);
+    tick(3, false, st);
+    g_ctx.launches += sa.seg_count > 1 ? 3 : 1;
+    g_ctx.last_gc_dec = sa;
+    CUDA_TRY(cudaGetLastError());
+    return VGB_OK;
+}
+
+int32_t vgb::gc_decode_seg_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st)
+{
+    const GcSegDecodeLayout L(n_channels, 0);
+    CUDA_TRY(cudaMemcpyAsync(status, static_cast<const char *>(d_workspace) + L.o_status, (size_t)n_channels * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return VGB_OK;
+}
+
 extern "C" {
+
+/* Bookkeeping of the most recent time-parallel GC-ADPCM decode on this thread's context (see the header).
+ * Synchronises the device. */
+int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n)
+{
+    if (!out || n < 0) return fail(VGB_E_ARG, "bad arguments");
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    for (int i = 0; i < n; i++) out[i] = 0;
+    if (!g_ctx.ready || !g_ctx.last_gc_dec.stats) return VGB_OK;
+    unsigned long long st[kGcDecStatWords] = {};
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(st, g_ctx.last_gc_dec.stats, sizeof st, cudaMemcpyDeviceToHost));
+    if (n > 0) out[0] = (uint64_t)g_ctx.last_gc_dec.seg_count;
+    for (int i = 1; i < n && i <= kGcDecStatWords; i++) out[i] = st[i - 1];
+    return VGB_OK;
+}
 
 int32_t vgb_gcadpcm_alignment(const vgb_gc_align_params *p, vgb_gc_alignment *out)
 {

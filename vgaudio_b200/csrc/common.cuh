@@ -69,6 +69,29 @@ struct GcSegArgs {
     int32_t min_seg_frames;      // no segment shorter than this
 };
 
+// Time-parallel GC-ADPCM decoding (gc_decode.cu, the gc_decode_seg_kernel family): the FULL frames of a channel (all 14
+// samples present) are cut into segments; the partial last frame, if any, is decoded from the true pair after them.
+struct GcDecChannel {
+    int64_t pcm_off;     // sample offset of the channel's output (multiple of 8)
+    int64_t adpcm_off;   // byte offset of the channel's row (multiple of 16)
+    int64_t trace_off;   // first word of the channel in the trace slab (one word per full frame)
+    int32_t n_samples;
+    int16_t hist1, hist2;  // start context (GcAdpcmChannel.GetPcmAudio, GcAdpcmChannel.cs:57-60)
+    int16_t coefs[16];
+};
+constexpr int kGcDecMinSegFrames = 1024;  // re-lock census (DESIGN.md §5.4b): median 9, p99 133, max 995 frames; VGB_GC_DEC_MIN_SEG_FRAMES overrides
+constexpr int kGcDecMaxSegments = 256;
+constexpr int kGcDecStatWords = 4;
+struct GcDecSegArgs {
+    uint32_t *trace;             // [trace_off[ch] + full frame] the biased pair (hist1 + 32768) | (hist2 + 32768) << 16 after it
+    uint32_t *used_start;        // [ch][kGcDecMaxSegments] the pair a boundary's run-on started from
+    unsigned long long *stats;   // [0] frames decoded by run-ons, [1] by the cascade, [2] boundaries the cascade repaired,
+                                 // [3] longest run-on
+    int32_t *status;             // [ch] bit 0: a frame that yields samples selects a predictor 8..15
+    int32_t seg_count;
+    int32_t min_seg_frames;
+};
+
 // One channel of a seek-table / loop-context request (gc_decode_kernel<true>).
 struct GcTapChannel {
     int64_t out_off;            // first short of the channel in the tap slab: [entries * 2 seek shorts][hist1][hist2]

@@ -14,6 +14,7 @@
 // byte, loop context), which the assemble kernel patches in.  Citations are relative to VGAudio's src/VGAudio/.
 #include <chrono>
 #include <cmath>
+#include <cstdarg>
 #include <cstdio>
 #include <deque>
 
@@ -185,6 +186,47 @@ __global__ void __launch_bounds__(256) wave_join_kernel(const int16_t *__restric
     const int n_el = ns * ch, n_words = n_el >> 1;
     for (int k = threadIdx.x; k < n_words; k += blockDim.x) reinterpret_cast<uint32_t *>(data)[k] = reinterpret_cast<const uint32_t *>(tile)[k];
     if ((n_el & 1) && threadIdx.x == 0) reinterpret_cast<int16_t *>(data)[n_el - 1] = tile[n_el - 1];
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// NintendoWare PCM rows -> the int16 rows the WAVE join reads (Common.ToPcm16Stream / ToPcm8Stream, Common.cs:99-116):
+// PCM16 is ToShortArray in the file's byte order, PCM8 is Pcm8Codec.DecodeSigned (Codecs/Pcm8/Pcm8Codec.cs:41-50).
+// wave_split_kernel's 8-bit path reads unsigned interleaved WAVE bytes; these rows are planar, signed and possibly
+// big-endian, so they get a kernel of their own instead of a caller switch inside the WAVE front end.  One CTA per
+// kNwPcmTile samples of one row; rows start 16-byte aligned on both sides.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kNwPcmTile = 8192;
+struct NwPcmRow {
+    int64_t in_off;    // bytes into the row slab
+    int64_t out_off;   // samples into the PCM slab (multiple of 8)
+    int32_t samples, mode;  // mode 0: PCM8 signed, 1: PCM16 little-endian, 2: PCM16 big-endian
+    int32_t tile_first, pad;
+};
+
+__global__ void __launch_bounds__(256) nw_pcm_kernel(const uint8_t *__restrict__ rows, const NwPcmRow *__restrict__ items, int n_items,
+                                                      int16_t *__restrict__ pcm)
+{
+    const int it = find_item(items, n_items, (int)blockIdx.x);
+    const NwPcmRow r = items[it];
+    const int s0 = ((int)blockIdx.x - r.tile_first) * kNwPcmTile;
+    const int ns = min(kNwPcmTile, r.samples - s0);
+    const uint8_t *src = rows + r.in_off;
+    int16_t *dst = pcm + r.out_off + s0;
+    if (r.mode == 0) {
+        for (int k = threadIdx.x; k < ns; k += blockDim.x) dst[k] = (int16_t)((uint32_t)src[s0 + k] << 8);
+        return;
+    }
+    const uint32_t *w = reinterpret_cast<const uint32_t *>(src + (int64_t)s0 * 2);  // two samples per word
+    uint32_t *o = reinterpret_cast<uint32_t *>(dst);
+    const bool swap = r.mode == 2;
+    for (int k = threadIdx.x; k < ns / 2; k += blockDim.x) {
+        const uint32_t v = w[k];
+        o[k] = swap ? __byte_perm(v, 0, 0x2301) : v;
+    }
+    if ((ns & 1) && threadIdx.x == 0) {
+        const uint8_t *b = src + (int64_t)(s0 + ns - 1) * 2;
+        dst[ns - 1] = (int16_t)(swap ? (b[0] << 8 | b[1]) : (b[1] << 8 | b[0]));
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------

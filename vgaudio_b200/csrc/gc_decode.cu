@@ -14,6 +14,9 @@
 // older-sample product, nibble extraction and scale multiply sit off the chain.  All sums are wrapping int32 like the
 // reference (A.7); folding constants is exact in the ring.
 // Bound: chain latency at <= 1 warp per SM sub-partition (8192 channels = 256 warps), HBM (2.57 B/sample) above that.
+#include <algorithm>
+#include <cstdlib>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -220,6 +223,218 @@ void launch_gc_taps(const uint8_t *adpcm, const GcChannelTable &tab, const int16
     if (tab.n_channels <= 0 || max_frames <= 0) return;
     const int blocks = (tab.n_channels + kDecThreads - 1) / kDecThreads;
     gc_decode_kernel<true><<<blocks, kDecThreads, 0, stream>>>(adpcm, tab, coefs, tap_slab, 0, INT32_MAX, taps);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// TIME-PARALLEL DECODING.  gc_decode_kernel runs one thread through a whole channel: right for many-channel batches,
+// far too serial for a few long stereo streams (a .brstm track lasts minutes).  The decoder is a state machine on
+// (hist1, hist2), so the three phases of the ADX decoder (adx.cu) carry over, with the frame-end pair as the only thing
+// compared:
+//   kGcChain    thread = (channel, segment) over full frames: segment 0 decodes from the channel's start context, the
+//               others from (0, 0); output and every full frame's end pair (`trace`) are written
+//   kGcRunOn    thread = (channel, boundary): from the previous segment's recorded end pair, decode on inside the segment
+//               until a frame-end pair equals the recorded one (from there the recorded output IS the true one)
+//   kGcCascade  thread = channel: repairs, in order, every boundary whose start pair changed after its run-on read it
+//               (a run-on that never locked: digital silence can hold a wrong pair under the >> 11), across segment
+//               ends if need be, then decodes the partial last frame from the true pair
+// Exact by construction: a matching pair after the same frame means identical output from there on.  The per-sample
+// chain is gc_decode_frame's (biased history, rounding constant and bias folded per frame).  Interior boundaries fall
+// on multiples of 4 frames, so every segment reads 32-byte groups through the same cp.async ring as the serial kernel;
+// the chain stores whole groups as 16-byte vectors, run-ons and the cascade store frame by frame (they may stop inside
+// a group).
+// ---------------------------------------------------------------------------------------------------------
+constexpr int kSegThreads = 64;
+constexpr int kGcChain = 0, kGcRunOn = 1, kGcCascade = 2;
+
+__host__ __device__ __forceinline__ int gc_dec_seg_len(int full, int seg_count, int min_seg)
+{
+    const int per = (full + seg_count - 1) / seg_count;
+    return (int)((((int64_t)(per > min_seg ? per : min_seg)) + 3) & ~(int64_t)3);  // interior boundaries on 4-frame groups
+}
+
+template <int kMode>
+__global__ void __launch_bounds__(kSegThreads)
+gc_decode_seg_kernel(const uint8_t *__restrict__ adpcm, const GcDecChannel *__restrict__ tab, int n_channels,
+                     int16_t *__restrict__ pcm, GcDecSegArgs sa)
+{
+    __shared__ uint32_t coef_smem[kSegThreads][9];
+    __shared__ __align__(16) uint4 ring_smem[kDecAhead][2][kSegThreads];
+    const int per_ch = kMode == kGcChain ? sa.seg_count : (kMode == kGcRunOn ? sa.seg_count - 1 : 1);
+    const int64_t idx = (int64_t)blockIdx.x * kSegThreads + threadIdx.x;
+    if (idx >= (int64_t)n_channels * per_ch) return;
+    const int ch = (int)(idx % n_channels);
+    const int s = (int)(idx / n_channels) + (kMode == kGcRunOn ? 1 : 0);
+    const GcDecChannel &c = tab[ch];
+    const int n = c.n_samples;
+    const int full = n / kGcFrameSamples, frames = div_round_up(n, kGcFrameSamples);
+    const int seg_len = gc_dec_seg_len(full, sa.seg_count, sa.min_seg_frames);
+    auto seg_lo = [&](int k) -> int {
+        return k == 0 ? 0 : (k >= sa.seg_count ? full : (int)min((int64_t)full, (int64_t)k * seg_len));
+    };
+    const uint8_t *src = adpcm + c.adpcm_off;
+    int16_t *dst = pcm + c.pcm_off;
+    uint32_t *trace = sa.trace + c.trace_off;
+    uint32_t *pairs = coef_smem[threadIdx.x];
+#pragma unroll
+    for (int p = 0; p < 8; p++) pairs[p] = (uint32_t)(uint16_t)c.coefs[2 * p] | ((uint32_t)(uint16_t)c.coefs[2 * p + 1] << 16);
+
+    // full frames [lo, hi) from st; splice: stop after the first frame whose end pair equals the recorded one.
+    // Returns the number of frames decoded.
+    auto run = [&](int lo, int hi, DecState &st, bool splice) -> int {
+        int done = 0;
+        auto finish = [&](int j) -> bool {  // frame j decoded: record its pair or stop at the recorded one
+            const uint32_t pair = (uint32_t)st.hb1 | ((uint32_t)st.hb2 << 16);
+            done++;
+            if (splice && trace[j] == pair) return true;
+            trace[j] = pair;
+            return false;
+        };
+        auto store7 = [&](int j, const uint32_t *o) {  // frame j's 14 samples: 4-byte aligned (pcm_off is a multiple of 8)
+            uint32_t *d = reinterpret_cast<uint32_t *>(dst + (int64_t)j * kGcFrameSamples);
+#pragma unroll
+            for (int k = 0; k < 7; k++) d[k] = o[k];
+        };
+        const int groups = (hi - lo) / kDecGroupFrames;  // lo is a multiple of 4
+        const uint4 *vin = reinterpret_cast<const uint4 *>(src + (int64_t)lo * kGcFrameBytes);
+        auto issue = [&](int q) {
+            if (q < groups) {
+                uint4 *slot = &ring_smem[q % kDecAhead][0][threadIdx.x];
+                cp_async16(slot, vin + (int64_t)q * 2);
+                cp_async16(slot + kSegThreads, vin + (int64_t)q * 2 + 1);
+            }
+            asm volatile("cp.async.commit_group;" ::: "memory");
+        };
+#pragma unroll
+        for (int a = 0; a < kDecAhead - 1; a++) issue(a);
+        bool stop = false;
+        for (int q = 0; q < groups && !stop; q++) {
+            issue(q + kDecAhead - 1);
+            asm volatile("cp.async.wait_group %0;" ::"n"(kDecAhead - 1) : "memory");
+            const uint4 a = ring_smem[q % kDecAhead][0][threadIdx.x], b = ring_smem[q % kDecAhead][1][threadIdx.x];
+            const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+            const int j0 = lo + q * kDecGroupFrames;
+            if (!splice) {
+                uint32_t o[28];
+#pragma unroll
+                for (int fr = 0; fr < kDecGroupFrames; fr++) {
+                    gc_decode_frame(w[2 * fr], w[2 * fr + 1], pairs, st, o + 7 * fr);
+                    finish(j0 + fr);
+                }
+                uint4 *vout = reinterpret_cast<uint4 *>(dst + (int64_t)j0 * kGcFrameSamples);
+#pragma unroll
+                for (int k = 0; k < 7; k++) vout[k] = make_uint4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
+            } else {
+#pragma unroll
+                for (int fr = 0; fr < kDecGroupFrames; fr++) {
+                    uint32_t o[7];
+                    gc_decode_frame(w[2 * fr], w[2 * fr + 1], pairs, st, o);
+                    store7(j0 + fr, o);
+                    if (finish(j0 + fr)) { stop = true; break; }
+                }
+            }
+        }
+        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        if (stop) return done;
+        for (int j = lo + groups * kDecGroupFrames; j < hi; j++) {  // whole frames short of a group: 8-byte loads
+            const uint2 v = *reinterpret_cast<const uint2 *>(src + (int64_t)j * kGcFrameBytes);
+            uint32_t o[7];
+            gc_decode_frame(v.x, v.y, pairs, st, o);
+            store7(j, o);
+            if (finish(j) && splice) break;
+        }
+        return done;
+    };
+    // the partial last frame from the true pair after the full frames: byte loads, only the samples that exist
+    auto tail = [&](DecState &st) {
+        if (frames <= full) return;
+        const int take = n - full * kGcFrameSamples;
+        const int bytes = 1 + (take + 1) / 2;
+        uint32_t w[2] = {0, 0};
+        for (int j = 0; j < bytes; j++) w[j >> 2] |= (uint32_t)src[(int64_t)full * kGcFrameBytes + j] << ((j & 3) * 8);
+        uint32_t o[7];
+        gc_decode_frame(w[0], w[1], pairs, st, o);
+        int16_t *d = dst + (int64_t)full * kGcFrameSamples;
+        for (int k = 0; k < take; k++) d[k] = (int16_t)((o[k >> 1] >> ((k & 1) * 16)) & 0xFFFFu);
+    };
+    // GcAdpcmDecoder indexes coefficients[predictor * 2] on every frame that yields samples: 8..15 throws there
+    auto report = [&](const DecState &st) { if (st.heads & 0x80u) atomicOr(&sa.status[ch], 1); };
+    auto from_pair = [](uint32_t pair) { return DecState{(int32_t)(pair & 0xFFFFu), (int32_t)(pair >> 16), 0u}; };
+
+    if (kMode == kGcChain) {
+        const int lo = seg_lo(s), hi = seg_lo(s + 1);
+        if (s > 0 && lo >= hi) return;
+        DecState st = s == 0 ? DecState{c.hist1 + 32768, c.hist2 + 32768, 0u} : DecState{32768, 32768, 0u};  // a guess but for s = 0
+        run(lo, hi, st, false);
+        if (s == 0 && (sa.seg_count == 1 || full == 0)) tail(st);  // else the cascade decodes it from the true pair
+        report(st);
+        return;
+    }
+    if (kMode == kGcRunOn) {
+        const int lo = seg_lo(s), hi = seg_lo(s + 1);
+        if (lo >= hi) return;
+        const uint32_t start = trace[lo - 1];
+        sa.used_start[(int64_t)ch * kGcDecMaxSegments + s] = start;
+        DecState st = from_pair(start);
+        const int done = run(lo, hi, st, true);
+        atomicAdd(&sa.stats[0], (unsigned long long)done);
+        atomicMax(&sa.stats[3], (unsigned long long)done);
+        return;
+    }
+    // cascade: one thread per channel walks the boundaries in order
+    int truth_upto = 0;
+    for (int k = 1; k < sa.seg_count; k++) {
+        const int lo = seg_lo(k);
+        if (lo >= full) break;
+        if (lo < truth_upto) continue;
+        const uint32_t start = trace[lo - 1];
+        if (start == sa.used_start[(int64_t)ch * kGcDecMaxSegments + k]) continue;
+        DecState st = from_pair(start);
+        const int done = run(lo, full, st, true);
+        truth_upto = lo + done;
+        atomicAdd(&sa.stats[1], (unsigned long long)done);
+        atomicAdd(&sa.stats[2], 1ull);
+    }
+    if (full == 0) return;  // segment 0's chain decoded the whole channel
+    DecState st = from_pair(trace[full - 1]);
+    tail(st);
+    report(st);
+}
+
+// Segments per channel of the time-parallel decode: about four waves of threads over the SMs, no segment shorter than
+// the minimum, at most kGcDecMaxSegments (VGB_GC_DEC_SEGMENTS / VGB_GC_DEC_MIN_SEG_FRAMES override both, read per call).
+int gc_decode_pick_segments(int n_channels, int max_full_frames, int *min_seg_out)
+{
+    int min_seg = kGcDecMinSegFrames;
+    if (const char *env = std::getenv("VGB_GC_DEC_MIN_SEG_FRAMES")) {
+        const int v = std::atoi(env);
+        if (v >= 1) min_seg = v;
+    }
+    if (min_seg_out) *min_seg_out = min_seg;
+    if (const char *env = std::getenv("VGB_GC_DEC_SEGMENTS")) {
+        const int v = std::atoi(env);
+        if (v >= 1) return std::min(v, kGcDecMaxSegments);
+    }
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) {
+        (void)cudaGetLastError();
+        sms = 132;  // H100 SXM
+    }
+    const long long want = (4ll * sms * 512 + n_channels - 1) / std::max(n_channels, 1);
+    const int max_s = std::max(1, std::min(kGcDecMaxSegments, max_full_frames / min_seg));
+    return (int)std::max<long long>(1, std::min<long long>(want, max_s));
+}
+
+void launch_gc_decode_seg(const uint8_t *adpcm, const GcDecChannel *tab, int n_channels, int16_t *pcm, GcDecSegArgs sa,
+                          cudaStream_t stream)
+{
+    if (n_channels <= 0) return;
+    auto blocks = [&](int per_ch) { return (unsigned)(((int64_t)n_channels * per_ch + kSegThreads - 1) / kSegThreads); };
+    gc_decode_seg_kernel<kGcChain><<<blocks(sa.seg_count), kSegThreads, 0, stream>>>(adpcm, tab, n_channels, pcm, sa);
+    if (sa.seg_count > 1) {
+        gc_decode_seg_kernel<kGcRunOn><<<blocks(sa.seg_count - 1), kSegThreads, 0, stream>>>(adpcm, tab, n_channels, pcm, sa);
+        gc_decode_seg_kernel<kGcCascade><<<blocks(1), kSegThreads, 0, stream>>>(adpcm, tab, n_channels, pcm, sa);
+    }
 }
 
 }  // namespace vgb

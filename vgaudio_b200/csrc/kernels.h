@@ -36,6 +36,11 @@ void launch_gc_encode_frames(int16_t *pcm_in_out, const int32_t *sample_count, c
 void launch_gc_decode(const uint8_t *adpcm, const GcChannelTable &tab, const int16_t *coefs, int16_t *pcm,
                       int max_frames, int frame_begin, int frame_end, cudaStream_t stream);
 
+// the time-parallel decode (chain / run-on / cascade); seg.trace, seg.status and seg.stats live in the caller's workspace
+int gc_decode_pick_segments(int n_channels, int max_full_frames, int *min_seg_out);
+void launch_gc_decode_seg(const uint8_t *adpcm, const GcDecChannel *tab, int n_channels, int16_t *pcm, GcDecSegArgs seg,
+                          cudaStream_t stream);
+
 // seek table (GcAdpcmSeekTable.cs:25-38) and loop context (GcAdpcmLoopContext.cs:17-26) of already encoded channels
 void launch_gc_taps(const uint8_t *adpcm, const GcChannelTable &tab, const int16_t *coefs, const GcTapChannel *taps,
                     int16_t *tap_slab, int max_frames, cudaStream_t stream);
