@@ -45,11 +45,11 @@ int32_t vgb_init(int32_t device, uint32_t flags);
 int32_t vgb_shutdown(void);
 /* Bind several devices (SURVEY §8b's vgb_init(n_devices, flags); the reference's counterpart is Parallel.ForEach over
  * files, src/VGAudio.Cli/Batch.cs:24-25).  devices[0] becomes the primary device (the one the *_dev entry points, timers
- * and debug taps use); every host-pointer codec *_batch call and both batch converters (vgb_convert_wave_batch,
- * vgb_convert_dsp_to_wave_batch) are then sharded over all bound devices by greedy longest-first bin packing of the
- * units' sample counts - one worker thread and one H2D / kernel / D2H pipeline per device, each over its own PCIe link,
- * results written straight into the caller's arrays (no collective: host data reaches a GPU fastest over that GPU's own
- * link).  The single-shot container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.
+ * and debug taps use); every host-pointer codec *_batch call and every batch converter (vgb_convert_wave_batch,
+ * vgb_convert_{dsp,hca,adx,nw}_to_wave_batch, vgb_transcode_batch) are then sharded over all bound devices by greedy
+ * longest-first bin packing of the units' sample or frame counts - one worker thread and one H2D / kernel / D2H pipeline
+ * per device, each over its own PCIe link, results written straight into the caller's arrays (no collective: host data
+ * reaches a GPU fastest over that GPU's own link).  The single-shot container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.
  * A device may be listed more than once. */
 int32_t vgb_init_devices(const int32_t *devices, int32_t n_devices, uint32_t flags);
 int32_t vgb_device_count(void);
