@@ -70,6 +70,9 @@ namespace VGAudio.Native
         public static extern int vgb_adx_debug_decode_stats(ulong* output, int n);
 
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_adx_debug_encode_stats(ulong* output, int n);
+
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_hca_query(VgbHcaParams* parameters, VgbHcaInfo* infoOut);
 
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]

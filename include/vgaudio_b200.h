@@ -332,6 +332,15 @@ uint64_t vgb_adx_workspace_bytes(int64_t total_samples, int32_t n_channels);
 int32_t vgb_adx_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, const int32_t *n_samples, const vgb_adx_params *params,
                            int32_t n_channels, int16_t *d_history_out, uint8_t *d_adpcm, const int64_t *adpcm_offset,
                            void *d_workspace, uint64_t workspace_bytes, void *cuda_stream);
+/* Bookkeeping of the most recent ADX encode launch on this thread's context (vgb_adx_encode_batch: its last channel group;
+ * vgb_adx_encode_dev: the call), whose 18-byte channels without padding are cut into segments encoded concurrently and
+ * spliced at the boundaries (adx.cu): out[0] segments per channel, out[1] the shortest segment in frames, out[2] frames
+ * re-encoded by the boundary run-ons, out[3] frames re-encoded by the serial cascade (boundaries whose run-on did not
+ * lock inside its segment), out[4] boundaries the cascade repaired.  A single-segment launch leaves out[2..4] zero.
+ * n = how many words to fill (up to 5).  Synchronises the device.  The words live in the workspace of that launch: after
+ * a vgb_adx_encode_dev the caller's workspace must still be allocated (and not yet reused) when this is called.
+ * VGB_ADX_SEGMENTS / VGB_ADX_MIN_SEG_FRAMES in the environment force the segment count and the shortest segment. */
+int32_t vgb_adx_debug_encode_stats(uint64_t *out, int32_t n);
 
 /* CriAdxCodec.Decode(byte[] adpcm, int sampleCount, CriAdxParameters config) (CriAdxCodec.cs:9-54).
  * n_bytes[c] = length of adpcm[c]; pcm_out[c] receives sample_count[c] samples.

@@ -77,40 +77,77 @@ static int32_t short_to_nibble(int32_t sample)
     return sat4(sample);
 }
 
-/* EncodeFrame (:107-147).  pcm[0..1] = history, pcm[2..] = samples; rewritten with the reconstruction. */
-void vgo_adx_encode_frame(int16_t *pcm, uint8_t *adpcm_out, const int16_t coefs[2], int samples_per_frame, int type,
-                          int version)
+/* EncodeFrame (:107-147).  pcm[0..1] = history, pcm[2..] = samples; rewritten with the reconstruction.  rec == NULL on
+ * the normal path; otherwise the frame's facts are added to it (recording reads values the frame computes anyway). */
+static void encode_frame(int16_t *pcm, uint8_t *adpcm_out, const int16_t coefs[2], int samples_per_frame, int type,
+                         int version, vgo_adx_frame_trace *rec)
 {
     int max_distance = 0;
-    int32_t nib[256];
+    int32_t nib[512];
+    if (rec) { rec->hist_in[0] = pcm[1]; rec->hist_in[1] = pcm[0]; }
     for (int i = 0; i < samples_per_frame; i++) {
         int32_t predicted = (wmul(pcm[i + 1], coefs[0]) >> 12) + (wmul(pcm[i], coefs[1]) >> 12);
-        int32_t distance = abs(sat16(pcm[i + 2] - predicted));
+        int32_t d = pcm[i + 2] - predicted;
+        int32_t distance = abs(sat16(d));
+        if (rec) { rec->clip1_hi += d > 32767; rec->clip1_lo += d < -32768; }
         if (distance > max_distance) max_distance = distance;
     }
     double gain;
     int scale_out;
+    if (rec) {
+        rec->max_distance = max_distance;
+        rec->scale_raw = (max_distance - 1) / 7 + 1;
+        rec->scale_lin = (rec->scale_raw > 0x1000 ? 0x1000 : rec->scale_raw) - 1;
+        rec->power = type == 4 ? (rec->scale_lin == 0 ? 0 : floor_log2(rec->scale_lin) + 1) : -1;
+    }
     int scale = calc_scale(max_distance, &gain, &scale_out, type == 4);
+    /* the maxDistance the gain is computed from (8 * scale - 1 for the Exponential type) */
+    const int md_gain = type == 4 ? 8 * scale - 1 : max_distance;
+    if (rec) { rec->scale_out = scale_out; rec->md_gain = md_gain; }
 
     for (int i = 0; i < samples_per_frame; i++) {
         int32_t predicted = (wmul(pcm[i + 1], coefs[0]) >> 12) + (wmul(pcm[i], coefs[1]) >> 12);
+        int32_t v4_predicted = wadd(wmul(pcm[i + 1], coefs[0]), wmul(pcm[i], coefs[1])) >> 12;
         int32_t raw = pcm[i + 2] - predicted;
-        int32_t scaled = sat16(cast_double_to_int(raw * gain));
+        int32_t cast = cast_double_to_int(raw * gain);
+        int32_t scaled = sat16(cast);
         int32_t q = short_to_nibble(scaled);
         nib[i] = q;
         int32_t decoded_distance = sat16(wmul(scale, q));
-        if (version == 4) predicted = wadd(wmul(pcm[i + 1], coefs[0]), wmul(pcm[i], coefs[1])) >> 12;
-        pcm[i + 2] = (int16_t)sat16(decoded_distance + predicted);
+        if (version == 4) predicted = v4_predicted;
+        int32_t recon = decoded_distance + predicted;
+        if (rec) {
+            double prod = raw * gain;
+            rec->cast_ovf += !(prod > -2147483649.0 && prod < 2147483648.0);
+            rec->clip2_hi += cast > 32767;
+            rec->clip2_lo += cast < -32768;
+            rec->nibbles[q & 15]++;
+            if (md_gain > 0)
+                for (int k = 1; k <= 7; k++)
+                    rec->ties[k] += (int64_t)abs(raw) * 32767 == (int64_t)(4681 * k - 2340) * md_gain;
+            rec->recon_hi += recon > 32767;
+            rec->recon_lo += recon < -32768;
+            rec->v4_differs += v4_predicted != (wmul(pcm[i + 1], coefs[0]) >> 12) + (wmul(pcm[i], coefs[1]) >> 12);
+        }
+        pcm[i + 2] = (int16_t)sat16(recon);
     }
     adpcm_out[0] = (uint8_t)((scale_out >> 8) & 0x1f);
     adpcm_out[1] = (uint8_t)scale_out;
     for (int i = 0; i < samples_per_frame / 2; i++)
         adpcm_out[i + 2] = (uint8_t)((nib[2 * i] << 4) | (nib[2 * i + 1] & 0xF));
+    if (rec) { rec->hist_out[0] = pcm[samples_per_frame + 1]; rec->hist_out[1] = pcm[samples_per_frame]; }
 }
 
-/* Encode (:56-105).  Returns the value the reference leaves in config.History (:73), 0 if untouched. */
-int vgo_adx_encode(const int16_t *pcm, int pcm_length, int sample_rate, int frame_size, int version, int padding,
-                   int type, int filter, uint8_t *adpcm_out)
+void vgo_adx_encode_frame(int16_t *pcm, uint8_t *adpcm_out, const int16_t coefs[2], int samples_per_frame, int type,
+                          int version)
+{
+    encode_frame(pcm, adpcm_out, coefs, samples_per_frame, type, version, NULL);
+}
+
+/* Encode (:56-105).  Returns the value the reference leaves in config.History (:73), 0 if untouched.  trace == NULL on
+ * the normal path, else one record per frame. */
+static int encode(const int16_t *pcm, int pcm_length, int sample_rate, int frame_size, int version, int padding, int type,
+                  int filter, uint8_t *adpcm_out, vgo_adx_frame_trace *trace)
 {
     int sample_count = pcm_length + padding;
     int spf = (frame_size - 2) * 2;
@@ -123,6 +160,7 @@ int vgo_adx_encode(const int16_t *pcm, int pcm_length, int sample_rate, int fram
     int16_t *buf = calloc((size_t)spf + 2, sizeof(int16_t));
     uint8_t *frame = calloc((size_t)frame_size, 1);
     memset(adpcm_out, 0, (size_t)frame_count * frame_size);
+    if (trace) memset(trace, 0, (size_t)frame_count * sizeof *trace);
     int history = 0;
     if (version == 4 && padding == 0 && pcm_length > 0) {
         buf[0] = pcm[0];
@@ -133,15 +171,22 @@ int vgo_adx_encode(const int16_t *pcm, int pcm_length, int sample_rate, int fram
         int to_copy = sample_count - i * spf;
         if (to_copy > spf) to_copy = spf;
         int start = 2;
+        vgo_adx_frame_trace *rec = trace ? trace + i : NULL;
+        if (rec) { rec->frame = i; rec->power = -1; }
         if (padding_remaining != 0) {
             while (padding_remaining > 0 && to_copy > 0) { padding_remaining--; to_copy--; start++; }
-            if (to_copy == 0) continue;
+            if (rec && start > 2) rec->layout |= VGO_ADX_FRAME_PADDED;
+            if (to_copy == 0) {
+                if (rec) rec->layout |= VGO_ADX_FRAME_SKIPPED;
+                continue;
+            }
         }
+        if (rec && start - 2 + to_copy < spf) rec->layout |= VGO_ADX_FRAME_PARTIAL;
         int src = i * spf - padding;
         if (src < 0) src = 0;
         memcpy(buf + start, pcm + src, (size_t)to_copy * sizeof(int16_t));
         memset(buf + start + to_copy, 0, (size_t)(spf - to_copy - start + 2) * sizeof(int16_t));
-        vgo_adx_encode_frame(buf, frame, coefs, spf, type, version);
+        encode_frame(buf, frame, coefs, spf, type, version, rec);
         if (type == 2) frame[0] |= (uint8_t)(filter << 5);
         memcpy(adpcm_out + (size_t)i * frame_size, frame, (size_t)frame_size);
         buf[0] = buf[spf];
@@ -151,6 +196,20 @@ int vgo_adx_encode(const int16_t *pcm, int pcm_length, int sample_rate, int fram
     free(frame);
     return history;
 }
+
+int vgo_adx_encode(const int16_t *pcm, int pcm_length, int sample_rate, int frame_size, int version, int padding,
+                   int type, int filter, uint8_t *adpcm_out)
+{
+    return encode(pcm, pcm_length, sample_rate, frame_size, version, padding, type, filter, adpcm_out, NULL);
+}
+
+int vgo_adx_encode_trace(const int16_t *pcm, int pcm_length, int sample_rate, int frame_size, int version, int padding,
+                         int type, int filter, uint8_t *adpcm_out, vgo_adx_frame_trace *trace_out)
+{
+    return encode(pcm, pcm_length, sample_rate, frame_size, version, padding, type, filter, adpcm_out, trace_out);
+}
+
+int vgo_adx_frame_trace_size(void) { return (int)sizeof(vgo_adx_frame_trace); }
 
 /* Decode (:9-54) */
 void vgo_adx_decode(const uint8_t *adpcm, int sample_count, int sample_rate, int highpass_freq, int frame_size,

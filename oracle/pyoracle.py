@@ -220,6 +220,32 @@ def adx_encode(pcm, sample_rate=48000, frame_size=18, version=4, padding=0, type
     return out, hist
 
 
+ADX_FRAME_SKIPPED, ADX_FRAME_PADDED, ADX_FRAME_PARTIAL = 1, 2, 4
+ADX_FRAME_TRACE = np.dtype([("frame", np.int32), ("layout", np.int32), ("hist_in", np.int32, 2), ("hist_out", np.int32, 2),
+                            ("max_distance", np.int32), ("clip1_hi", np.int32), ("clip1_lo", np.int32),
+                            ("scale_raw", np.int32), ("scale_lin", np.int32), ("scale_out", np.int32), ("power", np.int32),
+                            ("md_gain", np.int32), ("nibbles", np.int32, 16), ("ties", np.int32, 8), ("cast_ovf", np.int32),
+                            ("clip2_hi", np.int32), ("clip2_lo", np.int32), ("recon_hi", np.int32), ("recon_lo", np.int32),
+                            ("v4_differs", np.int32)], align=True)
+
+
+def adx_encode_trace(pcm, sample_rate=48000, frame_size=18, version=4, padding=0, type=ADX_LINEAR, filter=0):
+    """adx_encode() plus one vgo_adx_frame_trace record per frame: (adpcm bytes, History, trace)."""
+    L = lib()
+    if not getattr(L, "_adx_trace_ready", False):
+        L.vgo_adx_encode_trace.argtypes = [C.c_void_p] + [C.c_int] * 7 + [C.c_void_p, C.c_void_p]
+        if L.vgo_adx_frame_trace_size() != ADX_FRAME_TRACE.itemsize:
+            raise RuntimeError("vgo_adx_frame_trace layout differs from ADX_FRAME_TRACE")
+        L._adx_trace_ready = True
+    pcm = np.ascontiguousarray(pcm, dtype=np.int16)
+    n_bytes = L.vgo_adx_encoded_byte_count(len(pcm), padding, frame_size)
+    out = np.zeros(n_bytes, dtype=np.uint8)
+    trace = np.zeros(n_bytes // frame_size, dtype=ADX_FRAME_TRACE)
+    hist = L.vgo_adx_encode_trace(pcm.ctypes.data, len(pcm), sample_rate, frame_size, version, padding, type, filter,
+                                  out.ctypes.data, trace.ctypes.data)
+    return out, hist, trace
+
+
 def adx_decode(adpcm, sample_count, sample_rate=48000, highpass_freq=500, frame_size=18, version=4, history=0,
                padding=0, type=ADX_LINEAR):
     adpcm = np.ascontiguousarray(adpcm, dtype=np.uint8)

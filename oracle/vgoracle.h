@@ -137,6 +137,32 @@ void vgo_adx_encode_frame(int16_t *pcm, uint8_t *adpcm_out, const int16_t coefs[
 /* Encode :56-105; returns the History value the reference writes back into the config (:73) */
 int vgo_adx_encode(const int16_t *pcm, int pcm_length, int sample_rate, int frame_size, int version, int padding,
                    int type, int filter, uint8_t *adpcm_out);
+/* Encode with one record per frame of the facts of EncodeFrame's rare paths (:107-171), so that tests can show which of
+ * them an input reaches.  Same bytes and return value as vgo_adx_encode; recording only reads values the frame computes
+ * anyway.  A frame the padding skips (`continue`, :87) keeps a zero record apart from frame, layout and power = -1. */
+enum { VGO_ADX_FRAME_SKIPPED = 1 /* all padding: `continue`, the frame stays zero */,
+       VGO_ADX_FRAME_PADDED = 2 /* leading padding samples */, VGO_ADX_FRAME_PARTIAL = 4 /* zero-filled tail */ };
+typedef struct vgo_adx_frame_trace {
+    int32_t frame, layout;       /* frame index, VGO_ADX_FRAME_* */
+    int32_t hist_in[2];          /* (hist1, hist2) the frame starts from: pcmBuffer[1], pcmBuffer[0] */
+    int32_t hist_out[2];         /* the reconstructed pair it hands on */
+    int32_t max_distance;        /* pass 1 (:112-118) */
+    int32_t clip1_hi, clip1_lo;  /* pass-1 distances Clamp16 clipped at +32767 / -32768 */
+    int32_t scale_raw;           /* CalculateScale (:149-165): (maxDistance - 1) / 7 + 1 before the 0x1000 clamp */
+    int32_t scale_lin;           /* scale - 1 after the clamp: the Linear scaleOut, the Exponential power's argument */
+    int32_t scale_out;           /* the value written to the header */
+    int32_t power;               /* Exponential: the power of two (0..12); -1 for the other types */
+    int32_t md_gain;             /* the maxDistance of gain = 32767 / maxDistance (8 * scale - 1 for Exponential) */
+    int32_t nibbles[16];         /* histogram of the written nibbles, by nibble & 15 */
+    int32_t ties[8];             /* [k], k = 1..7: samples with |raw| * 32767 == (4681 k - 2340) * md_gain */
+    int32_t cast_ovf;            /* raw * gain outside int32: (int) gives INT_MIN */
+    int32_t clip2_hi, clip2_lo;  /* Clamp16 of the scaled distance (:126) */
+    int32_t recon_hi, recon_lo;  /* Clamp16 of the reconstruction (:133) */
+    int32_t v4_differs;          /* samples where version 4's prediction differs from version 3's */
+} vgo_adx_frame_trace;
+int vgo_adx_encode_trace(const int16_t *pcm, int pcm_length, int sample_rate, int frame_size, int version, int padding,
+                         int type, int filter, uint8_t *adpcm_out, vgo_adx_frame_trace *trace_out);
+int vgo_adx_frame_trace_size(void); /* sizeof(vgo_adx_frame_trace), checked by the Python wrapper */
 /* Decode :9-54 */
 void vgo_adx_decode(const uint8_t *adpcm, int sample_count, int sample_rate, int highpass_freq, int frame_size,
                     int version, int history, int padding, int type, int16_t *pcm_out);

@@ -123,6 +123,12 @@ def test_adx_host_helpers_match_the_oracle(vg, oracle):
         for hp in (0, 1, 100, 500, 1000, rate // 4):
             assert vg.lib.vgb_adx_calculate_coefficients(hp, rate, out.ctypes.data) == 0
             assert out.tolist() == oracle.adx_coefficients(hp, rate).tolist(), (hp, rate)
+    # the encoder's own pair (500 Hz) at every rate 1..4000: below 1000 Hz cos(2 pi 500 / rate) stops looking like a
+    # high-pass filter, and at every divisor of 500 the pair is (8192, -4096)
+    for rate in range(1, 4001):
+        for hp in (500, rate // 2, rate):
+            assert vg.lib.vgb_adx_calculate_coefficients(hp, rate, out.ctypes.data) == 0
+            assert out.tolist() == oracle.adx_coefficients(hp, rate).tolist(), (hp, rate)
     L = oracle.lib()
     for n in (0, 1, 31, 32, 33, 1000, 123457):
         for padding in (0, 1, 31, 32, 100):

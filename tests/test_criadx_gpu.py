@@ -104,7 +104,7 @@ def test_errors(vg):
 def test_time_parallel_encode_is_bit_exact(vg, oracle, seg):
     """The ADX encoder cuts a channel's whole frames into segments encoded concurrently from raw history and splices them
     at the boundaries (adx.cu); VGB_ADX_SEGMENTS forces the count.  Mixed batch: every type / version, ragged lengths with
-    partial last frames, full-scale noise and squares (slow to re-lock), and channels the segmentation must leave to the
+    partial last frames, full-scale noise and squares (slow to re-lock), 500 Hz noise (never re-locks), and channels the segmentation must leave to the
     serial loop (another frame size, padding)."""
     import os
 
@@ -116,6 +116,8 @@ def test_time_parallel_encode_is_bit_exact(vg, oracle, seg):
     cfgs = [_cfg(vg, sample_rate=48000, version=4 - (i % 2), type=2 + (i % 3), filter=i % 4) for i in range(len(chans))]
     cfgs[8] = _cfg(vg, sample_rate=44100, frame_size=34, version=4, type=3)   # not the standard layout
     cfgs[9] = _cfg(vg, sample_rate=48000, padding=45, version=4, type=3)      # padded stream
+    chans.append(rng.integers(-6000, 6000, 32 * 2400 + 5).astype(np.int16))   # never re-locks at 500 Hz: the cascade
+    cfgs.append(_cfg(vg, sample_rate=500, version=4, type=3))
     saved = {k: os.environ.get(k) for k in ("VGB_ADX_SEGMENTS", "VGB_ADX_MIN_SEG_FRAMES")}
     os.environ["VGB_ADX_MIN_SEG_FRAMES"] = "256"  # the default (4096) is sized for the run-on tail; short inputs must still be cut
     if seg is None:

@@ -200,6 +200,7 @@ SIGNATURES = {
                                        C.c_void_p, C.c_uint64, C.c_void_p]),
     "vgb_adx_decode_dev_status": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p]),
     "vgb_adx_debug_decode_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
+    "vgb_adx_debug_encode_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_adx_workspace_bytes": (C.c_uint64, [C.c_int64, C.c_int32]),
     "vgb_adx_encode_dev": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_void_p, C.c_uint64, C.c_void_p]),

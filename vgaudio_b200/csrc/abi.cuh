@@ -112,7 +112,8 @@ struct Context {
     bool ev_used[kTimers] = {};
     std::atomic<int64_t> launches{0};
     GcSegArgs last_seg{};            // bookkeeping of the most recent encode launch (vgb_gcadpcm_debug_splice_stats)
-    AdxDecSegArgs last_adx_dec{};    // the same for the most recent time-parallel ADX decode (vgb_adx_debug_decode_stats)
+    AdxSegArgs last_adx_enc{};       // the same for the most recent ADX encode launch (vgb_adx_debug_encode_stats)
+    AdxDecSegArgs last_adx_dec{};    // and time-parallel ADX decode (vgb_adx_debug_decode_stats)
     GcDecSegArgs last_gc_dec{};      // and GC-ADPCM decode (vgb_gcadpcm_debug_decode_stats)
     HcaTableStore hca_tables;
     std::atomic<ContainerState *> containers{nullptr};  // created on first use, released by containers_release

@@ -169,6 +169,7 @@ static int32_t adx_encode_one(const int16_t *const *pcm, const int32_t *n_sample
         launch_adx_encode(static_cast<const int16_t *>(g_ctx.pcm.p), d_tab + c0, n, static_cast<uint8_t *>(g_ctx.adpcm.p), d_hist + c0, seg[g], st);
         if (n_groups == 1) tick(4, false, st);
         g_ctx.launches += seg[g].seg_count > 1 ? 3 : 1;
+        g_ctx.last_adx_enc = seg[g];
         CUDA_TRY(cudaGetLastError());
         return VGB_OK;
     };
@@ -203,6 +204,21 @@ int32_t vgb_adx_encode_batch(const int16_t *const *pcm, const int32_t *n_samples
         if (history_out) put_rows(history_out, u, s_hist);
         return VGB_OK;
     });
+}
+
+/* Bookkeeping of the most recent ADX encode launch on this thread's context (see the header).  Synchronises the device. */
+int32_t vgb_adx_debug_encode_stats(uint64_t *out, int32_t n)
+{
+    if (!out || n < 0) return fail(VGB_E_ARG, "bad arguments");
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    for (int i = 0; i < n; i++) out[i] = 0;
+    if (!g_ctx.ready || !g_ctx.last_adx_enc.stats) return VGB_OK;
+    unsigned long long st[3] = {};
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(st, g_ctx.last_adx_enc.stats, sizeof st, cudaMemcpyDeviceToHost));
+    const uint64_t words[5] = {(uint64_t)g_ctx.last_adx_enc.seg_count, (uint64_t)g_ctx.last_adx_enc.min_seg_frames, st[0], st[1], st[2]};
+    for (int i = 0; i < n && i < 5; i++) out[i] = words[i];
+    return VGB_OK;
 }
 
 /* ---- device-resident ADX encode (see the header) ---- */
@@ -250,6 +266,7 @@ int32_t vgb_adx_encode_dev(const int16_t *d_pcm, const int64_t *pcm_offset, cons
     launch_adx_encode(d_pcm, reinterpret_cast<const AdxChannel *>(ws), n_channels, d_adpcm, d_hist, seg, st);
     tick(4, false, st);
     g_ctx.launches += seg.seg_count > 1 ? 3 : 1;
+    g_ctx.last_adx_enc = seg;
     CUDA_TRY(cudaGetLastError());
     return VGB_OK;
 }
