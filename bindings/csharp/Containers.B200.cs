@@ -63,7 +63,7 @@ namespace VGAudio.Native
     [StructLayout(LayoutKind.Sequential)]
     internal struct VgbConvertOptions
     {
-        public int OutType;                 // 1 .dsp, 2 .adx, 3 .hca
+        public int OutType;                 // 1 .dsp, 2 .adx, 3 .hca, 4 .brstm, 5 .bcstm, 6 .bfstm
         public int NoTrim;
         public int DspSamplesPerInterleave, DspLoopPointAlignment;
         public int AdxVersion, AdxFrameSize, AdxType, AdxFilterPlus1;
@@ -73,6 +73,10 @@ namespace VGAudio.Native
         public int Reserved;
         public ulong HcaKeyCode;
         public long GroupBytes;
+        public int NwCodecPlus1;            // 0 = GC-ADPCM; else NwCodec + 1
+        public int NwEndianness;            // 0 = the target's, 1 = little, 2 = big (BRSTM is always big)
+        public int NwLoopPointAlignment;    // 0 = BytesToSamples(0x2000, codec)
+        public int NwPad;
     }
 
     internal static unsafe class VgAudioB200Containers

@@ -626,7 +626,13 @@ int32_t vgb_hca_write_batch(const vgb_hca_info *info, int32_t n_files, const uin
 #define VGB_CONTAINER_DSP 1
 #define VGB_CONTAINER_ADX 2
 #define VGB_CONTAINER_HCA 3
-#define VGB_CONTAINER_BRSTM 4 /* NintendoWare streams: readers only (vgb_convert_nw_to_wave_batch) */
+/* NintendoWare streams (BrstmWriter, BCFstmWriter with BxstmConfiguration's defaults: interleave 0x2000 bytes, a seek
+ * entry every 0x2000 bytes' worth of samples, BRSTM standard track and seek-table types, BCSTM version 2.1, BFSTM
+ * version 0.3, seek table and loop context recalculated).  vgb_convert_wave_batch writes them; vgb_transcode_batch does
+ * not take them as a target; vgb_convert_nw_to_wave_batch reads them.  A looping GC-ADPCM file whose loop start is not
+ * a multiple of the loop point alignment goes through GcAdpcmFormat.WithAlignment as in the reference: the loop moves
+ * to the next multiple and the tail behind the kept frames is re-encoded on the device. */
+#define VGB_CONTAINER_BRSTM 4
 #define VGB_CONTAINER_BCSTM 5
 #define VGB_CONTAINER_BFSTM 6
 typedef struct vgb_convert_options {
@@ -640,6 +646,11 @@ typedef struct vgb_convert_options {
     int32_t reserved;
     uint64_t hca_key_code;
     int64_t group_bytes;                /* input bytes per GPU batch; 0 = an eighth of the job, 64..512 MiB */
+    /* NintendoWare targets (BxstmConfiguration); zero selects the reference's default */
+    int32_t nw_codec_plus1;             /* 0 = GC-ADPCM; else NwCodec + 1: 1 = PCM8, 2 = PCM16, 3 = GC-ADPCM */
+    int32_t nw_endianness;              /* 0 = the target's (BCSTM little, BFSTM big), 1 = little, 2 = big; BRSTM is always big */
+    int32_t nw_loop_point_alignment;    /* 0 = BytesToSamples(0x2000, codec) (14336 for GC-ADPCM) */
+    int32_t nw_pad;
 } vgb_convert_options;
 /* Pass files_out == NULL for the sizing pass: out_sizes[i] = size of output i (0 for a file that failed), status_out[i]
  * (may be NULL) = VGB_OK or the error of file i - a bad file does not stop the batch (Batch.cs:39-43).  The sizing pass

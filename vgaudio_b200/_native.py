@@ -137,7 +137,8 @@ class VgbConvertOptions(C.Structure):
                                          "adx_version", "adx_frame_size", "adx_type", "adx_filter_plus1",
                                          "adx_encryption_type", "adx_has_key", "adx_key_seed", "adx_key_mult", "adx_key_inc",
                                          "hca_quality", "hca_bitrate", "hca_limit_bitrate", "hca_key_type", "reserved")] + [
-        ("hca_key_code", C.c_uint64), ("group_bytes", C.c_int64)]
+        ("hca_key_code", C.c_uint64), ("group_bytes", C.c_int64)] + [
+        (n, C.c_int32) for n in ("nw_codec_plus1", "nw_endianness", "nw_loop_point_alignment", "nw_pad")]
 
 
 PROGRESS_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_int64)

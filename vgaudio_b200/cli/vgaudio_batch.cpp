@@ -1,5 +1,5 @@
 // vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
-// .dsp / .adx / .hca, and .dsp, .adx, .hca, .brstm, .bcstm and .bfstm files to WAVE.
+// .dsp / .adx / .hca, WAVE files to .brstm / .bcstm / .bfstm, and .dsp, .adx, .hca, .brstm, .bcstm and .bfstm files to WAVE.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
@@ -7,7 +7,7 @@
 // (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch for coded files, vgb_convert_*_to_wave_batch for
 // --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
-//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm and .bfstm inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
+//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm and .bfstm inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
@@ -47,8 +47,8 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
 }
 
 // the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, 4 .brstm, 5 .bcstm, 6 .bfstm, -1 none of them.  The
-// extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs): the NintendoWare streams are
-// read (decoded to WAVE), not written.
+// extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs).  The NintendoWare streams are
+// decoded to WAVE with --out-format wav, and written from WAVE inputs only with --out-format brstm|bcstm|bfstm.
 static int kind_of(const fs::path &p)
 {
     std::string ext = p.extension().string();
@@ -60,9 +60,10 @@ static const int32_t kContainerOfKind[3] = {VGB_CONTAINER_DSP, VGB_CONTAINER_HCA
 
 static int usage()
 {
-    std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
+    std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
-                         "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n");
+                         "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
+                         "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian]\n");
     return 2;
 }
 
@@ -109,6 +110,14 @@ int main(int argc, char **argv)
         else if (a == "--version") opt.adx_version = std::atoi(next());
         else if (a == "--chunk-mb") chunk_mb = (size_t)std::atoll(next());
         else if (a == "--devices") { if (!parse_devices(next(), devices)) return usage(); }
+        else if (a == "--loop-align") opt.nw_loop_point_alignment = std::atoi(next());
+        else if (a == "--little-endian") opt.nw_endianness = 1;
+        else if (a == "--big-endian") opt.nw_endianness = 2;
+        else if (a == "-f") {  // NwCodec + 1
+            const std::string c = next();
+            opt.nw_codec_plus1 = strcasecmp(c.c_str(), "pcm8") == 0 ? 1 : strcasecmp(c.c_str(), "pcm16") == 0 ? 2 : strcasecmp(c.c_str(), "gcadpcm") == 0 ? 3 : 0;
+            if (!opt.nw_codec_plus1) return usage();
+        }
         else if (a == "--hcaquality") {
             const std::string q = next();
             const char *names[] = {"", "highest", "high", "middle", "low", "lowest"};
@@ -123,6 +132,9 @@ int main(int argc, char **argv)
     const bool to_wave = fmt == "wav";  // the decode direction: .dsp, .hca and .adx files in, 16-bit WAVE files out
     if (fmt == "dsp") opt.out_type = VGB_CONTAINER_DSP;
     else if (fmt == "adx") opt.out_type = VGB_CONTAINER_ADX;
+    else if (fmt == "brstm") opt.out_type = VGB_CONTAINER_BRSTM;
+    else if (fmt == "bcstm") opt.out_type = VGB_CONTAINER_BCSTM;
+    else if (fmt == "bfstm") opt.out_type = VGB_CONTAINER_BFSTM;
     else if (fmt == "hca") opt.out_type = VGB_CONTAINER_HCA;
     else if (!to_wave) return usage();
     vgb_adx_key adx_key{};  // the CriAdxKey of --keystring / --keycode, for writing .adx files or reading keyed ones
@@ -152,7 +164,8 @@ int main(int argc, char **argv)
         if (!e.is_regular_file()) return;
         const int kind = kind_of(e.path());
         if (kind < 0) return;
-        if (to_wave ? kind != 3 : (kind == 3 || (kind < 3 && kContainerOfKind[kind] != opt.out_type))) files.push_back(e.path());
+        const bool nw_out = opt.out_type >= VGB_CONTAINER_BRSTM;  // NintendoWare targets take WAVE inputs only
+        if (to_wave ? kind != 3 : (kind == 3 || (!nw_out && kind < 3 && kContainerOfKind[kind] != opt.out_type))) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);

@@ -141,10 +141,20 @@ int32_t hca_encode_fault(int32_t status, const char *what, int index);
 int32_t adx_decode_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st);
 // abi_gcadpcm.cu, the time-parallel GC-ADPCM decode of the NintendoWare -> WAVE converter: workspace bytes for
 // n_channels channels holding full_frames full frames in all, the asynchronous decode (tab: host table; trace_off is
-// filled here), and the per-channel status words (bit 0: a predictor 8..15), which synchronise `st`
+// filled here), and the per-channel status words (bit 0: a predictor 8..15), which synchronise `st`.  With d_coefs
+// (16 coefficients per channel, channel-major, on the device) the table's coefficients are taken from there in stream
+// order instead of from `tab`, so an encoder's output can be decoded without a round trip to the host.
 uint64_t gc_decode_seg_workspace_bytes(int32_t n_channels, int64_t full_frames);
-int32_t gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &tab, int16_t *d_pcm, void *d_workspace, cudaStream_t st);
+int32_t gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &tab, int16_t *d_pcm, void *d_workspace, cudaStream_t st,
+                      const int16_t *d_coefs = nullptr);
 int32_t gc_decode_seg_words(const void *d_workspace, int32_t n_channels, int32_t *status, cudaStream_t st);
+// abi_gcadpcm.cu, GcAdpcmAlignment's tail (GcAdpcmAlignment.cs:44-57) on device rows, as vgb_gcadpcm_align_batch runs it:
+// per channel the samples to re-encode from its first decode at d_src + src_off, encoded with its own coefficients
+// (d_coefs, 16 per channel, in `chans` order) from the history in front of the kept frames.  dst_off is filled here;
+// tail_adpcm_off receives each channel's encoded tail as a byte offset into d_workspace.  Asynchronous on `st`.
+uint64_t gc_align_tails_workspace_bytes(const std::vector<GcAlignChannel> &chans);
+int32_t gc_align_tails(const int16_t *d_src, std::vector<GcAlignChannel> &chans, const int16_t *d_coefs, void *d_workspace, cudaStream_t st,
+                       std::vector<int64_t> &tail_adpcm_off);
 void tick(int slot, bool begin, cudaStream_t stream);
 
 // hooks of containers.cu, which keeps its own slabs and streams per context (Context::containers)

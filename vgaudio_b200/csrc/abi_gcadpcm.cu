@@ -412,6 +412,53 @@ int32_t align_plan(const uint8_t *const *adpcm, const int32_t *n_bytes, const vg
     return VGB_OK;
 }
 
+// GcAdpcmAlignment.cs:44-62 on device rows, after the first decode: the tails from that decode (d_src, gc_align_tail_kernel,
+// :44-55), their encode with each channel's own coefficients from the history the tail kernel leaves in the encoder's
+// table (:57), and, with `dec`, their decode (:61).  enc / dec lay the tails out in d_pcm / d_adpcm; their tables go to
+// ws_enc / ws_dec here.  The caller holds g_ctx.mu.
+int32_t align_tails(const int16_t *d_src, const GcAlignChannel *d_chans, const GcLayout &enc, const GcLayout *dec, const int16_t *d_coefs,
+                    int16_t *d_pcm, uint8_t *d_adpcm, char *ws_enc, const GcWorkspace &w_enc, char *ws_dec, const GcWorkspace &w_dec,
+                    cudaStream_t st)
+{
+    const int m = enc.n_channels;
+    if (m == 0) return VGB_OK;
+    VGB_TRY(upload_tables(enc, w_enc, ws_enc, st));
+    if (dec) VGB_TRY(upload_tables(*dec, w_dec, ws_dec, st));
+    const GcChannelTable t_enc = table_view(ws_enc, w_enc, m);
+    const GcChannelTable t_dec = dec ? table_view(ws_dec, w_dec, m) : t_enc;
+    launch_gc_align_tail(d_src, d_chans, m, d_pcm, t_enc.hist, t_dec.hist, st);
+    g_ctx.launches += 1;
+    CUDA_TRY(cudaGetLastError());
+    VGB_TRY(run_gc_encode(d_pcm, enc, d_coefs, const_cast<int16_t *>(d_coefs), d_adpcm, ws_enc, w_enc, st,
+                          /*do_encode=*/true, /*timed=*/false, /*tables_uploaded=*/true));
+    if (dec) {
+        launch_gc_decode(d_adpcm, t_dec, d_coefs, d_pcm, dec->max_frames, 0, INT_MAX, st);
+        g_ctx.launches += dec->max_frames > 0 ? 1 : 0;
+        CUDA_TRY(cudaGetLastError());
+    }
+    return VGB_OK;
+}
+
+// The workspace of vgb::gc_align_tails: [channel table | tail PCM rows | tail ADPCM rows | encoder workspace]
+struct TailWs {
+    GcLayout enc;
+    GcWorkspace w{};
+    size_t o_pcm = 0, o_adpcm = 0, o_enc = 0, total = 0;
+    int32_t build(const std::vector<GcAlignChannel> &chans)
+    {
+        std::vector<int32_t> n(chans.size());
+        for (size_t i = 0; i < chans.size(); i++) n[i] = chans[i].count;
+        VGB_TRY(layout_common(enc, n.data(), nullptr, (int32_t)n.size(), true));
+        layout_pack_offsets(enc);
+        w = carve(enc.rec_total, enc.n_channels);
+        o_pcm = align_up(std::max<size_t>(chans.size(), 1) * sizeof(GcAlignChannel), 256);
+        o_adpcm = o_pcm + align_up((size_t)enc.pcm_total * 2, 256);
+        o_enc = o_adpcm + align_up((size_t)enc.adpcm_total, 256);
+        total = o_enc + w.total;
+        return VGB_OK;
+    }
+};
+
 // One device: H2D of the prefixes, then decode -> tail -> encode (-> decode) on one stream, D2H into the caller's rows
 // and one synchronisation.  A predictor 8..15 below loop_end leaves the lowest such channel in *bad and returns
 // VGB_E_DATA.
@@ -489,24 +536,14 @@ int32_t align_one(const uint8_t *const *adpcm, const int32_t *n_bytes, const int
     CUDA_TRY(cudaMemcpyAsync(g_ctx.coefs.p, co.data(), co.size() * 2, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(g_ctx.misc.p, chans.data(), chans.size() * sizeof(GcAlignChannel), cudaMemcpyHostToDevice, st));
     VGB_TRY(upload_tables(pre, w_pre, g_ctx.ws.p, st));
-    VGB_TRY(upload_tables(enc, w_enc, g_ctx.ws.c() + at_enc, st));
-    VGB_TRY(upload_tables(dec, w_dec, g_ctx.ws.c() + at_dec, st));
     const GcChannelTable t_pre = table_view(g_ctx.ws.p, w_pre, m);
-    const GcChannelTable t_enc = table_view(g_ctx.ws.c() + at_enc, w_enc, m);
-    const GcChannelTable t_dec = table_view(g_ctx.ws.c() + at_dec, w_dec, m);
 
     CUDA_TRY(cudaMemsetAsync(t_pre.status, 0x7f, 4, st));  // "no channel": any index is smaller
     launch_gc_decode(d_adpcm, t_pre, d_coefs, d_pcm, pre.max_frames, 0, INT_MAX, st);           // :41-42
-    launch_gc_align_tail(d_pcm, d_chans, m, d_pcm, t_enc.hist, t_dec.hist, st);                 // :44-55
-    g_ctx.launches += (pre.max_frames > 0 ? 1 : 0) + 1;
+    g_ctx.launches += pre.max_frames > 0 ? 1 : 0;
     CUDA_TRY(cudaGetLastError());
-    VGB_TRY(run_gc_encode(d_pcm, enc, d_coefs, const_cast<int16_t *>(d_coefs), d_adpcm, g_ctx.ws.c() + at_enc, w_enc, st,
-                          /*do_encode=*/true, /*timed=*/false, /*tables_uploaded=*/true));  // :57
-    if (pcm_out) {                                                                             // :61
-        launch_gc_decode(d_adpcm, t_dec, d_coefs, d_pcm, dec.max_frames, 0, INT_MAX, st);
-        g_ctx.launches += dec.max_frames > 0 ? 1 : 0;
-        CUDA_TRY(cudaGetLastError());
-    }
+    VGB_TRY(align_tails(d_pcm, d_chans, enc, pcm_out ? &dec : nullptr, d_coefs, d_pcm, d_adpcm, g_ctx.ws.c() + at_enc, w_enc,
+                        g_ctx.ws.c() + at_dec, w_dec, st));                                    // :44-61
     VGB_TRY(copy_units(cudaMemcpyDeviceToHost, g_ctx.adpcm.c(), enc.adpcm_off.data(), tail_dst.data(), tail_bytes.data(), 0, m, st));
     if (pcm_out) {  // PcmAligned = first decode on [0, keep), the tail's decode on [keep, sample_count_aligned) (:43, :62)
         VGB_TRY(copy_units(cudaMemcpyDeviceToHost, g_ctx.pcm.c(), pre_pcm_b.data(), pcm_pre_dst.data(), pre_pcm_len.data(), 0, m, st));
@@ -546,7 +583,8 @@ uint64_t vgb::gc_decode_seg_workspace_bytes(int32_t n_channels, int64_t full_fra
     return GcSegDecodeLayout(n_channels, full_frames).bytes;
 }
 
-int32_t vgb::gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &tab, int16_t *d_pcm, void *d_workspace, cudaStream_t st)
+int32_t vgb::gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &tab, int16_t *d_pcm, void *d_workspace, cudaStream_t st,
+                           const int16_t *d_coefs)
 {
     const int n_channels = (int)tab.size();
     if (n_channels == 0) return VGB_OK;
@@ -569,6 +607,9 @@ int32_t vgb::gc_decode_seg(const uint8_t *d_adpcm, std::vector<GcDecChannel> &ta
     sa.status = reinterpret_cast<int32_t *>(ws + L.o_status);
     sa.seg_count = gc_decode_pick_segments(n_channels, max_full, &sa.min_seg_frames);
     CUDA_TRY(cudaMemcpyAsync(ws, tab.data(), tab.size() * sizeof(GcDecChannel), cudaMemcpyHostToDevice, st));  // pageable: staged before return
+    if (d_coefs)
+        CUDA_TRY(cudaMemcpy2DAsync(ws + offsetof(GcDecChannel, coefs), sizeof(GcDecChannel), d_coefs, 32, 32, (size_t)n_channels,
+                                   cudaMemcpyDeviceToDevice, st));
     CUDA_TRY(cudaMemsetAsync(ws + L.o_status, 0, (size_t)n_channels * 4, st));
     CUDA_TRY(cudaMemsetAsync(ws + L.o_stats, 0, kGcDecStatWords * sizeof(unsigned long long), st));
     tick(3, true, st);
@@ -586,6 +627,29 @@ int32_t vgb::gc_decode_seg_words(const void *d_workspace, int32_t n_channels, in
     CUDA_TRY(cudaMemcpyAsync(status, static_cast<const char *>(d_workspace) + L.o_status, (size_t)n_channels * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     return VGB_OK;
+}
+
+uint64_t vgb::gc_align_tails_workspace_bytes(const std::vector<GcAlignChannel> &chans)
+{
+    TailWs t;
+    return t.build(chans) == VGB_OK ? t.total : 0;
+}
+
+int32_t vgb::gc_align_tails(const int16_t *d_src, std::vector<GcAlignChannel> &chans, const int16_t *d_coefs, void *d_workspace,
+                            cudaStream_t st, std::vector<int64_t> &tail_adpcm_off)
+{
+    TailWs t;
+    VGB_TRY(t.build(chans));
+    for (size_t i = 0; i < chans.size(); i++) chans[i].dst_off = t.enc.pcm_off[i];
+    tail_adpcm_off.resize(chans.size());
+    for (size_t i = 0; i < chans.size(); i++) tail_adpcm_off[i] = (int64_t)t.o_adpcm + t.enc.adpcm_off[i];
+    if (chans.empty()) return VGB_OK;
+    std::lock_guard<std::mutex> lock(g_ctx.mu);
+    VGB_TRY(ensure_ready_locked());
+    char *ws = static_cast<char *>(d_workspace);
+    CUDA_TRY(cudaMemcpyAsync(ws, chans.data(), chans.size() * sizeof(GcAlignChannel), cudaMemcpyHostToDevice, st));  // pageable: staged before return
+    return align_tails(d_src, reinterpret_cast<const GcAlignChannel *>(ws), t.enc, nullptr, d_coefs, reinterpret_cast<int16_t *>(ws + t.o_pcm),
+                       reinterpret_cast<uint8_t *>(ws + t.o_adpcm), ws + t.o_enc, t.w, nullptr, t.w, st);
 }
 
 extern "C" {

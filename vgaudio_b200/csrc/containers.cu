@@ -510,6 +510,141 @@ __global__ void __launch_bounds__(kHcaFramesPerTile * 32) hca_assemble_kernel(co
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// NintendoWare stream writers (BrstmWriter.cs, BCFstmWriter.cs).  Tile 0 of a file copies the host-built header
+// (everything in front of the audio data: RSTM/HEAD/ADPC/DATA or header/INFO/SEEK/DATA, device fields zero) and, for
+// GC-ADPCM, patches what only the device has: each channel's coefficients, its start context (predictor/scale of frame
+// 0, zero history) and loop context (GcAdpcmLoopContext.cs:17-26 at the loop start, or the start context when the
+// stream does not loop), and the seek table (GcAdpcmSeekTable.cs:25-38, interleaved per entry and resized to the
+// writer's entry count, GcAdpcmFormat.BuildSeekTable).  The other tiles write 16 KB of the data region each, with
+// InterleaveExtensions.Interleave's block layout (Interleave.cs:43-78) from the channel arrays the writer hands it:
+// GC-ADPCM rows (GcAdpcmAlignment.AdpcmAligned when the loop was aligned: the kept frames of the encoded row, then the
+// re-encoded tail), PCM16 in the file's byte order, PCM8 as (byte)(s >> 8) (Pcm8Codec.EncodeSigned).  InterleaveSize is
+// always 0x2000 and every block ends on a multiple of 32 bytes, so an 8-byte word never straddles two channel runs.
+// ---------------------------------------------------------------------------------------------------------------
+struct NwChan {
+    int64_t row_off;         // GC-ADPCM: bytes into the ADPCM slab (multiple of 16); PCM: samples into the PCM slab (multiple of 8)
+    int64_t pcm_off;         // GC-ADPCM: samples into the decoded-PCM slab (the channel decoded in full)
+    int64_t tail_off;        // GC-ADPCM, aligned loop: bytes of the re-encoded tail into the tail slab (multiple of 16)
+    int32_t coef_index, pad;
+};
+struct NwFile {
+    int64_t out_off;         // bytes into the output slab (multiple of 16)
+    int64_t hdr_off;         // bytes into the header blob
+    int32_t hdr_size;        // AudioDataOffset (a multiple of 32)
+    int32_t channels, first_ch;
+    int32_t codec;           // NwCodec: 0 PCM8, 1 PCM16, 2 GC-ADPCM
+    int32_t big_endian;      // byte order of the coefficients, contexts and PCM16 samples
+    int32_t in_size;         // bytes of each channel's array (the whole encoded or converted channel, or AdpcmAligned)
+    int32_t keep_bytes;      // bytes of that array taken from the encoded row; the rest is the aligned tail (a multiple of 8)
+    int32_t data_size;       // AudioDataSize
+    int32_t bpi;             // InterleaveSize
+    int32_t info_off;        // GC-ADPCM: file offset of channel 0's coefficients
+    int32_t info_stride;     // bytes between two channels' coefficients
+    int32_t ctx_off;         // start context relative to the coefficients (behind BRSTM's gain)
+    int32_t looping, loop_start;  // loop_start: where the loop context is taken (the unaligned loop start, see nw_plan_target)
+    int32_t seek_off;        // file offset of the first seek entry
+    int32_t seek_entries;    // SeekTableEntryCount (the resized table)
+    int32_t chan_entries;    // entries GcAdpcmSeekTable computes from the channel's own length
+    int32_t seek_spe, seek_be;
+    int32_t tile_first, pad;
+};
+
+__device__ __forceinline__ void put16(uint8_t *p, int v, bool be)
+{
+    if (be) { p[0] = (uint8_t)(v >> 8); p[1] = (uint8_t)v; }
+    else { p[0] = (uint8_t)v; p[1] = (uint8_t)(v >> 8); }
+}
+
+__global__ void __launch_bounds__(256) nw_assemble_kernel(const NwFile *__restrict__ files, int n_files, const NwChan *__restrict__ chans,
+                                                           const uint8_t *__restrict__ hdr_blob, const uint8_t *__restrict__ adpcm,
+                                                           const uint8_t *__restrict__ tail,
+                                                           const int16_t *__restrict__ coefs, const int16_t *__restrict__ decoded,
+                                                           const int16_t *__restrict__ pcm, uint8_t *__restrict__ out)
+{
+    const int fi = find_item(files, n_files, (int)blockIdx.x);
+    const NwFile f = files[fi];
+    const int tile = (int)blockIdx.x - f.tile_first;
+    uint8_t *dst = out + f.out_off;
+    const int ch = f.channels;
+    if (tile == 0) {
+        for (int t = threadIdx.x; t < f.hdr_size; t += blockDim.x) dst[t] = hdr_blob[f.hdr_off + t];
+        if (f.codec != 2) return;
+        __syncthreads();
+        const bool be = f.big_endian != 0;
+        for (int t = threadIdx.x; t < ch * 22; t += blockDim.x) {  // 16 coefficients and 2 x 3 context halfwords per channel
+            const int c = t / 22, h = t - c * 22;
+            const NwChan cc = chans[f.first_ch + c];
+            uint8_t *info = dst + f.info_off + c * f.info_stride;
+            if (h < 16) { put16(info + 2 * h, coefs[(int64_t)cc.coef_index * 16 + h], be); continue; }
+            const int k = h - 16;                  // 0..2 start context, 3..5 loop context
+            const bool loop_ctx = k >= 3 && f.looping;
+            const int ls = f.loop_start;
+            int v = 0;
+            switch (loop_ctx ? k - 3 : k % 3) {
+            case 0: v = loop_ctx ? adpcm[cc.row_off + (int64_t)(ls / kGcFrameSamples) * kGcFrameBytes] : adpcm[cc.row_off]; break;
+            case 1: v = loop_ctx && ls >= 1 ? decoded[cc.pcm_off + ls - 1] : 0; break;
+            default: v = loop_ctx && ls >= 2 ? decoded[cc.pcm_off + ls - 2] : 0; break;
+            }
+            put16(info + f.ctx_off + 2 * k, v, be);
+        }
+        const int n_words = f.seek_entries * ch;   // one (hist1, hist2) pair per entry and channel, entry-major
+        for (int t = threadIdx.x; t < n_words; t += blockDim.x) {
+            const int j = t / ch, c = t - j * ch;
+            int h1 = 0, h2 = 0;
+            if (j >= 1 && j < f.chan_entries) {   // entry 0 is always zero; entries past the channel's own table are Array.Resize's zeros
+                const int64_t at = chans[f.first_ch + c].pcm_off + (int64_t)j * f.seek_spe;
+                h1 = decoded[at - 1];
+                h2 = decoded[at - 2];
+            }
+            put16(dst + f.seek_off + 4 * t, h1, f.seek_be != 0);
+            put16(dst + f.seek_off + 4 * t + 2, h2, f.seek_be != 0);
+        }
+        return;
+    }
+    uint8_t *data = dst + f.hdr_size;
+    const uint32_t region = (uint32_t)f.data_size * (uint32_t)ch;  // a file is below 2 GiB (FileSize is an int)
+    const uint32_t q0 = (uint32_t)(tile - 1) * kTileBytes;
+    const int in_blocks = div_round_up(f.in_size, f.bpi), out_blocks = div_round_up(f.data_size, f.bpi);
+    const int last_in = f.in_size - (in_blocks - 1) * f.bpi, last_out = f.data_size - (out_blocks - 1) * f.bpi;
+    const int copy_blocks = min(in_blocks, out_blocks);
+    const uint32_t block_span = (uint32_t)f.bpi * (uint32_t)ch;
+#pragma unroll 4
+    for (int w = threadIdx.x; w < kTileBytes / 8; w += blockDim.x) {
+        const uint32_t q = q0 + (uint32_t)w * 8;
+        if (q >= region) break;
+        int b = (int)(q / block_span);
+        if (b > out_blocks - 1) b = out_blocks - 1;
+        const int cur_out = b == out_blocks - 1 ? last_out : f.bpi;
+        const int r = (int)(q - (uint32_t)b * block_span);
+        const int i = r / cur_out, k = r - i * cur_out;
+        const int cur_in = b == in_blocks - 1 ? last_in : f.bpi;
+        const int n = b < copy_blocks ? min(cur_in, cur_out) : 0;
+        uint2 v = make_uint2(0u, 0u);
+        if (k < n) {
+            const int64_t pos = (int64_t)f.bpi * b + k;  // byte of channel i's array (a multiple of 8)
+            const NwChan cc = chans[f.first_ch + i];
+            if (f.codec == 2) {
+                v = pos < f.keep_bytes ? *reinterpret_cast<const uint2 *>(adpcm + cc.row_off + pos)
+                                       : *reinterpret_cast<const uint2 *>(tail + cc.tail_off + (pos - f.keep_bytes));
+            } else if (f.codec == 1) {
+                v = *reinterpret_cast<const uint2 *>(pcm + cc.row_off + pos / 2);
+                if (f.big_endian) v = make_uint2(__byte_perm(v.x, 0, 0x2301), __byte_perm(v.y, 0, 0x2301));
+            } else {
+                const uint4 s = *reinterpret_cast<const uint4 *>(pcm + cc.row_off + pos);
+                v = make_uint2(__byte_perm(s.x, s.y, 0x7531), __byte_perm(s.z, s.w, 0x7531));
+            }
+            const int valid = n - k;
+            if (valid < 8) {
+                uint64_t x = ((uint64_t)v.y << 32) | v.x;
+                x &= ~0ull >> (8 * (8 - valid));
+                v = make_uint2((uint32_t)x, (uint32_t)(x >> 32));
+            }
+        }
+        *reinterpret_cast<uint2 *>(data + q) = v;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // host state of this translation unit: its own slabs and streams per context (Context::containers), so a converter call
 // sharded over several devices gives every worker its own on that worker's device
 // ---------------------------------------------------------------------------------------------------------------
@@ -678,6 +813,175 @@ void adx_build_header(const vgb_adx_desc &d, const AdxGeom &g, const int16_t *hi
     be32(p + 20, g.audio_offset + next_multiple(adx_bytes(g.loop_end, d.frame_size), d.frame_size) * d.channel_count);
     std::memcpy(h.data() + g.header_size - 2, "(c)CRI", 6);
     h.resize((size_t)g.audio_offset);
+}
+
+// ---- NintendoWare stream geometry (BrstmWriter.cs:24-74, BCFstmWriter.cs:23-83, BxstmConfiguration defaults) ----
+struct NwGeom {
+    int type = 0, codec = 0, be = 0, channels = 0, rate = 0, looping = 0, loop_start = 0;
+    int sample_count = 0;      // the writer's SampleCount: LoopEnd when looping
+    int in_samples = 0;        // samples of each channel's array (the whole WAVE channel)
+    int spi = 0, bpi = 0;      // SamplesPerInterleave, InterleaveSize
+    int audio_data_size = 0, interleave_count = 0, last_samples = 0, last_size_np = 0, last_size = 0;
+    int spe = 0;               // SamplesPerSeekTableEntry as the header states it
+    int seek_entries = 0, chan_entries = 0;
+    int head_size = 0, info1 = 0, info2 = 0, info3 = 0, seek_off = 0, seek_size = 0, data_off = 0, data_size = 0;
+    int tracks = 0;
+    int aligned = 0, ctx_loop_start = 0, keep = 0, keep_bytes = 0, tail_count = 0, in_size = 0;
+    int64_t file_size = 0;
+    int audio_offset() const { return data_off + 0x20; }
+};
+
+int nw_bytes(int samples, int codec)  // Common.SamplesToBytes
+{
+    return codec == 2 ? gc_sample_count_to_byte_count(samples) : codec == 1 ? samples * 2 : samples;
+}
+
+// type: VGB_CONTAINER_BRSTM / _BCSTM / _BFSTM; codec: NwCodec; be: the file's byte order.  No throw is possible here
+// except the ones the caller checks (channel count, FileSize as an int).
+void nw_geometry(int type, int codec, int be, int channels, int rate, int samples, bool looping, int loop_start, int loop_end, NwGeom &g)
+{
+    g = NwGeom{};
+    g.type = type; g.codec = codec; g.be = be; g.channels = channels; g.rate = rate; g.looping = looping;
+    g.loop_start = looping ? loop_start : 0;
+    g.sample_count = looping ? loop_end : samples;
+    g.in_samples = samples;
+    g.in_size = nw_bytes(samples, codec);
+    g.ctx_loop_start = g.loop_start;
+    g.keep_bytes = INT_MAX;
+    g.spi = codec == 2 ? gc_nibble_count_to_sample_count(0x2000 * 2) : codec == 1 ? 0x1000 : 0x2000;  // BytesToSamples(0x2000)
+    g.bpi = nw_bytes(g.spi, codec);
+    g.audio_data_size = next_multiple(nw_bytes(g.sample_count, codec), 0x20);
+    g.interleave_count = div_round_up(g.sample_count, g.spi);
+    g.last_samples = g.sample_count - (g.interleave_count - 1) * g.spi;
+    g.last_size_np = nw_bytes(g.last_samples, codec);
+    g.last_size = next_multiple(g.last_size_np, 0x20);
+    g.tracks = div_round_up(channels, 2);                          // AudioTrack.GetDefaultTrackList
+    const bool adpcm = codec == 2;
+    const int seek_spe = g.spi;                                    // SamplesPerSeekTableEntry's default equals the interleave's
+    g.spe = type == VGB_CONTAINER_BRSTM && !adpcm ? 0 : seek_spe;
+    if (adpcm) {
+        g.seek_entries = div_round_up(g.sample_count, seek_spe);
+        g.chan_entries = div_round_up(samples, seek_spe);
+    }
+    const int C = channels, T = g.tracks;
+    if (type == VGB_CONTAINER_BRSTM) {
+        const int h2 = 4 + 8 * T + 0x0c * T, h3 = 4 + 8 * C + (adpcm ? 0x38 : 8) * C;
+        g.info2 = h2;
+        g.head_size = next_multiple(8 + 24 + 0x34 + h2 + h3, 0x20);
+        g.seek_off = adpcm ? 0x40 + g.head_size : 0;
+        g.seek_size = adpcm ? next_multiple(8 + g.seek_entries * C * 4, 0x20) : 0;
+        g.data_off = 0x40 + g.head_size + g.seek_size;
+    } else {
+        const bool track_info = type == VGB_CONTAINER_BCSTM;       // version 2.1 has track info, 0.3 does not; both have region info
+        g.info1 = 0x38 + 0xc;
+        g.info2 = track_info ? 4 + 8 * T : 0;
+        g.info3 = 4 + 8 * C + (track_info ? 0x14 * T : 0) + 8 * C + (adpcm ? 0x2e : 0) * C;
+        g.head_size = next_multiple(8 + 24 + g.info1 + g.info2 + g.info3, 0x20);
+        g.seek_off = adpcm ? 0x40 + g.head_size : 0;
+        g.seek_size = adpcm ? next_multiple(8 + g.seek_entries * C * 4, 0x20) : 0;
+        g.data_off = 0x40 + g.head_size + g.seek_size;
+    }
+    g.data_size = 0x20 + g.audio_data_size * C;
+    g.file_size = (int64_t)g.data_off + (int64_t)0x20 + (int64_t)g.audio_data_size * C;
+}
+
+// A BinaryWriter over a zeroed header image in the file's byte order
+struct NwOut {
+    std::vector<uint8_t> &h;
+    bool be;
+    size_t at = 0;
+    void u8(int v) { h[at++] = (uint8_t)v; }
+    void u16(int v) { if (be) { u8(v >> 8); u8(v); } else { u8(v); u8(v >> 8); } }
+    void u32(int32_t v) { const uint32_t u = (uint32_t)v; if (be) { u16((int)(u >> 16)); u16((int)(u & 0xffff)); } else { u16((int)(u & 0xffff)); u16((int)(u >> 16)); } }
+    void tag(const char *s) { for (int i = 0; i < 4; i++) u8(s[i]); }
+    void ref(int type, int32_t off) { u16(type); u16(0); u32(off); }
+};
+
+// Everything in front of the audio data, with the device's fields (coefficients, contexts, seek entries) left zero.
+// info_off / info_stride / ctx_off say where the kernel patches them.
+void nw_build_header(const NwGeom &g, std::vector<uint8_t> &h, int &info_off, int &info_stride, int &ctx_off)
+{
+    h.assign((size_t)g.audio_offset(), 0);
+    const bool adpcm = g.codec == 2;
+    const int C = g.channels, T = g.tracks;
+    NwOut w{h, g.type == VGB_CONTAINER_BRSTM || g.be != 0};
+    auto track = [&](int t, int &cc, int &left, int &right) { cc = std::min(C - 2 * t, 2); left = 2 * t; right = cc >= 2 ? 2 * t + 1 : 0; };
+    if (g.type == VGB_CONTAINER_BRSTM) {  // WriteRstmHeader, WriteHeadBlock (BrstmWriter.cs:139-259)
+        const int marker = 0x01000000, h2 = g.info2;
+        w.tag("RSTM"); w.u16(0xfeff); w.u16(0x0100); w.u32((int32_t)g.file_size); w.u16(0x40); w.u16(2);
+        w.u32(0x40); w.u32(g.head_size); w.u32(g.seek_off); w.u32(g.seek_size); w.u32(g.data_off); w.u32(g.data_size);
+        w.at = 0x40;
+        w.tag("HEAD"); w.u32(g.head_size);
+        w.u32(marker); w.u32(24); w.u32(marker); w.u32(24 + 0x34); w.u32(marker); w.u32(24 + 0x34 + h2);
+        w.u8(g.codec); w.u8(g.looping); w.u8(C); w.u8(0); w.u16(g.rate & 0xffff); w.u16(0);  // (ushort)SampleRate
+        w.u32(g.loop_start); w.u32(g.sample_count); w.u32(g.audio_offset()); w.u32(g.interleave_count); w.u32(g.bpi); w.u32(g.spi);
+        w.u32(g.last_size_np); w.u32(g.last_samples); w.u32(g.last_size); w.u32(g.spe); w.u32(adpcm ? 4 : 0);
+        w.u8(T); w.u8(1); w.u16(0);
+        const int base2 = 24 + 0x34 + 4;
+        for (int t = 0; t < T; t++) { w.u32(0x01010000); w.u32(base2 + 8 * T + 0x0c * t); }
+        for (int t = 0; t < T; t++) {
+            int cc, l, r;
+            track(t, cc, l, r);
+            w.u8(0x7f); w.u8(0x40); w.u16(0); w.u32(0); w.u8(cc); w.u8(l); w.u8(r); w.u8(0);
+        }
+        w.u8(C); w.u8(0); w.u16(0);
+        const int base3 = 24 + 0x34 + h2 + 4, cis = adpcm ? 0x38 : 8;
+        for (int c = 0; c < C; c++) { w.u32(marker); w.u32(base3 + 8 * C + cis * c); }
+        info_off = 0;
+        for (int c = 0; c < C; c++) {
+            w.u32(marker);
+            if (!adpcm) { w.u32(0); continue; }
+            w.u32(base3 + 8 * C + cis * c + 8);
+            if (c == 0) info_off = (int)w.at;
+            w.at += 0x30;  // coefficients, gain, start and loop context, padding
+        }
+        info_stride = 0x38;
+        ctx_off = 0x22;
+        if (adpcm) { w.at = (size_t)g.seek_off; w.tag("ADPC"); w.u32(g.seek_size); }
+        w.at = (size_t)g.data_off;
+        w.tag("DATA"); w.u32(g.data_size); w.u32(0x18);
+        return;
+    }
+    // WriteHeader, WriteInfoBlock (BCFstmWriter.cs:164-332)
+    const bool track_info = g.type == VGB_CONTAINER_BCSTM;
+    w.tag(g.type == VGB_CONTAINER_BCSTM ? "CSTM" : "FSTM"); w.u16(0xfeff); w.u16(0x40);
+    w.u32((track_info ? 0x201 : 3) << 16); w.u32((int32_t)g.file_size);
+    w.u16(adpcm ? 3 : 2); w.u16(0);
+    w.ref(0x4000, 0x40); w.u32(g.head_size);
+    if (adpcm) { w.ref(0x4001, g.seek_off); w.u32(g.seek_size); }
+    w.ref(0x4002, g.data_off); w.u32(g.data_size);
+    w.at = 0x40;
+    w.tag("INFO"); w.u32(g.head_size);
+    w.ref(0x4100, 24);
+    if (track_info) w.ref(0x0101, 24 + g.info1);
+    else { w.u32(0); w.u32(-1); }
+    w.ref(0x0101, 24 + g.info1 + g.info2);
+    w.u8(g.codec); w.u8(g.looping); w.u8(C); w.u8(0); w.u32(g.rate); w.u32(g.loop_start); w.u32(g.sample_count);
+    w.u32(g.interleave_count); w.u32(g.bpi); w.u32(g.spi); w.u32(g.last_size_np); w.u32(g.last_samples); w.u32(g.last_size);
+    w.u32(4); w.u32(g.spe); w.ref(0x1F00, 0x18);
+    w.ref(0x0100, 0); w.u32(-1);  // region info
+    if (track_info) {
+        w.u32(T);
+        for (int t = 0; t < T; t++) w.ref(0x4101, (4 + 8 * T) + (4 + 8 * C) + 0x14 * t);
+    }
+    w.u32(C);
+    for (int c = 0; c < C; c++) w.ref(0x4102, (4 + 8 * C) + (track_info ? 0x14 * T : 0) + 8 * c);
+    if (track_info)
+        for (int t = 0; t < T; t++) {
+            int cc, l, r;
+            track(t, cc, l, r);
+            w.u8(0x7f); w.u8(0x40); w.u16(0); w.ref(0x0100, 0xc); w.u32(cc); w.u8(l); w.u8(r); w.u16(0);
+        }
+    for (int c = 0; c < C; c++) {
+        if (adpcm) w.ref(0x0300, 8 * C - 8 * c + 0x2e * c);
+        else { w.u32(0); w.u32(-1); }
+    }
+    info_off = (int)w.at;
+    info_stride = 0x2e;
+    ctx_off = 0x20;
+    if (adpcm) { w.at = (size_t)g.seek_off; w.tag("SEEK"); w.u32(g.seek_size); }
+    w.at = (size_t)g.data_off;
+    w.tag("DATA"); w.u32(g.data_size);
 }
 
 const uint8_t kPcmGuid[16] = {0x01, 0x00, 0x00, 0x00, 0x00, 0x00, 0x10, 0x00, 0x80, 0x00, 0x00, 0xAA, 0x00, 0x38, 0x9B, 0x71};
