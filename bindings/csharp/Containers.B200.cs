@@ -63,7 +63,7 @@ namespace VGAudio.Native
     [StructLayout(LayoutKind.Sequential)]
     internal struct VgbConvertOptions
     {
-        public int OutType;                 // 1 .dsp, 2 .adx, 3 .hca, 4 .brstm, 5 .bcstm, 6 .bfstm
+        public int OutType;                 // 1 .dsp, 2 .adx, 3 .hca, 4 .brstm, 5 .bcstm, 6 .bfstm, 7 .idsp, 8 .hps
         public int NoTrim;
         public int DspSamplesPerInterleave, DspLoopPointAlignment;
         public int AdxVersion, AdxFrameSize, AdxType, AdxFilterPlus1;

@@ -635,6 +635,16 @@ int32_t vgb_hca_write_batch(const vgb_hca_info *info, int32_t n_files, const uin
 #define VGB_CONTAINER_BRSTM 4
 #define VGB_CONTAINER_BCSTM 5
 #define VGB_CONTAINER_BFSTM 6
+/* IDSP (IdspWriter with IdspConfiguration's default block size of 16 bytes: the loop start moves to a multiple of 28
+ * samples, and no_trim maps to TrimFile as for .dsp) and HPS (HpsWriter: blocks of at most 0x10000 bytes, the loop start
+ * moves to a multiple of one block's samples per channel), both GC-ADPCM only.  vgb_convert_wave_batch writes them;
+ * vgb_transcode_batch does not take them as a target; the nw_* options are ignored.  Per-file refusals besides the
+ * usual ones (no samples, loop points GcAdpcmAlignment refuses, 2 GiB of output, more than 255 channels - this
+ * converter's limit): an HPS file with 3, 7, 11 ... channels, whose block headers HpsWriter writes 0x20 bytes past the
+ * block map's offsets; and an HPS file whose loop moved and that has a block starting more than one sample behind the
+ * input's last sample, where HpsWriter reads the block's history past the unaligned decode (IndexOutOfRangeException). */
+#define VGB_CONTAINER_IDSP 7
+#define VGB_CONTAINER_HPS 8
 typedef struct vgb_convert_options {
     int32_t out_type;                   /* VGB_CONTAINER_* */
     int32_t no_trim;                    /* Configuration.TrimFile = !no_trim */

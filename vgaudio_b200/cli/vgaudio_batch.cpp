@@ -1,5 +1,5 @@
 // vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
-// .dsp / .adx / .hca, WAVE files to .brstm / .bcstm / .bfstm, and .dsp, .adx, .hca, .brstm, .bcstm and .bfstm files to WAVE.
+// .dsp / .adx / .hca, WAVE files to .brstm / .bcstm / .bfstm / .idsp / .hps, and .dsp, .adx, .hca, .brstm, .bcstm and .bfstm files to WAVE.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
@@ -7,7 +7,7 @@
 // (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch for coded files, vgb_convert_*_to_wave_batch for
 // --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
-//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm and .bfstm inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
+//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm and .bfstm inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
@@ -60,7 +60,7 @@ static const int32_t kContainerOfKind[3] = {VGB_CONTAINER_DSP, VGB_CONTAINER_HCA
 
 static int usage()
 {
-    std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
+    std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian]\n");
@@ -135,8 +135,16 @@ int main(int argc, char **argv)
     else if (fmt == "brstm") opt.out_type = VGB_CONTAINER_BRSTM;
     else if (fmt == "bcstm") opt.out_type = VGB_CONTAINER_BCSTM;
     else if (fmt == "bfstm") opt.out_type = VGB_CONTAINER_BFSTM;
+    else if (fmt == "idsp") opt.out_type = VGB_CONTAINER_IDSP;
+    else if (fmt == "hps") opt.out_type = VGB_CONTAINER_HPS;
     else if (fmt == "hca") opt.out_type = VGB_CONTAINER_HCA;
     else if (!to_wave) return usage();
+    if ((opt.out_type == VGB_CONTAINER_IDSP || opt.out_type == VGB_CONTAINER_HPS) && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2)) {
+        // CreateConfiguration.Idsp / .Hps (src/VGAudio.Cli/CreateConfiguration.cs:57-75, 103-115): GC-ADPCM only
+        std::fprintf(stderr, "Can't use format %s with %s files\n", opt.nw_codec_plus1 == 2 ? "PCM16" : "PCM8",
+                     opt.out_type == VGB_CONTAINER_IDSP ? "IDSP" : "HPS");
+        return 1;
+    }
     vgb_adx_key adx_key{};  // the CriAdxKey of --keystring / --keycode, for writing .adx files or reading keyed ones
     const bool have_adx_key = have_code || !key_string.empty();
     if ((opt.out_type == VGB_CONTAINER_ADX || to_wave) && have_adx_key) {
@@ -164,7 +172,7 @@ int main(int argc, char **argv)
         if (!e.is_regular_file()) return;
         const int kind = kind_of(e.path());
         if (kind < 0) return;
-        const bool nw_out = opt.out_type >= VGB_CONTAINER_BRSTM;  // NintendoWare targets take WAVE inputs only
+        const bool nw_out = opt.out_type >= VGB_CONTAINER_BRSTM;  // NintendoWare, IDSP and HPS targets take WAVE inputs only
         if (to_wave ? kind != 3 : (kind == 3 || (!nw_out && kind < 3 && kContainerOfKind[kind] != opt.out_type))) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);

@@ -15,6 +15,7 @@ from . import _native as N
 
 CONTAINER_DSP, CONTAINER_ADX, CONTAINER_HCA = 1, 2, 3
 CONTAINER_BRSTM, CONTAINER_BCSTM, CONTAINER_BFSTM = 4, 5, 6   # written by convert_wave_batch, read by convert_nw_to_wave_batch
+CONTAINER_IDSP, CONTAINER_HPS = 7, 8                          # GC-ADPCM only, written by convert_wave_batch
 NW_CODEC_PCM8, NW_CODEC_PCM16, NW_CODEC_GCADPCM = 0, 1, 2        # NwCodec; convert_options(nw_codec_plus1=codec + 1)
 
 

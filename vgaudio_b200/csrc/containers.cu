@@ -645,6 +645,177 @@ __global__ void __launch_bounds__(256) nw_assemble_kernel(const NwFile *__restri
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// IDSP and HPS writers (IdspWriter.cs, HpsWriter.cs), big-endian GC-ADPCM containers.  Their channels are rows of
+// NwChan, as for the NintendoWare writer: the array each writer hands on is GetAdpcmAudio(), the encoded row, or when the
+// loop moved, its kept frames followed by the re-encoded tail (keep_bytes, a multiple of 8, so an 8-byte word never
+// straddles the two).  Tile 0 of a file copies the host-built header and patches what only the device has; the other
+// tiles write 16 KB of the rest each.
+// ---------------------------------------------------------------------------------------------------------------
+struct IdspFile {
+    int64_t out_off;         // bytes into the output slab (multiple of 16)
+    int64_t hdr_off;         // bytes into the header blob
+    int32_t hdr_size;        // HeaderSize = 0x40 + 0x60 * channels
+    int32_t channels, first_ch;
+    int32_t in_size;         // bytes of each channel's array
+    int32_t keep_bytes;      // bytes of that array taken from the encoded row
+    int32_t data_size;       // AudioDataSize (a multiple of the 16-byte interleave)
+    int32_t ctx_loop_start;  // where the loop context is taken (the unaligned loop start); 0: the context stays (0, 0, 0)
+    int32_t tile_first;
+};
+struct HpsBlock {
+    int32_t at;              // file offset of the block (BlockInfo.Offset)
+    int32_t start_sample, byte_in, chan_size;  // StartSample, ByteInIndex (a multiple of 32), ChannelSize
+    int32_t written, end_nibble, next;         // WrittenSize, EndNibble, NextOffset
+    int32_t pad;
+};
+struct HpsFile {
+    int64_t out_off, hdr_off;
+    int32_t hdr_size;        // HeaderSize
+    int32_t channels, first_ch;
+    int32_t keep_bytes;
+    int32_t block_hdr;       // bytes in front of a block's audio: GetNextMultiple(12 + 8 * channels, 0x20)
+    int32_t first_block, n_blocks;
+    int32_t file_size;
+    int32_t tile_first, pad;
+};
+
+__device__ __forceinline__ void put16be(uint8_t *p, int v) { p[0] = (uint8_t)(v >> 8); p[1] = (uint8_t)v; }
+
+// byte `pos` of a channel's array
+__device__ __forceinline__ int gc_array_byte(const NwChan &cc, int64_t pos, int keep_bytes, const uint8_t *adpcm, const uint8_t *tail)
+{
+    return pos < keep_bytes ? adpcm[cc.row_off + pos] : tail[cc.tail_off + (pos - keep_bytes)];
+}
+
+// the 8 bytes of a channel's array from `pos` (a multiple of 8), those from `valid` on zero
+__device__ __forceinline__ uint2 gc_array_word(const NwChan &cc, int64_t pos, int keep_bytes, const uint8_t *adpcm, const uint8_t *tail, int valid)
+{
+    uint2 v = pos < keep_bytes ? *reinterpret_cast<const uint2 *>(adpcm + cc.row_off + pos)
+                               : *reinterpret_cast<const uint2 *>(tail + cc.tail_off + (pos - keep_bytes));
+    if (valid < 8) {
+        uint64_t x = ((uint64_t)v.y << 32) | v.x;
+        x &= ~0ull >> (8 * (8 - valid));
+        v = make_uint2((uint32_t)x, (uint32_t)(x >> 32));
+    }
+    return v;
+}
+
+// IdspWriter: per channel the coefficients, the start context's predictor/scale (Adpcm[0], history 0) and the loop
+// context (the first encode's, at the unaligned loop start), then Interleave(16, AudioDataSize) (Interleave.cs:43-73):
+// AudioDataSize is a multiple of 16, so every block is whole and byte `pos` of a channel is in the file iff pos < in_size.
+__global__ void __launch_bounds__(256) idsp_assemble_kernel(const IdspFile *__restrict__ files, int n_files, const NwChan *__restrict__ chans,
+                                                             const uint8_t *__restrict__ hdr_blob, const uint8_t *__restrict__ adpcm,
+                                                             const uint8_t *__restrict__ tail, const int16_t *__restrict__ coefs,
+                                                             const int16_t *__restrict__ decoded, uint8_t *__restrict__ out)
+{
+    const int fi = find_item(files, n_files, (int)blockIdx.x);
+    const IdspFile f = files[fi];
+    const int tile = (int)blockIdx.x - f.tile_first;
+    uint8_t *dst = out + f.out_off;
+    const int ch = f.channels;
+    if (tile == 0) {
+        for (int t = threadIdx.x; t < f.hdr_size; t += blockDim.x) dst[t] = hdr_blob[f.hdr_off + t];
+        __syncthreads();
+        const int ls = f.ctx_loop_start;
+        for (int t = threadIdx.x; t < ch * 20; t += blockDim.x) {  // 16 coefficients, the start predictor/scale, 3 loop context halfwords
+            const int c = t / 20, h = t - c * 20;
+            const NwChan cc = chans[f.first_ch + c];
+            uint8_t *info = dst + 0x40 + 0x60 * c;
+            if (h < 16) put16be(info + 0x1c + 2 * h, coefs[(int64_t)cc.coef_index * 16 + h]);
+            else if (h == 16) put16be(info + 0x3e, adpcm[cc.row_off]);
+            else if (ls > 0) {
+                const int k = h - 17;
+                const int v = k == 0 ? adpcm[cc.row_off + (int64_t)(ls / kGcFrameSamples) * kGcFrameBytes]
+                                     : ls >= k ? decoded[cc.pcm_off + ls - k] : 0;
+                put16be(info + 0x44 + 2 * k, v);
+            }
+        }
+        return;
+    }
+    uint8_t *data = dst + f.hdr_size;
+    const uint32_t region = (uint32_t)f.data_size * (uint32_t)ch;
+    const uint32_t q0 = (uint32_t)(tile - 1) * kTileBytes;
+    const uint32_t block_span = 16u * (uint32_t)ch;
+#pragma unroll 4
+    for (int w = threadIdx.x; w < kTileBytes / 8; w += blockDim.x) {
+        const uint32_t q = q0 + (uint32_t)w * 8;
+        if (q >= region) break;
+        const uint32_t b = q / block_span, r = q - b * block_span;
+        const int64_t pos = (int64_t)b * 16 + (r & 15);
+        const int valid = f.in_size - (int)pos;
+        uint2 v = make_uint2(0u, 0u);
+        if (valid > 0) v = gc_array_word(chans[f.first_ch + (int)(r >> 4)], pos, f.keep_bytes, adpcm, tail, valid);
+        *reinterpret_cast<uint2 *>(data + q) = v;
+    }
+}
+
+// HpsWriter: per channel the coefficients and the start context's predictor/scale; per block (WriteBlock) WrittenSize,
+// EndNibble, NextOffset and per channel (predictor/scale of GetAdpcmAudio() at StartSample, Hist1 and Hist2 from the
+// first encode's full decode, 0), then each channel's ChannelSize bytes, every part padded to 0x20.  Tile 0 writes the
+// headers, the other tiles the audio of the blocks.
+__global__ void __launch_bounds__(256) hps_assemble_kernel(const HpsFile *__restrict__ files, int n_files, const HpsBlock *__restrict__ blocks,
+                                                            const NwChan *__restrict__ chans, const uint8_t *__restrict__ hdr_blob,
+                                                            const uint8_t *__restrict__ adpcm, const uint8_t *__restrict__ tail,
+                                                            const int16_t *__restrict__ coefs, const int16_t *__restrict__ decoded,
+                                                            uint8_t *__restrict__ out)
+{
+    const int fi = find_item(files, n_files, (int)blockIdx.x);
+    const HpsFile f = files[fi];
+    const int tile = (int)blockIdx.x - f.tile_first;
+    uint8_t *dst = out + f.out_off;
+    const int ch = f.channels;
+    const HpsBlock *B = blocks + f.first_block;
+    if (tile == 0) {
+        for (int t = threadIdx.x; t < f.hdr_size; t += blockDim.x) dst[t] = hdr_blob[f.hdr_off + t];
+        __syncthreads();
+        for (int t = threadIdx.x; t < ch * 17; t += blockDim.x) {  // 16 coefficients and the start predictor/scale
+            const int c = t / 17, h = t - c * 17;
+            const NwChan cc = chans[f.first_ch + c];
+            uint8_t *info = dst + 0x10 + 0x38 * c;
+            put16be(info + (h < 16 ? 0x10 + 2 * h : 0x32), h < 16 ? coefs[(int64_t)cc.coef_index * 16 + h] : adpcm[cc.row_off]);
+        }
+        const int halves = f.block_hdr / 2;
+        for (int t = threadIdx.x; t < f.n_blocks * halves; t += blockDim.x) {
+            const int bi = t / halves, j = 2 * (t - bi * halves);
+            const HpsBlock blk = B[bi];
+            int v = 0;
+            if (j < 12) {
+                const int word = j < 4 ? blk.written : j < 8 ? blk.end_nibble : blk.next;
+                v = (j & 2) ? word & 0xffff : (int)((uint32_t)word >> 16);
+            } else if (j < 12 + 8 * ch) {
+                const int c = (j - 12) >> 3, m = ((j - 12) & 7) >> 1;
+                const NwChan cc = chans[f.first_ch + c];
+                const int s = blk.start_sample;
+                if (m == 0) v = gc_array_byte(cc, blk.byte_in, f.keep_bytes, adpcm, tail);
+                else if (m < 3 && s >= m) v = decoded[cc.pcm_off + s - m];
+            }
+            put16be(dst + blk.at + j, v);
+        }
+        return;
+    }
+    const int q0 = f.hdr_size + (tile - 1) * kTileBytes;
+#pragma unroll 4
+    for (int w = threadIdx.x; w < kTileBytes / 8; w += blockDim.x) {
+        const int q = q0 + w * 8;
+        if (q >= f.file_size) break;
+        int lo = 0, hi = f.n_blocks - 1;  // the last block at or before q
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (B[mid].at <= q) lo = mid; else hi = mid - 1;
+        }
+        const HpsBlock blk = B[lo];
+        int r = q - blk.at - f.block_hdr;
+        if (r < 0) continue;  // the block's header: tile 0
+        const int cpad = (blk.chan_size + 31) & ~31;
+        const int i = r / cpad, k = r - i * cpad;
+        const int valid = blk.chan_size - k;
+        uint2 v = make_uint2(0u, 0u);
+        if (valid > 0) v = gc_array_word(chans[f.first_ch + i], (int64_t)blk.byte_in + k, f.keep_bytes, adpcm, tail, valid);
+        *reinterpret_cast<uint2 *>(dst + q) = v;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // host state of this translation unit: its own slabs and streams per context (Context::containers), so a converter call
 // sharded over several devices gives every worker its own on that worker's device
 // ---------------------------------------------------------------------------------------------------------------
@@ -982,6 +1153,101 @@ void nw_build_header(const NwGeom &g, std::vector<uint8_t> &h, int &info_off, in
     if (adpcm) { w.at = (size_t)g.seek_off; w.tag("SEEK"); w.u32(g.seek_size); }
     w.at = (size_t)g.data_off;
     w.tag("DATA"); w.u32(g.data_size);
+}
+
+// ---- IDSP (IdspWriter.cs) and HPS (HpsWriter.cs) geometry, after the writers' GcAdpcmFormat.WithAlignment ----
+struct GcGeom {
+    int type = 0, channels = 0, rate = 0, looping = 0;
+    int sample_count = 0;      // IDSP: the writer's SampleCount; HPS: the format's (SampleCountAligned when the loop moved)
+    int loop_start = 0, loop_end = 0;  // the format's loop points (aligned), 0 without a loop
+    int chan_samples = 0;      // each channel's own SampleCount
+    int aligned = 0, ctx_loop_start = 0, keep = 0, keep_bytes = INT_MAX, tail_count = 0, in_size = 0;
+    int header_size = 0;
+    int audio_data_size = 0;   // IDSP
+    int block_hdr = 0;         // HPS
+    std::vector<HpsBlock> blocks;  // HPS: CreateBlockMap
+    int64_t file_size = 0;
+};
+
+int gc_sample_to_nibble(int s) { return s / kGcFrameSamples * 16 + s % kGcFrameSamples + 2; }  // GcAdpcmMath.SampleToNibble
+int gc_nibble_to_sample(int n) { return n / 16 * kGcFrameSamples + n % 16 - 2; }                // GcAdpcmMath.NibbleToSample
+
+constexpr int kIdspBlockSize = 16;  // IdspConfiguration.BlockSize's default (BytesPerFrame * 2); the CLI never sets it
+
+void idsp_geometry(bool trim, GcGeom &g)
+{
+    g.sample_count = trim && g.looping ? g.loop_end : std::max(g.chan_samples, g.loop_end);
+    g.audio_data_size = next_multiple(gc_sample_count_to_byte_count(g.sample_count), kIdspBlockSize);
+    g.header_size = 0x40 + 0x60 * g.channels;
+    g.file_size = (int64_t)g.header_size + (int64_t)g.audio_data_size * g.channels;
+}
+
+int hps_channel_size(int channels) { return next_multiple(0x10000 / channels, 0x20); }
+
+// CreateBlockMap (HpsWriter.cs:113-157) for the format's sample count and loop.  False where the reference would leave a
+// null entry in its block array (the even split running out of nibbles before the last block).
+bool hps_geometry(GcGeom &g)
+{
+    const int C = g.channels;
+    g.sample_count = g.chan_samples;
+    g.header_size = next_multiple(std::max(0x80, 0x10 + 0x38 * C), 0x20);
+    g.block_hdr = next_multiple(12 + 8 * C, 0x20);
+    const int nibbles = gc_sample_count_to_nibble_count(g.sample_count);
+    const int max_nibbles = hps_channel_size(C) * C / C * 2;
+    const int count = div_round_up(nibbles, max_nibbles);
+    const int loop_block = g.looping ? gc_sample_to_nibble(g.loop_start) / max_nibbles : count - 1;
+    g.blocks.clear();
+    int cur = 0;
+    auto add = [&](int size) {
+        HpsBlock b{};
+        b.start_sample = gc_nibble_to_sample(cur + 2);
+        b.byte_in = cur / 2;
+        b.end_nibble = size - 1;
+        b.chan_size = (size + 1) / 2;
+        b.written = next_multiple(b.chan_size, 0x20) * C;
+        g.blocks.push_back(b);
+        cur += size;
+    };
+    while ((int)g.blocks.size() < loop_block) add(max_nibbles);
+    while (cur < nibbles) {
+        const int left = count - (int)g.blocks.size(), rem = nibbles - cur;
+        add(std::min(rem, next_multiple(div_round_up(rem, left), 0x40)));
+    }
+    if ((int)g.blocks.size() != count) return false;
+    int64_t at = g.header_size;
+    for (HpsBlock &b : g.blocks) {
+        b.at = (int32_t)std::min<int64_t>(at, INT_MAX);
+        at += next_multiple(4 + 8 * C, 0x20) + b.written;  // BlockInfo.TotalSize
+    }
+    for (int i = 0; i < count; i++) g.blocks[i].next = i + 1 < count ? g.blocks[i + 1].at : g.looping ? g.blocks[loop_block].at : -1;
+    g.file_size = at;
+    return true;
+}
+
+// Everything the writers put in front of the audio (IDSP) or the first block (HPS), big-endian, with the device's
+// fields (coefficients, contexts) left zero
+void gc_build_header(const GcGeom &g, std::vector<uint8_t> &h)
+{
+    h.assign((size_t)g.header_size, 0);
+    NwOut w{h, true};
+    if (g.type == VGB_CONTAINER_IDSP) {  // WriteHeader (IdspWriter.cs:66-104)
+        w.tag("IDSP"); w.u32(0); w.u32(g.channels); w.u32(g.rate); w.u32(g.sample_count); w.u32(g.loop_start); w.u32(g.loop_end);
+        w.u32(kIdspBlockSize); w.u32(0x40); w.u32(0x60); w.u32(g.header_size); w.u32(g.audio_data_size);
+        for (int c = 0; c < g.channels; c++) {
+            w.at = (size_t)(0x40 + 0x60 * c);
+            w.u32(g.chan_samples); w.u32(gc_sample_count_to_nibble_count(g.chan_samples)); w.u32(g.rate); w.u16(g.looping); w.u16(0);
+            w.u32(gc_sample_to_nibble(g.looping ? g.loop_start : 0));
+            w.u32(gc_sample_to_nibble(g.looping ? g.loop_end : g.sample_count - 1));
+            w.u32(gc_sample_to_nibble(0));
+        }
+        return;
+    }
+    w.tag(" HAL"); w.tag("PST\0");  // WriteHpsHeader, WriteChannelInfo (HpsWriter.cs:63-84)
+    w.u32(g.rate); w.u32(g.channels);
+    for (int c = 0; c < g.channels; c++) {
+        w.at = (size_t)(0x10 + 0x38 * c);
+        w.u32(0x10000); w.u32(gc_sample_to_nibble(0)); w.u32(gc_sample_to_nibble(g.sample_count - 1)); w.u32(gc_sample_to_nibble(0));
+    }
 }
 
 const uint8_t kPcmGuid[16] = {0x01, 0x00, 0x00, 0x00, 0x00, 0x00, 0x10, 0x00, 0x80, 0x00, 0x00, 0xAA, 0x00, 0x38, 0x9B, 0x71};
