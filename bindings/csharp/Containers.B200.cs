@@ -61,6 +61,39 @@ namespace VGAudio.Native
     }
 
     [StructLayout(LayoutKind.Sequential)]
+    internal unsafe struct VgbIdspInfo   // IdspStructure (Containers/Idsp/IdspStructure.cs) with the region DeInterleave reads
+    {
+        public int ChannelCount, SampleRate, SampleCount, LoopStart, LoopEnd, InterleaveSize;
+        public int HeaderSize, ChannelInfoSize, AudioDataOffset, AudioDataLength;
+        public int Looping, Interleave, OutputSize, Reserved;
+        public long AudioOffset, AudioLength;
+        public fixed int ChSampleCount[255], ChNibbleCount[255], ChSampleRate[255];
+        public fixed int ChLooping[255], StartAddress[255], EndAddress[255];
+        public fixed int CurrentAddress[255];
+        public fixed short Coefs[255 * 16];
+        public fixed short Gain[255];
+        public fixed short StartContext[255 * 3], LoopContext[255 * 3];
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    internal unsafe struct VgbHpsInfo   // HpsStructure (Containers/Hps/HpsStructure.cs)
+    {
+        public int SampleRate, ChannelCount, SampleCount, Looping, LoopStart, BlockCount;
+        public int FirstBlock, LoopBlock;
+        public fixed int MaxBlockSize[255], EndAddress[255];
+        public fixed long ChannelAudioBytes[255];
+        public fixed short Coefs[255 * 16];
+        public fixed short Gain[255];
+        public fixed short StartContext[255 * 3], LoopContext[255 * 3];
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
+    internal struct VgbHpsBlock   // HpsBlock (Containers/Hps/HpsBlock.cs)
+    {
+        public int Offset, Size, FinalNibble, NextOffset;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     internal struct VgbConvertOptions
     {
         public int OutType;                 // 1 .dsp, 2 .adx, 3 .hca, 4 .brstm, 5 .bcstm, 6 .bfstm, 7 .idsp, 8 .hps
@@ -113,6 +146,11 @@ namespace VGAudio.Native
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_bcfstm_parse(byte* file, long length, VgbNwInfo* info);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_nw_to_wave_batch(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_idsp_parse(byte* file, long length, VgbIdspInfo* info);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_hps_parse(byte* file, long length, VgbHpsInfo* info, VgbHpsBlock* blocks, int blockCapacity);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_convert_idsp_hps_to_wave_batch(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_gcadpcm_debug_decode_stats(ulong* output, int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_wave_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, long* outSizes,
@@ -320,6 +358,24 @@ namespace VGAudio.Cli
         // (4 / 5 / 6).  A file whose GC-ADPCM frames select a predictor outside 0..7 fails in the second pass alone.
         public static unsafe void ConvertNwToWave(string[] inPaths, int[] inTypes, string[] outPaths, Action<string> log, Action<int> reportAdd)
         {
+            ConvertTypedToWave(inPaths, inTypes, outPaths, log, reportAdd, VgAudioB200Containers.vgb_convert_nw_to_wave_batch);
+        }
+
+        // The decode direction for a chunk of IDSP and HPS streams (`-b --out-format wav` over .idsp / .hps): IdspReader or
+        // HpsReader as the extension names it (ContainerTypes.cs) -> ToPcm16 -> WaveWriter per file in one native call per
+        // pass.  inTypes[i] is VGB_CONTAINER_IDSP / _HPS (7 / 8).  A file whose frames select a predictor outside 0..7 fails
+        // in the second pass alone.
+        public static unsafe void ConvertIdspHpsToWave(string[] inPaths, int[] inTypes, string[] outPaths, Action<string> log, Action<int> reportAdd)
+        {
+            ConvertTypedToWave(inPaths, inTypes, outPaths, log, reportAdd, VgAudioB200Containers.vgb_convert_idsp_hps_to_wave_batch);
+        }
+
+        private unsafe delegate int TypedToWave(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
+
+        // The two passes of a converter whose files carry an in_type each (the reader), with per-file status
+        private static unsafe void ConvertTypedToWave(string[] inPaths, int[] inTypes, string[] outPaths, Action<string> log, Action<int> reportAdd,
+                                                      TypedToWave convert)
+        {
             int n = inPaths.Length;
             byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
             var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
@@ -334,7 +390,7 @@ namespace VGAudio.Cli
                 for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
                 fixed (int* types = inTypes)
                 {
-                    VgAudioB200.Check(VgAudioB200Containers.vgb_convert_nw_to_wave_batch(inPtr, len, types, n, outSize, null, status));
+                    VgAudioB200.Check(convert(inPtr, len, types, n, outSize, null, status));
                     var outputs = new byte[n][];
                     for (int i = 0; i < n; i++)
                     {
@@ -344,7 +400,7 @@ namespace VGAudio.Cli
                         outPins.Add(GCHandle.Alloc(outputs[i], GCHandleType.Pinned));
                         outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
                     }
-                    VgAudioB200.Check(VgAudioB200Containers.vgb_convert_nw_to_wave_batch(inPtr, len, types, n, outSize, outPtr, status));
+                    VgAudioB200.Check(convert(inPtr, len, types, n, outSize, outPtr, status));
                     for (int i = 0; i < n; i++)
                     {
                         if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); }   // Batch.cs:39-43

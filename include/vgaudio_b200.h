@@ -46,7 +46,7 @@ int32_t vgb_shutdown(void);
 /* Bind several devices (SURVEY §8b's vgb_init(n_devices, flags); the reference's counterpart is Parallel.ForEach over
  * files, src/VGAudio.Cli/Batch.cs:24-25).  devices[0] becomes the primary device (the one the *_dev entry points, timers
  * and debug taps use); every host-pointer codec *_batch call and every batch converter (vgb_convert_wave_batch,
- * vgb_convert_{dsp,hca,adx,nw}_to_wave_batch, vgb_transcode_batch) are then sharded over all bound devices by greedy
+ * vgb_convert_{dsp,hca,adx,nw,idsp_hps}_to_wave_batch, vgb_transcode_batch) are then sharded over all bound devices by greedy
  * longest-first bin packing of the units' sample or frame counts - one worker thread and one H2D / kernel / D2H pipeline
  * per device, each over its own PCIe link, results written straight into the caller's arrays (no collective: host data
  * reaches a GPU fastest over that GPU's own link).  The single-shot container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.
@@ -597,6 +597,65 @@ typedef struct vgb_nw_info {
 int32_t vgb_brstm_parse(const uint8_t *file, int64_t length, vgb_nw_info *info_out);
 int32_t vgb_bcfstm_parse(const uint8_t *file, int64_t length, vgb_nw_info *info_out);
 
+/* IdspStructure (Containers/Idsp/IdspStructure.cs) as IdspReader.ReadFile (Containers/Idsp/IdspReader.cs:13-112) leaves
+ * it, big-endian: the main header's fields, looping (set when any channel's flag is 1), and per channel its header
+ * (IdspChannelInfo: sample count, nibble count, rate, looping flag, start / end / current address, coefficients, gain,
+ * start and loop contexts as PredScale, Hist1, Hist2).  ReadIdspData's Stream.DeInterleave reads audio_length =
+ * channel_count * audio_data_length bytes (C# int) at audio_offset = audio_data_offset, in blocks of `interleave`
+ * (interleave_size, or audio_data_length when that is 0), into rows of output_size = SampleCountToByteCount(sample_count)
+ * bytes: a shorter last block, rows zero-filled or truncated, nothing copied when interleave or the per-channel length
+ * is <= 0. */
+typedef struct vgb_idsp_info {
+    int32_t channel_count, sample_rate, sample_count, loop_start, loop_end, interleave_size;
+    int32_t header_size, channel_info_size, audio_data_offset, audio_data_length;
+    int32_t looping, interleave, output_size, reserved;
+    int64_t audio_offset, audio_length;
+    int32_t ch_sample_count[VGB_NW_MAX_CHANNELS], ch_nibble_count[VGB_NW_MAX_CHANNELS], ch_sample_rate[VGB_NW_MAX_CHANNELS];
+    int32_t ch_looping[VGB_NW_MAX_CHANNELS], start_address[VGB_NW_MAX_CHANNELS], end_address[VGB_NW_MAX_CHANNELS];
+    int32_t current_address[VGB_NW_MAX_CHANNELS];
+    int16_t coefs[VGB_NW_MAX_CHANNELS][16];
+    int16_t gain[VGB_NW_MAX_CHANNELS];
+    int16_t start_context[VGB_NW_MAX_CHANNELS][3], loop_context[VGB_NW_MAX_CHANNELS][3];
+} vgb_idsp_info;
+/* IdspReader on a file image, host only.  Every read and check runs in the reference's order and fails with VGB_E_DATA
+ * and the reference's message: "File has no IDSP header", a read past the image, a negative channel-info position
+ * (HeaderSize + i * ChannelInfoSize), and Stream.DeInterleave's checks (Utilities/Interleave.cs:118-133: the region stays
+ * in the image, and its length divides evenly by the channel count - zero channels divide by zero, "Attempted to divide
+ * by zero."; a negative output size overflows).  Refused on purpose: a channel count above VGB_NW_MAX_CHANNELS (255, the
+ * writers' limit) or below 0, right after the main header ("... channels (this reader takes 0..255)"). */
+int32_t vgb_idsp_parse(const uint8_t *file, int64_t length, vgb_idsp_info *info_out);
+
+/* HpsStructure (Containers/Hps/HpsStructure.cs) as HpsReader.ReadFile (Containers/Hps/HpsReader.cs:14-163) leaves it,
+ * big-endian: rate, channel count, per channel (HpsChannelInfo) the max block size, end address, coefficients, gain and
+ * start context; sample_count = NibbleToSample(EndAddress) + 1 of channel 0; looping, loop_start and the loop contexts
+ * from VerifyData; the block chain's length and where it starts (first_block = GetNextMultiple(Max(0x80, position after
+ * the header), 0x20)); loop_block = the index of the loop block, or -1.  channel_audio_bytes[c] is the length of the
+ * channel's concatenated block pieces (ToAudioStream's Sum; INT64 so an overflowing sum can be seen). */
+typedef struct vgb_hps_info {
+    int32_t sample_rate, channel_count, sample_count, looping, loop_start, block_count;
+    int32_t first_block, loop_block;
+    int32_t max_block_size[VGB_NW_MAX_CHANNELS], end_address[VGB_NW_MAX_CHANNELS];
+    int64_t channel_audio_bytes[VGB_NW_MAX_CHANNELS];
+    int16_t coefs[VGB_NW_MAX_CHANNELS][16];
+    int16_t gain[VGB_NW_MAX_CHANNELS];
+    int16_t start_context[VGB_NW_MAX_CHANNELS][3], loop_context[VGB_NW_MAX_CHANNELS][3];
+} vgb_hps_info;
+/* One block of the chain (HpsBlock.cs): where it sits, its Size, FinalNibble and NextOffset.  Channel c's piece of the
+ * block is ReadBytes(AudioSizeBytes = (FinalNibble + 1) / 2 rounded up) at the block's audio start (its header, 12 + 8 *
+ * channel_count bytes, rounded up to a multiple of 0x20) + Size / ChannelCount * c. */
+typedef struct vgb_hps_block {
+    int32_t offset, size, final_nibble, next_offset;
+} vgb_hps_block;
+/* HpsReader on a file image, host only: the header, the chain walk `while (nextBlock > currentBlock)` and VerifyData.
+ * Every read and check runs in the reference's order and fails with VGB_E_DATA and the reference's message: "File has no
+ * HALPST header", a read past the image, a negative position (audio start + Size / ChannelCount * c), a negative
+ * AudioSizeBytes ("Non-negative number required."), "Channels have differing sample counts".  ReadBytes at or past the
+ * end of the image returns a short or empty piece, as in the reference.  Zero or fewer channels end in VerifyData's
+ * First() on an empty list ("Sequence contains no elements.").  Refused on purpose: a channel count above
+ * VGB_NW_MAX_CHANNELS (255, the writers' limit), right after the header.  info_out->block_count is always set on
+ * success; blocks_out (may be NULL) receives the first min(block_count, block_capacity) blocks. */
+int32_t vgb_hps_parse(const uint8_t *file, int64_t length, vgb_hps_info *info_out, vgb_hps_block *blocks_out, int32_t block_capacity);
+
 /* HcaReader.ReadHcaHeader (Containers/Hca/HcaReader.cs:59-121) on a file image, host only: the chunk walk over
  * header_size bytes ("fmt", "comp", "dec", "loop", "ath", "ciph", "rva", "vbr", "comm", "pad"; every id byte masked with
  * 0x7f, so the ids of encrypted files read the same; a later chunk overwrites what an earlier one set), UseAthCurve for
@@ -738,7 +797,26 @@ int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t
  * been written. */
 int32_t vgb_convert_nw_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                                      int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
-/* Bookkeeping of the most recent time-parallel GC-ADPCM decode of vgb_convert_nw_to_wave_batch on this thread's
+/* The decode direction of the batch job for IDSP and HPS streams: .idsp and .hps file images in, 16-bit WAVE images out -
+ * IdspReader / HpsReader (vgb_idsp_parse / vgb_hps_parse) -> ToAudioStream -> GcAdpcmFormat.ToPcm16 -> WaveWriter.
+ * in_type[i] is VGB_CONTAINER_IDSP or VGB_CONTAINER_HPS and names the reader (no sniffing); anything else fails that
+ * file.  Same two-pass protocol, per-file status and sharding as vgb_convert_nw_to_wave_batch (files weigh sample_count *
+ * channel_count).  Per group of files, on the device: one H2D of each IDSP audio region and of each HPS file's span of
+ * block pieces; IDSP rows by the existing de-interleave, HPS rows by hps_gather_kernel (each channel row is the
+ * concatenation of its pieces of every block, as HpsReader.ToAudioStream builds it; rows are cleared first); every row
+ * through the time-parallel GC-ADPCM decoder from the header's coefficients and start history (GcAdpcmChannel.GetPcmAudio;
+ * the HPS per-block and loop contexts are not used, as in the reference); the WAVE join.  The sizing pass, in the
+ * reference's order: a negative sample count (VGB_E_DATA, on purpose), for HPS an overflowing sum of a channel's piece
+ * lengths (VGB_E_DATA) and "Audio array length is too short for the specified number of samples." (GcAdpcmChannel,
+ * VGB_E_ARG), WithLoop's messages when looping (AudioFormatBaseBuilder.cs:23-50, VGB_E_ARG; IDSP with (LoopStart,
+ * LoopEnd), HPS with (LoopStart, SampleCount) - also the WAVE loop), 2 GiB of PCM or more, too many channels for the WAVE
+ * join.  In the fill pass a frame header that selects a predictor 8..15 fails its file alone, as in
+ * vgb_convert_nw_to_wave_batch; with status_out NULL such a file fails the call (VGB_E_DATA) after every other file has
+ * been written. */
+int32_t vgb_convert_idsp_hps_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                                           int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* Bookkeeping of the most recent time-parallel GC-ADPCM decode of vgb_convert_nw_to_wave_batch or
+ * vgb_convert_idsp_hps_to_wave_batch on this thread's
  * context (its last group of files): out[0] segments per channel, [1] frames decoded by run-ons, [2] frames decoded by
  * the cascade, [3] boundaries the cascade repaired, [4] longest run-on in frames.  Synchronises the device. */
 int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n);

@@ -132,6 +132,33 @@ class VgbNwInfo(C.Structure):
         ("start_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS), ("loop_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS)]
 
 
+class VgbIdspInfo(C.Structure):
+    """IdspStructure as IdspReader leaves it, with the region Stream.DeInterleave reads (see the header)."""
+
+    _fields_ = [(n, C.c_int32) for n in ("channel_count", "sample_rate", "sample_count", "loop_start", "loop_end", "interleave_size",
+                                         "header_size", "channel_info_size", "audio_data_offset", "audio_data_length",
+                                         "looping", "interleave", "output_size", "reserved")] + [
+        ("audio_offset", C.c_int64), ("audio_length", C.c_int64)] + [
+        (n, C.c_int32 * VGB_NW_MAX_CHANNELS) for n in ("ch_sample_count", "ch_nibble_count", "ch_sample_rate", "ch_looping", "start_address",
+                                      "end_address", "current_address")] + [
+        ("coefs", (C.c_int16 * 16) * VGB_NW_MAX_CHANNELS), ("gain", C.c_int16 * VGB_NW_MAX_CHANNELS),
+        ("start_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS), ("loop_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS)]
+
+
+class VgbHpsInfo(C.Structure):
+    """HpsStructure as HpsReader leaves it (see the header)."""
+
+    _fields_ = [(n, C.c_int32) for n in ("sample_rate", "channel_count", "sample_count", "looping", "loop_start", "block_count",
+                                         "first_block", "loop_block")] + [
+        ("max_block_size", C.c_int32 * VGB_NW_MAX_CHANNELS), ("end_address", C.c_int32 * VGB_NW_MAX_CHANNELS), ("channel_audio_bytes", C.c_int64 * VGB_NW_MAX_CHANNELS),
+        ("coefs", (C.c_int16 * 16) * VGB_NW_MAX_CHANNELS), ("gain", C.c_int16 * VGB_NW_MAX_CHANNELS),
+        ("start_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS), ("loop_context", (C.c_int16 * 3) * VGB_NW_MAX_CHANNELS)]
+
+
+class VgbHpsBlock(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("offset", "size", "final_nibble", "next_offset")]
+
+
 class VgbConvertOptions(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("out_type", "no_trim", "dsp_samples_per_interleave", "dsp_loop_point_alignment",
                                          "adx_version", "adx_frame_size", "adx_type", "adx_filter_plus1",
@@ -259,6 +286,10 @@ SIGNATURES = {
     "vgb_brstm_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
     "vgb_bcfstm_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
     "vgb_convert_nw_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_idsp_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "vgb_hps_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32]),
+    "vgb_convert_idsp_hps_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p]),
     "vgb_gcadpcm_debug_decode_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_convert_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),

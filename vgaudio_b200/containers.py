@@ -15,7 +15,8 @@ from . import _native as N
 
 CONTAINER_DSP, CONTAINER_ADX, CONTAINER_HCA = 1, 2, 3
 CONTAINER_BRSTM, CONTAINER_BCSTM, CONTAINER_BFSTM = 4, 5, 6   # written by convert_wave_batch, read by convert_nw_to_wave_batch
-CONTAINER_IDSP, CONTAINER_HPS = 7, 8                          # GC-ADPCM only, written by convert_wave_batch
+CONTAINER_IDSP, CONTAINER_HPS = 7, 8                          # GC-ADPCM only, written by convert_wave_batch,
+#                                                               read by convert_idsp_hps_to_wave_batch
 NW_CODEC_PCM8, NW_CODEC_PCM16, NW_CODEC_GCADPCM = 0, 1, 2        # NwCodec; convert_options(nw_codec_plus1=codec + 1)
 
 
@@ -322,6 +323,34 @@ def convert_nw_to_wave_batch(files: Sequence, in_types: Sequence[int]) -> Tuple[
     predictor outside 0..7 fails alone."""
     types = (C.c_int32 * max(len(in_types), 1))(*in_types)
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_nw_to_wave_batch(
+        ftab, lens, types, n, sizes, otab, st), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def idsp_parse(file) -> N.VgbIdspInfo:
+    """IdspReader.ReadFile on a file image; raises VgbError(VGB_E_DATA)."""
+    f = _bytes_arr(file)
+    info = N.VgbIdspInfo()
+    N.check(N.lib.vgb_idsp_parse(f.ctypes.data, f.size, C.byref(info)))
+    return info
+
+
+def hps_parse(file) -> Tuple[N.VgbHpsInfo, List[N.VgbHpsBlock]]:
+    """HpsReader.ReadFile on a file image: (HpsStructure, the block chain in walk order); raises VgbError(VGB_E_DATA)."""
+    f = _bytes_arr(file)
+    info = N.VgbHpsInfo()
+    N.check(N.lib.vgb_hps_parse(f.ctypes.data, f.size, C.byref(info), None, 0))
+    blocks = (N.VgbHpsBlock * max(info.block_count, 1))()
+    N.check(N.lib.vgb_hps_parse(f.ctypes.data, f.size, C.byref(info), blocks, info.block_count))
+    return info, list(blocks[:info.block_count])
+
+
+def convert_idsp_hps_to_wave_batch(files: Sequence, in_types: Sequence[int]) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """The decode direction of the batch job for .idsp / .hps images (in_types: CONTAINER_IDSP or CONTAINER_HPS per file,
+    naming the reader): ([WAVE bytes or None], [per-file status]); a file whose frames select a predictor outside 0..7
+    fails alone."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_idsp_hps_to_wave_batch(
         ftab, lens, types, n, sizes, otab, st), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
 

@@ -823,6 +823,49 @@ constexpr int kWays = 4;  // groups of the batch converter in flight: each has i
 
 }  // namespace
 
+// ---------------------------------------------------------------------------------------------------------------
+// HPS block pieces -> channel rows (HpsReader.ToAudioStream, Containers/Hps/HpsReader.cs:37-50: each channel's audio is
+// the concatenation of its pieces of every block).  One CTA per kHpsGatherTile bytes of one piece.  Hostile chains give
+// pieces of any length at any byte of the image and of the row; writer-made files give whole frames at 0x20 multiples on
+// both sides.  So each tile copies with the widest word the common alignment of its source and destination allows
+// (16, 8 or 4 bytes), byte-wise up to the first aligned address and behind the last whole word, and byte-wise
+// throughout when source and destination disagree below 4 bytes.
+// ---------------------------------------------------------------------------------------------------------------
+namespace vgb {
+
+template <class W>
+__device__ __forceinline__ void gather_words(const uint8_t *src, uint8_t *dst, int n)
+{
+    constexpr int kW = (int)sizeof(W);
+    const int head = min(n, (int)((kW - ((uintptr_t)dst & (kW - 1))) & (kW - 1)));
+    for (int k = threadIdx.x; k < head; k += blockDim.x) dst[k] = src[k];
+    const int words = (n - head) / kW;
+    const W *s = reinterpret_cast<const W *>(src + head);
+    W *d = reinterpret_cast<W *>(dst + head);
+#pragma unroll 4
+    for (int k = threadIdx.x; k < words; k += blockDim.x) d[k] = s[k];
+    for (int k = head + words * kW + threadIdx.x; k < n; k += blockDim.x) dst[k] = src[k];
+}
+
+__global__ void __launch_bounds__(256) hps_gather_kernel(const uint8_t *__restrict__ in, const HpsPiece *__restrict__ pieces, int n_pieces,
+                                                          uint8_t *__restrict__ rows)
+{
+    const int it = find_item(pieces, n_pieces, (int)blockIdx.x);
+    const HpsPiece p = pieces[it];
+    const int b0 = ((int)blockIdx.x - p.tile_first) * kHpsGatherTile;
+    const int n = min(kHpsGatherTile, p.len - b0);
+    if (n <= 0) return;
+    const uint8_t *src = in + p.src_off + b0;
+    uint8_t *dst = rows + p.dst_off + b0;
+    const unsigned mis = (unsigned)((uintptr_t)src ^ (uintptr_t)dst);
+    if ((mis & 15) == 0) gather_words<uint4>(src, dst, n);
+    else if ((mis & 7) == 0) gather_words<uint2>(src, dst, n);
+    else if ((mis & 3) == 0) gather_words<uint32_t>(src, dst, n);
+    else gather_words<uint8_t>(src, dst, n);
+}
+
+}  // namespace vgb
+
 namespace vgb {
 // Created on the context's device, used and freed with that device current.  Lock order: ContainerState::mu before
 // Context::mu (the *_dev codec calls a converter group makes take the latter).

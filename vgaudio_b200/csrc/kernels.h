@@ -85,4 +85,15 @@ cudaError_t launch_interleave(const void *in, int64_t in_channel_stride, int64_t
 cudaError_t launch_deinterleave(const void *in, int64_t in_item_stride, void *out, int64_t out_channel_stride, int64_t out_item_stride,
                                 int n_items, int count, int64_t in_size, int64_t interleave, int64_t out_size, cudaStream_t stream);
 
+// containers.cu — HpsReader.ToAudioStream's concatenation (Containers/Hps/HpsReader.cs:37-50): piece i copies len bytes
+// from in + src_off to rows + dst_off; tile_first numbers its first CTA of kHpsGatherTile bytes (the launch has as many
+// CTAs as the pieces' tiles together, 256 threads each)
+struct HpsPiece {
+    int64_t src_off, dst_off;
+    int32_t len, tile_first;
+};
+constexpr int kHpsGatherTile = 8192;
+__global__ void __launch_bounds__(256) hps_gather_kernel(const uint8_t *__restrict__ in, const HpsPiece *__restrict__ pieces, int n_pieces,
+                                                          uint8_t *__restrict__ rows);
+
 }  // namespace vgb
