@@ -7,8 +7,8 @@ control flow: the loop head is the target of the backward branch that closes it,
 round-1 vote's branch (the first predicate VOTE.ANY), round 1 from there to that branch's target, and the tail from the
 target to the backward branch.  The `i == 15` block at the loop head (wait for and widen the next chunk, once per 16
 frames) is left out.  Opcodes are binned by the pipe that issues them on Hopper: the IMAD family (multiply-add pipe),
-the integer ALU (adds, shifts, logic, min/max, compares, selects) and everything else (shared memory, shuffles,
-votes, control).
+the integer ALU (adds, shifts, logic, min/max, compares, selects), the FP32 instructions (FADD, FFMA, ...) and everything
+else (shared memory, shuffles, votes, conversions, control).
 """
 import argparse
 import os
@@ -21,6 +21,7 @@ KERNEL = "_ZN3vgb16gc_encode_kernelILi{}EEEvPKsNS_14GcChannelTableES2_PhiiNS_9Gc
 LINE = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P[0-9T]\s+)?([A-Z0-9_.]+)\s*([^;]*);")
 ALU = ("IADD3", "VIADD", "LEA", "SHF", "LOP3", "VIMNMX", "VIMNMX3", "VIADDMNMX", "SEL", "ISETP", "PRMT", "IABS", "FLO", "PLOP3",
        "MOV", "BMSK", "UIADD3", "ULOP3", "USHF", "UMOV", "P2R", "R2P", "VABSDIFF", "IMNMX")
+FP32 = ("FADD", "FMUL", "FFMA", "FSETP", "FSEL", "FMNMX")
 
 
 def pipe(op: str) -> str:
@@ -29,6 +30,8 @@ def pipe(op: str) -> str:
         return "imad"
     if root in ALU:
         return "alu"
+    if root in FP32:
+        return "fp32"
     return "other"
 
 
@@ -72,7 +75,7 @@ def main():
     for name, (n, by_pipe, ops) in census(sass(args.obj, args.mode)).items():
         wide = sum(c for op, c in ops.items() if op.startswith("IMAD.WIDE"))
         print(f"{name:8s} {n:5d} instructions: IMAD pipe {by_pipe['imad']:4d} (IMAD.WIDE {wide:3d}), "
-              f"ALU {by_pipe['alu']:4d}, other {by_pipe['other']:4d}")
+              f"ALU {by_pipe['alu']:4d}, FP32 {by_pipe['fp32']:4d}, other {by_pipe['other']:4d}")
         if args.opcodes:
             for op, c in ops.most_common():
                 print(f"    {c:5d} {op}")

@@ -1,7 +1,7 @@
 // tools/microbench.cu — dependent-chain latencies on sm_90a (H100) for the ops the codec kernels' critical paths use.
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 --fmad=false -o tools/microbench tools/microbench.cu
 // Default: one warp, one CTA; cycles per op = (clock after - clock before) / chain length.
-// `microbench t`: issue throughput of the integer pipes with many warps and independent chains (run_tp below).
+// `microbench t`: issue throughput of the integer and FP32 pipes with many warps and independent chains (run_tp below).
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -70,9 +70,13 @@ __global__ void __launch_bounds__(1024, 1) throughput(long long *out, int seed)
 {
     int a[T_CHAINS];
     long long w[T_CHAINS];
+    unsigned lo[T_CHAINS];
+    float f[T_CHAINS];
     const int b = seed * 3 + 1, c = seed ^ 0x55;
+    const int xs = seed * 5 + 1000, xb = xs | 0x4B000000;
+    const float fb = 1.0f + seed * 1e-6f, fc = 0.25f * seed;
 #pragma unroll
-    for (int k = 0; k < T_CHAINS; k++) { a[k] = seed + threadIdx.x * 7 + k; w[k] = a[k]; }
+    for (int k = 0; k < T_CHAINS; k++) { a[k] = seed + threadIdx.x * 7 + k; w[k] = a[k]; lo[k] = a[k]; f[k] = (float)a[k]; }
     __syncthreads();
     const long long t0 = clock64();
 #pragma unroll 4
@@ -100,12 +104,45 @@ __global__ void __launch_bounds__(1024, 1) throughput(long long *out, int seed)
                 x = t_imad(x, c, k);
                 a[k] = __viaddmin_s32_relu(x, 8, 15 + k);
             }
+            // The encoder's per-sample squared error, around a stand-in for its recurrence (IMAD, then the clamp of the
+            // reconstructed sample as VIADDMNMX.RELU) so that every iteration squares a new value.
+            if (OP == 4 || OP == 5) {
+                const int ob = __viaddmin_s32_relu(t_imad(a[k], b, c), 32768, 65535);
+                a[k] = ob;
+                if (OP == 4) {  // miss, then IMAD.WIDE with a 64-bit accumulate: 4 instructions
+                    const int miss = t_imad(ob, -1, xs);
+                    w[k] += (long long)miss * miss;
+                } else {  // float image (LOP3), miss, 32-bit IMAD sum, FADD, FFMA: 7 instructions
+                    const int obb = ob | 0x4B000000;
+                    const int miss = t_imad(obb, -1, xb);
+                    lo[k] = (unsigned)t_imad(miss, miss, (int)lo[k]);
+                    const float mf = __fsub_rn(__int_as_float(xb), __int_as_float(obb));
+                    f[k] = __fmaf_rn(mf, mf, f[k]);
+                }
+            }
+            if (OP == 6) {  // 4 x IMAD + 4 x FFMA: do FP32 instructions take IMAD slots?
+                a[k] = t_imad(a[k], b, c); f[k] = __fmaf_rn(f[k], fb, fc);
+                a[k] = t_imad(a[k], b, k); f[k] = __fmaf_rn(f[k], fc, fb);
+                a[k] = t_imad(a[k], c, b); f[k] = __fmaf_rn(f[k], fb, fb);
+                a[k] = t_imad(a[k], b, i); f[k] = __fmaf_rn(f[k], fc, fc);
+            }
+            if (OP == 7) {  // 2 x IMAD + 2 ALU (LOP3, VIADDMNMX) + FADD + FFMA
+                int x = t_imad(a[k], b, c) ^ i;
+                x = t_imad(x, c, k);
+                a[k] = __viaddmin_s32_relu(x, 8, 15 + k);
+                const float g = __fadd_rn(f[k], fb);
+                f[k] = __fmaf_rn(g, fc, fb);
+            }
+            if (OP == 8) {  // 4 x FFMA
+                f[k] = __fmaf_rn(f[k], fb, fc); f[k] = __fmaf_rn(f[k], fc, fb);
+                f[k] = __fmaf_rn(f[k], fb, fb); f[k] = __fmaf_rn(f[k], fc, fc);
+            }
         }
     }
     const long long t1 = clock64();
     long long s = 0;
 #pragma unroll
-    for (int k = 0; k < T_CHAINS; k++) s += a[k] + w[k];
+    for (int k = 0; k < T_CHAINS; k++) s += a[k] + w[k] + lo[k] + (long long)f[k];
     if (threadIdx.x == 0) out[2 * blockIdx.x] = t1 - t0;
     if (s == 0x123456789LL) out[2 * blockIdx.x + 1] = s;  // keeps the chains alive
 }
@@ -126,8 +163,9 @@ void run_tp(const char *name, int ops_per_chain_iter)
     for (int i = 0; i < sms; i++) cyc += (double)h[2 * i];
     cyc /= sms;
     const double warp_instr = 32.0 * T_ITER * T_CHAINS * ops_per_chain_iter;  // per CTA = per SM
-    printf("%-44s %6.3f warp instr / clk / sub-partition (%d ops x %d chains per iter, %.0f cycles)\n", name,
-           warp_instr / (cyc * 4.0), ops_per_chain_iter, T_CHAINS, cyc);
+    // cycles per body: sub-partition cycles per loop body of one chain of one warp (8 warps per sub-partition)
+    printf("%-52s %6.3f warp instr / clk / sub-partition, %5.2f cycles per body (%d ops x %d chains per iter, %.0f cycles)\n",
+           name, warp_instr / (cyc * 4.0), cyc * 4.0 / (32.0 * T_ITER * T_CHAINS), ops_per_chain_iter, T_CHAINS, cyc);
     delete[] h;
     cudaFree(d_out);
 }
@@ -139,6 +177,11 @@ int main(int argc, char **argv)
         run_tp<1>("IMAD.WIDE + 64-bit sum (IMAD.WIDE only; +LOP3)", 1);
         run_tp<2>("ALU only (LOP3 LEA.HI SHF VIMNMX VIADDMNMX)", 5);
         run_tp<3>("IMAD / ALU 50/50 (IMAD IADD3 IMAD VIADDMNMX)", 4);
+        run_tp<4>("error, 64-bit (IMAD VIADDMNMX IMAD IMAD.WIDE)", 4);
+        run_tp<5>("error, IMAD + FP32 (IMAD VIADDMNMX LOP3 2xIMAD FADD FFMA)", 7);
+        run_tp<6>("IMAD / FFMA 50/50", 8);
+        run_tp<7>("IMAD / ALU / FP32 (2 IMAD, LOP3 VIADDMNMX, FADD FFMA)", 6);
+        run_tp<8>("FFMA only", 4);
         return 0;
     }
     run<0>("IMAD a=a*b+7", 1);

@@ -51,6 +51,11 @@ constexpr int kEncRowPad = 4;                                         // int32 w
 #endif
 constexpr int kEncChainBlocksPerSm = VGB_ENC_BLOCKS_PER_SM;               // register budget of the chain launch: 8 CTAs x 2 warps = 4 warps per sub-partition
 constexpr uint32_t kErrSat = (1u << 27) - 1;                          // one 32-bit argmin while err < 2^27 - 1
+// The bits 0x4B000000 + v are the float32 2^23 + v for 0 <= v < 2^23, so a biased sample in [0, 65535] carries its own
+// float image.  The staged samples hold x + kStageBias; every integer use of them is a wrapping multiply-add whose
+// constant absorbs the image (0x4B000000 * 2048 == 0 modulo 2^32).
+constexpr uint32_t kFloatImage = 0x4B000000u;
+constexpr uint32_t kStageBias = 32768u + kFloatImage;
 
 template <bool kGeneral>
 struct GcTrial {
@@ -167,15 +172,16 @@ __device__ __forceinline__ uint32_t gc_peak_key(int32_t older, int32_t newer, in
 // two samples at a time.  gc_peak_pack folds the pair back into the key format above (|distance| << 5 | order << 1 |
 // sign); Clamp16 (:113) is applied to the winner there - clamping commutes with the maximum, and among clamped
 // samples sign and order no longer matter: every |distance| >= 18432 gives scalePower 12 whatever its sign.
-// All three samples carry the +32768 bias of the staged data; neg_bias = -32768 * (c0 + c1) removes it from the sum.
+// All three samples carry kStageBias, the bias of the staged data; neg_bias = -kStageBias * (c0 + c1) removes it from
+// the sum (modulo 2^32: the true sums fit in int32, so the wrapping ones are exact).
 __device__ __forceinline__ void gc_peak_terms(int32_t older, int32_t newer, int32_t cur, int32_t c0, int32_t c1, int s,
                                               int32_t neg_bias, int32_t &tp, int32_t &tn)
 {
     const int32_t g = imad(newer, c0, imad(older, c1, neg_bias));
     const int32_t q = (int32_t)(g + (int32_t)((uint32_t)(g >> 31) >> 21)) >> 11;  // g / 2048, truncating toward zero (A.6)
-    const int32_t d = imad(q, -1, cur);                                           // distance + 32768; |distance| < 2^21
-    tp = imad(d, 16, 15 - s - 32768 * 16);
-    tn = imad(d, -16, 15 - s + 32768 * 16);
+    const int32_t d = imad(q, -1, cur);                                           // distance + kStageBias; |distance| < 2^21
+    tp = imad(d, 16, (int32_t)(15u - s - kStageBias * 16u));
+    tn = imad(d, -16, (int32_t)(15u - s + kStageBias * 16u));
 }
 __device__ __forceinline__ uint32_t gc_peak_pack(int32_t kp, int32_t kn)
 {
@@ -253,7 +259,8 @@ struct GcPass {
     uint32_t nearmin;    // smallest distance of (diff + half) to a multiple of 2^shift, scaled
     uint32_t near_even;  // that distance of the last even sample (folded in with the odd one)
     uint32_t nw0, nw1;   // nibbles, biased +8
-    uint64_t e0, e1;     // squared error of even / odd samples (exact; < 2^36)
+    uint32_t elo;        // squared error modulo 2^32 (the wrap is intended; the error is < 14 * 2^32)
+    float ef;            // the same sum in float32, within 2^16 of it: the multiple of 2^32 (gc_err_exact)
 };
 
 __device__ __forceinline__ void gc_pass_begin(GcPass &P, int sp_raw, int32_t bias_c, int32_t p1, int32_t p2)
@@ -274,16 +281,21 @@ __device__ __forceinline__ void gc_pass_begin(GcPass &P, int sp_raw, int32_t bia
     P.nearmin = 0xFFFFFFFFu;
     P.near_even = 0xFFFFFFFFu;
     P.nw0 = 0; P.nw1 = 0;
-    P.e0 = 0; P.e1 = 0;
+    P.elo = 0; P.ef = 0.0f;
 }
 
-// Sample s (a compile-time constant once unrolled) of the recurrence; xs = the sample, biased +32768, and xw = xs * 2048
-// (shared by the lane's passes).  Per sample the dependent chain is IMAD -> IADD3 -> LEA.HI -> SHF -> VIADDMNMX.RELU ->
-// IMAD -> VIADDMNMX.RELU; range of raw (maxOverflow), distance to a rounding threshold, squared error and nibble
-// packing ride along as independent work and nothing per sample is kept in registers.  The IMAD and the integer ALU
-// pipes each take one warp instruction every two cycles (DESIGN.md §5.3), so the side work is split between them:
-// tm1 is rebuilt from wf with one IADD3 instead of its own multiply-adds (modulo 2^32,
-// x*2048 + base_m - c0*r1 - c1*r2 == x*2048 + base_t - wf).
+// Sample s (a compile-time constant once unrolled) of the recurrence; xs = the staged sample (x + kStageBias), and
+// xw = xs * 2048 = (x + 32768) * 2048 (shared by the lane's passes).  Per sample the dependent chain is IMAD -> IADD3 ->
+// LEA.HI -> SHF -> VIADDMNMX.RELU -> IMAD -> VIADDMNMX.RELU; range of raw (maxOverflow), distance to a rounding
+// threshold, squared error and nibble packing ride along as independent work and nothing per sample is kept in
+// registers.  The IMAD and the integer ALU pipes each take one warp instruction every two cycles (DESIGN.md §5.3), so
+// the side work is split between them: tm1 is rebuilt from wf with one IADD3 instead of its own multiply-adds (modulo
+// 2^32, x*2048 + base_m - c0*r1 - c1*r2 == x*2048 + base_t - wf).  The squared error stays off IMAD.WIDE (a 64-bit
+// accumulate takes three IMAD slots): a 32-bit IMAD sums it modulo 2^32 and the FP32 pipe, idle otherwise, sums it
+// again in float32 (an FP32 instruction costs about half an IMAD slot).  The float images of the sample and of the
+// reconstruction are in [2^23, 2^24), so their difference is the exact miss; each FFMA rounds once, by at most 2^11
+// below 2^36, so the float sum is within 14 * 2^11 < 2^16 of the exact one (tools/gc_err_check.c checks that bound on
+// worst-case frames).
 __device__ __forceinline__ void gc_pass_step(GcPass &P, int s, int32_t xs, int32_t xw, int32_t c0, int32_t c1)
 {
     const int32_t gn = imad(P.r2, c1, P.base_g);     // r2 term: one step off the chain
@@ -307,9 +319,11 @@ __device__ __forceinline__ void gc_pass_step(GcPass &P, int s, int32_t xs, int32
     const uint32_t near = (uint32_t)imad(tm1, P.lmul, (int32_t)P.near_k);   // (tm1 << lsh) + near_k
     if (s & 1) P.nearmin = __vimin3_u32(P.nearmin, P.near_even, near);
     else P.near_even = near;
-    const int32_t miss = imad(ob, -1, xs);
-    const uint64_t sq = (uint64_t)((int64_t)miss * miss);
-    if (s & 1) P.e1 += sq; else P.e0 += sq;
+    const int32_t obf = (int32_t)((uint32_t)ob | kFloatImage);   // float image of ob: 2^23 + ob
+    const int32_t miss = imad(obf, -1, xs);                        // x - out: the images cancel
+    P.elo = (uint32_t)imad(miss, miss, (int32_t)P.elo);
+    const float mf = __fsub_rn(__int_as_float(xs), __int_as_float(obf));  // x - out, exact
+    P.ef = __fmaf_rn(mf, mf, P.ef);  // explicit: the build runs with --fmad=false
     const int byte = 1 + s / 2, bit = (byte & 3) * 8 + ((s & 1) ? 0 : 4);
     if (byte < 4) P.nw0 = (uint32_t)imad(qb, 1 << bit, (int32_t)P.nw0);
     else P.nw1 = (uint32_t)imad(qb, (int32_t)(1u << bit), (int32_t)P.nw1);  // disjoint bit fields: add == or
@@ -336,6 +350,14 @@ __device__ __forceinline__ void gc_pass_end(const GcPass &P, bool &term, bool &t
     const bool near = (P.nearmin <= 2u * P.near_c) | over_ge_240;
     trouble = P.valid & ((huge | (big & near)) | ((P.sp < 12) & over_gt_248));
     term = P.valid & (over_le_1 | (P.sp >= 12));
+}
+
+// The exact squared error of a pass from its two sums: err = ef + d with |d| < 2^16, and err == elo modulo 2^32.  Only
+// the loud-frame argmin needs it; below 2^31, ef already proves err == elo (the tail's saturated key).
+__device__ __forceinline__ uint64_t gc_err_exact(float ef, uint32_t elo)
+{
+    const uint64_t approx = __float2ull_rz(ef);  // a whole number (every float32 >= 2^24 is one, and below it the sum is exact)
+    return approx + (uint64_t)(int64_t)(int32_t)(elo - (uint32_t)approx);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -427,6 +449,7 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
     const int32_t c0 = coefs[(int64_t)ch * 16 + 2 * pred];
     const int32_t c1 = coefs[(int64_t)ch * 16 + 2 * pred + 1];
     const int32_t bias_c = wmul(32768, wadd(c0, c1));  // undoes the +32768 bias of both history samples
+    const int32_t neg_bias_s = (int32_t)(0u - kStageBias * (uint32_t)wadd(c0, c1));  // undoes kStageBias (gc_peak_terms)
     int16_t (*const in_row)[kEncChunkSamples] = in_buf[warp][qc];
     int32_t *const x_row = x_buf[warp][qc];
 
@@ -454,7 +477,8 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
         __syncwarp();
     };
     // int16 -> int32 once per chunk (frames pred and pred + 8 of the chunk) instead of a 16-bit load and a sign
-    // extension per sample use: the frame loop then reads whole 64-bit pairs, broadcast to the 8 lanes of a channel
+    // extension per sample use: the frame loop then reads whole 64-bit pairs, broadcast to the 8 lanes of a channel.
+    // Stored as x + kStageBias: the +32768 bias and the float image of the biased sample
     auto widen_chunk = [&](int b) {
 #pragma unroll
         for (int h = 0; h < 2; h++) {
@@ -464,7 +488,8 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
 #pragma unroll
             for (int k = 0; k < kGcFrameSamples / 2; k++) {
                 const uint32_t w = from[k];
-                to[k] = make_int2((int32_t)(int16_t)(w & 0xFFFFu) + 32768, ((int32_t)w >> 16) + 32768);  // stored with the +32768 bias
+                to[k] = make_int2((int32_t)((uint32_t)(int16_t)(w & 0xFFFFu) + kStageBias),
+                                  (int32_t)((uint32_t)((int32_t)w >> 16) + kStageBias));
             }
         }
         __syncwarp();
@@ -478,8 +503,8 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
 #pragma unroll
         for (int j = 2; j < 14; j += 2) {
             int32_t tpa, tna, tpb, tnb;
-            gc_peak_terms(v[j - 2], v[j - 1], v[j], c0, c1, j, -bias_c, tpa, tna);
-            gc_peak_terms(v[j - 1], v[j], v[j + 1], c0, c1, j + 1, -bias_c, tpb, tnb);
+            gc_peak_terms(v[j - 2], v[j - 1], v[j], c0, c1, j, neg_bias_s, tpa, tna);
+            gc_peak_terms(v[j - 1], v[j], v[j + 1], c0, c1, j + 1, neg_bias_s, tpb, tnb);
             kp = __vimax3_s32(kp, tpa, tpb);
             kn = __vimax3_s32(kn, tna, tnb);
         }
@@ -488,12 +513,13 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
 
     // ---- jobs: a chain job is one segment; a run-on job is one segment boundary; the cascade walks the boundaries ----
     const int job_first = kMode == kGcChain ? (int)blockIdx.y : (kMode == kGcRunOn ? (int)blockIdx.y + 1 : 1);
-    const int job_last = kMode == kGcCascade ? sa.seg_count - 1 : job_first;
+    const int n_jobs = kMode == kGcCascade ? sa.seg_count - 1 : 1;  // a compile-time 1 for chain and run-on: no job loop
     int truth_upto = 0;           // cascade: frames below this index were finished by an earlier job of this pass
     int reencoded = 0;            // run-on / cascade statistics (frames encoded again)
     int32_t p1 = 0, p2 = 0;       // biased history (newest, older)
 
-    for (int job = job_first; job <= job_last; job++) {
+    for (int j = 0; j < n_jobs; j++) {
+        const int job = job_first + j;
         const int seg_lo = frame_begin + job * seg_len;   // this channel's first frame (a multiple of 16 past frame_begin)
         bool need = live && seg_lo < f_end;
         uint32_t start_pair = 0;
@@ -556,22 +582,24 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
             const bool active = i < frames_here && !spliced;  // a finished channel idles while its warp mates go on
             const int32_t *frame = chunk + i * kGcFrameSamples;
             const int32_t *frame_next = (i + 1 < kEncChunkFrames) ? frame + kGcFrameSamples : other;
-            // the frame's samples, biased (same address for the 8 lanes of a channel: broadcast).  Not carried in
-            // registers from the previous frame: 14 registers fewer per thread buy resident warps
+            // the frame's samples, x + kStageBias (same address for the 8 lanes of a channel: broadcast).  Not carried
+            // in registers from the previous frame: 14 registers fewer per thread buy resident warps
             int32_t x[14];
 #pragma unroll
             for (int j = 0; j < 14; j++) x[j] = frame[j];
 
             // ---------------- head ----------------
             int32_t tp0, tn0, tp1, tn1;
-            gc_peak_terms(p2, p1, x[0], c0, c1, 0, -bias_c, tp0, tn0);
-            gc_peak_terms(p1, x[0], x[1], c0, c1, 1, -bias_c, tp1, tn1);
+            const int32_t p1s = (int32_t)((uint32_t)p1 + kFloatImage), p2s = (int32_t)((uint32_t)p2 + kFloatImage);
+            gc_peak_terms(p2s, p1s, x[0], c0, c1, 0, neg_bias_s, tp0, tn0);
+            gc_peak_terms(p1s, x[0], x[1], c0, c1, 1, neg_bias_s, tp1, tn1);
             const uint32_t key = min(max(key_rest, gc_peak_pack(max(tp0, tp1), max(tn0, tn1))), kPeakKeyMax);
             const int sp_first = gc_first_scale_power(key);
 
             // result of this lane's chain-ending pass (or its latest, while unresolved)
             uint32_t w0 = 0, w1 = 0;
-            uint64_t err = 0;
+            uint32_t elo = 0;   // its squared error modulo 2^32 ...
+            float ef = 0.0f;    // ... and in float32 (GcPass)
             int sp = 0;
             int32_t q1 = p1, q2 = p2;  // newest two reconstructed samples of that pass (biased)
             uint32_t key_rest_next = 0;
@@ -604,7 +632,8 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
                 const bool use_b = round == 0 && !term_a;
                 if (take) {
                     trouble = trouble | (active & (trouble_a | (use_b & trouble_b)));
-                    err = use_b ? B.e0 + B.e1 : A.e0 + A.e1;
+                    elo = use_b ? B.elo : A.elo;
+                    ef = use_b ? B.ef : A.ef;
                     w0 = (use_b ? B.nw0 : A.nw0) ^ 0x88888800u;  // remove the +8 nibble bias (q & 15 == (q + 8) ^ 8)
                     w1 = (use_b ? B.nw1 : A.nw1) ^ 0x88888888u;
                     sp = use_b ? B.sp : A.sp;
@@ -618,13 +647,14 @@ gc_encode_kernel(const int16_t *__restrict__ pcm, GcChannelTable tab, const int1
             trouble = trouble | !resolved;
 
             // ---------------- tail: argmin over predictors ----------------
-            // first minimum wins (:66-76): the key is monotone in the predictor
-            const uint32_t e_sat = err < (uint64_t)kErrSat ? (uint32_t)err : kErrSat;
+            // first minimum wins (:66-76): the key is monotone in the predictor.  ef < 2^31 proves err < 2^32, so
+            // err == elo; otherwise err > 2^31 - 2^16 > kErrSat.
+            const uint32_t e_sat = ef < 2147483648.0f ? min(elo, kErrSat) : kErrSat;
             uint32_t best = quarter_min_u32(active ? ((e_sat << 3) | (uint32_t)pred) : 0xFFFFFFFFu);
             const bool sat = (best >> 3) >= kErrSat && best != 0xFFFFFFFFu;
             if (__any_sync(kFull, sat)) {
                 // loud frame (warp-uniform): candidate errors of >= 2^27 - 1, reduce on the full 64-bit value
-                const uint64_t full_key = active ? ((err << 3) | (uint64_t)pred) : ~0ull;
+                const uint64_t full_key = active ? ((gc_err_exact(ef, elo) << 3) | (uint64_t)pred) : ~0ull;
                 const uint32_t hi = (uint32_t)(full_key >> 16);
                 const uint32_t min_hi = quarter_min_u32(hi);
                 best = quarter_min_u32(hi == min_hi ? (uint32_t)(full_key & 0xFFFFu) : 0xFFFFFFFFu);  // low 3 bits = winner
