@@ -144,6 +144,14 @@ namespace VGAudio.Native
         public static extern int vgb_convert_hca_to_wave_batch(byte** files, long* lengths, int nFiles, ulong* keyCode, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_brstm_parse(byte* file, long length, VgbNwInfo* info);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_bcfstm_parse(byte* file, long length, VgbNwInfo* info);
+        // NintendoWare wave files and prefetch streams (read only), named by the reader the extension picks (ContainerTypes.cs)
+        public const int VGB_CONTAINER_BRWAV = 9;    // BrwavReader: .brwav .rwav
+        public const int VGB_CONTAINER_BCWAV = 10;   // BCFstmReader: .bcwav .cwav .bms
+        public const int VGB_CONTAINER_BFWAV = 11;   // BCFstmReader: .bfwav
+        public const int VGB_CONTAINER_BCSTP = 12;   // BCFstmReader: .bcstp
+        public const int VGB_CONTAINER_BFSTP = 13;   // BCFstmReader: .bfstp
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_nw_file_parse(byte* file, long length, int inType, VgbNwInfo* info, long* channelOffsets);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_nw_to_wave_batch(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_idsp_parse(byte* file, long length, VgbIdspInfo* info);
@@ -352,10 +360,12 @@ namespace VGAudio.Cli
             }
         }
 
-        // The decode direction for a chunk of NintendoWare streams (`-b --out-format wav` over .brstm / .bcstm / .bfstm): the
-        // reader the extension names (ContainerTypes.cs: BrstmReader for .brstm, BCFstmReader for .bcstm and .bfstm) ->
-        // ToPcm16 -> WaveWriter per file in one native call per pass.  inTypes[i] is VGB_CONTAINER_BRSTM / _BCSTM / _BFSTM
-        // (4 / 5 / 6).  A file whose GC-ADPCM frames select a predictor outside 0..7 fails in the second pass alone.
+        // The decode direction for a chunk of NintendoWare files (`-b --out-format wav` over .brstm / .bcstm / .bfstm, the
+        // wave files .brwav / .rwav / .bcwav / .cwav / .bms / .bfwav and the prefetch streams .bcstp / .bfstp): the reader
+        // the extension names (ContainerTypes.cs: BrstmReader, BrwavReader, BCFstmReader for the others) -> ToPcm16 ->
+        // WaveWriter per file in one native call per pass.  inTypes[i] is VGB_CONTAINER_BRSTM / _BCSTM / _BFSTM (4 / 5 / 6)
+        // or VGB_CONTAINER_BRWAV / _BCWAV / _BFWAV / _BCSTP / _BFSTP (9 .. 13).  A file whose GC-ADPCM frames select a
+        // predictor outside 0..7 fails in the second pass alone.
         public static unsafe void ConvertNwToWave(string[] inPaths, int[] inTypes, string[] outPaths, Action<string> log, Action<int> reportAdd)
         {
             ConvertTypedToWave(inPaths, inTypes, outPaths, log, reportAdd, VgAudioB200Containers.vgb_convert_nw_to_wave_batch);

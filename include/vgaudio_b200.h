@@ -592,10 +592,35 @@ typedef struct vgb_nw_info {
  * region stays in the image and splits evenly over the channels).  Refused on purpose, where the reference would fail
  * later or read something these readers do not carry: codec 3 (IMA; ToAudioStream returns null) and any codec above
  * it, a GC-ADPCM stream with fewer channel infos than channels, and CWAV / FWAV / CSTP / FSTP images, wave info blocks
- * and prefetch / wave data blocks (BCFstmReader accepts them; "... are not read").  vgb_bcfstm_parse accepts CSTM and
- * FSTM alike. */
+ * and prefetch / wave data blocks (BCFstmReader accepts them; "... are not read" - vgb_nw_file_parse with a wave or
+ * prefetch type reads them).  vgb_bcfstm_parse accepts CSTM and FSTM alike. */
 int32_t vgb_brstm_parse(const uint8_t *file, int64_t length, vgb_nw_info *info_out);
 int32_t vgb_bcfstm_parse(const uint8_t *file, int64_t length, vgb_nw_info *info_out);
+/* Every NintendoWare reader behind one call, host only; in_type (VGB_CONTAINER_*) names the reader as the file extension
+ * does in the reference.  BRSTM, BCSTM and BFSTM behave exactly as vgb_brstm_parse / vgb_bcfstm_parse, through the same
+ * code.  BCWAV, BFWAV, BCSTP and BFSTP run the whole BCFstmReader (BCFstmReader.cs:14-288) on any of its six magics:
+ * the wave info block (StreamInfo.ReadBfwav: the unaligned loop start from BFWAV 0.1.2 / BCWAV 2.1.1, the channel count
+ * peeked from the channel reference table; ChannelInfo.ReadBfstm with the wave channels' audio offsets, GC-ADPCM info
+ * without gain), the wave data block and the prefetch data block.  BRWAV runs BrwavReader (BrwavReader.cs,
+ * RwavWaveInfo.cs, RwavChannelInfo.cs), big-endian; as in the reference its loop start and sample count go through
+ * NibbleToSample whatever the codec, and every channel's coefficients, gain and contexts are read at its ADPCM info
+ * offset whatever the codec.  info_out describes what Common.ToAudioStream builds:
+ *   - a wave file (a wave data block, or BRWAV): each channel is ReadBytes(SamplesToBytes(sample_count)) at its own
+ *     offset behind the DATA header, so a channel's bytes may be shorter than output_size (or empty) at the image's end;
+ *     interleave_size = 0; channel_offsets_out[c] (c < channel_count) is the absolute file offset of channel c's bytes;
+ *     audio_offset / audio_length span the channels' bytes that lie in the image (0 / 0 when none do);
+ *   - a prefetch file (a PDAT block): the region and geometry of the first entry, read as a stream by Stream.DeInterleave
+ *     (PDAT size bytes, rows of that size); sample_count = BytesToSamples(size / channel_count) and looping = 0, as
+ *     ToAudioStream sets them;
+ *   - a stream: as vgb_bcfstm_parse.
+ * channel_offsets_out (VGB_NW_MAX_CHANNELS entries, or NULL) is -1 wherever no wave channel is described.  The reference's
+ * failures, with its messages: a channel position before the image, a channel reference that is not a wave channel
+ * (WaveAudioOffsets[i] is out of range), no channel info at all (a null reference), a wave info block with a stream
+ * data block (no audio reference), a PDAT count of 0 (PrefetchData[0] is out of range), a prefetch file of 0 channels
+ * (a divide by zero), a negative wave channel length (new byte[n]).  Refused on purpose: codec 3 (IMA) and above, as
+ * for the streams, and a wave info block of more than 255 (or fewer than 0) channels.  An in_type that names no
+ * NintendoWare reader is VGB_E_ARG. */
+int32_t vgb_nw_file_parse(const uint8_t *file, int64_t length, int32_t in_type, vgb_nw_info *info_out, int64_t *channel_offsets_out);
 
 /* IdspStructure (Containers/Idsp/IdspStructure.cs) as IdspReader.ReadFile (Containers/Idsp/IdspReader.cs:13-112) leaves
  * it, big-endian: the main header's fields, looping (set when any channel's flag is 1), and per channel its header
@@ -704,6 +729,15 @@ int32_t vgb_hca_write_batch(const vgb_hca_info *info, int32_t n_files, const uin
  * input's last sample, where HpsWriter reads the block's history past the unaligned decode (IndexOutOfRangeException). */
 #define VGB_CONTAINER_IDSP 7
 #define VGB_CONTAINER_HPS 8
+/* NintendoWare wave files and prefetch streams, named by the reader the reference picks for the file extension
+ * (src/VGAudio.Cli/ContainerTypes.cs).  They are read only: vgb_nw_file_parse and vgb_convert_nw_to_wave_batch take them;
+ * vgb_convert_wave_batch does not take them as a target and vgb_transcode_batch not as a source (the reference has no
+ * writer for them).  BCFstmReader accepts any of its six magics under any of the four BCFstmReader types. */
+#define VGB_CONTAINER_BRWAV 9    /* BrwavReader: .brwav .rwav */
+#define VGB_CONTAINER_BCWAV 10   /* BCFstmReader: .bcwav .cwav .bms */
+#define VGB_CONTAINER_BFWAV 11   /* BCFstmReader: .bfwav */
+#define VGB_CONTAINER_BCSTP 12   /* BCFstmReader: .bcstp */
+#define VGB_CONTAINER_BFSTP 13   /* BCFstmReader: .bfstp */
 typedef struct vgb_convert_options {
     int32_t out_type;                   /* VGB_CONTAINER_* */
     int32_t no_trim;                    /* Configuration.TrimFile = !no_trim */
@@ -774,12 +808,20 @@ int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t
  * status_out NULL such a file fails the call (VGB_E_DATA) after every other file has been written. */
 int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_adx_key *key,
                                       int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
-/* The decode direction of the batch job for NintendoWare streams: .brstm, .bcstm and .bfstm file images in, 16-bit
- * WAVE images out - BrstmReader / BCFstmReader (vgb_brstm_parse / vgb_bcfstm_parse) -> Common.ToAudioStream
- * (Containers/NintendoWare/Common.cs:45-116) -> ToPcm16 -> WaveWriter.  in_type[i] (VGB_CONTAINER_BRSTM, _BCSTM or
- * _BFSTM) names the reader, as the reference picks one by file extension: BRSTM uses BrstmReader, BCSTM and BFSTM both
- * use BCFstmReader, which accepts either magic; the magic is not sniffed, so a .bcstm image passed as BRSTM fails as in
- * the reference.  Same two-pass protocol, per-file status and sharding as vgb_convert_adx_to_wave_batch (files weigh
+/* The decode direction of the batch job for NintendoWare files: .brstm, .bcstm and .bfstm streams, .brwav, .bcwav and
+ * .bfwav wave files and .bcstp / .bfstp prefetch streams in, 16-bit WAVE images out - BrstmReader / BrwavReader /
+ * BCFstmReader (vgb_nw_file_parse) -> Common.ToAudioStream (Containers/NintendoWare/Common.cs:45-116) -> ToPcm16 ->
+ * WaveWriter.  in_type[i] (VGB_CONTAINER_BRSTM, _BCSTM, _BFSTM, _BRWAV, _BCWAV, _BFWAV, _BCSTP or _BFSTP; any other
+ * value, IDSP and HPS included, fails that file) names the reader, as the reference picks one by file extension: BRSTM
+ * uses BrstmReader, BRWAV BrwavReader, the others BCFstmReader, which accepts any of its magics (the stream types
+ * refuse wave and prefetch files on purpose); the magic is not sniffed, so a .bcstm image passed as BRSTM fails as in
+ * the reference.  A wave file's channels are separate runs: their bytes (ReadBytes, short or empty at the image's end)
+ * are gathered into the channel rows by hps_gather_kernel, one launch per group, in place of the de-interleave; a
+ * prefetch file's first region goes through the de-interleave as a stream.  The sizing pass adds ToAudioStream's checks
+ * on such rows: GcAdpcmChannel's "Audio array length is too short for the specified number of samples." (VGB_E_ARG);
+ * for PCM, the builders' sample count from channel 0's row ("All channels must have the same sample count", a
+ * big-endian PCM16 row of odd length indexes past it, VGB_E_DATA), WithLoop(Looping, LoopStart, SampleCount) against
+ * that count, and "Channels parameter cannot be empty or null" for no channels.  The WAVE holds that many samples.  Same two-pass protocol, per-file status and sharding as vgb_convert_adx_to_wave_batch (files weigh
  * sample_count * channel_count).  Per group of files, on the device: one H2D of the DATA regions, the existing
  * de-interleave (Stream.DeInterleave: a shorter last block, rows of SamplesToBytes(sample_count) bytes zero-filled or
  * truncated; an interleave size <= 0 copies nothing, so the rows are zeros), then the GC-ADPCM rows through the
@@ -789,7 +831,7 @@ int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t
  * when looping, extensible fmt above two channels), one D2H of the finished files.  Gain, tracks, regions and seek
  * tables do not change the output and are not read by the decode.  Loop points follow WithLoop(Looping, LoopStart,
  * SampleCount) (AudioFormatBaseBuilder.cs:23-50; VGB_E_ARG with its messages).  Per-file errors, each failing that
- * file only: in_type not one of the three, a parse error, bad loop points, a negative sample count (refused on purpose:
+ * file only: in_type not one of the eight, a parse error, bad loop points, a negative sample count (refused on purpose:
  * the reference allocates from it), 2 GiB of PCM or more, too many channels for the WAVE join - all known in the sizing
  * pass - and, found on the device in the fill pass, a GC-ADPCM frame header that selects a predictor 8..15 (the
  * reference indexes coefficients[predictor * 2] and throws): that file gets its status_out entry, out_sizes[i] = 0 and

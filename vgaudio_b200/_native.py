@@ -285,6 +285,7 @@ SIGNATURES = {
     "vgb_convert_adx_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_brstm_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
     "vgb_bcfstm_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "vgb_nw_file_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
     "vgb_convert_nw_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_idsp_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
     "vgb_hps_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32]),

@@ -1,6 +1,7 @@
 // vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
 // .dsp / .adx / .hca, WAVE files to .brstm / .bcstm / .bfstm / .idsp / .hps, and .dsp, .adx, .hca, .brstm, .bcstm, .bfstm,
-// .idsp and .hps files to WAVE.
+// .idsp and .hps files, the NintendoWare wave files (.brwav / .rwav, .bcwav / .cwav / .bms, .bfwav) and prefetch
+// streams (.bcstp, .bfstp) to WAVE.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
@@ -8,7 +9,7 @@
 // (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch for coded files, vgb_convert_*_to_wave_batch for
 // --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
-//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp and .hps inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
+//   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav, .bcstp and .bfstp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
 //
@@ -47,17 +48,23 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
     return n == 0 || (bool)f.read(reinterpret_cast<char *>(out.data()), n);
 }
 
-// the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, 4 .brstm, 5 .bcstm, 6 .bfstm, 7 .idsp, 8 .hps, -1 none of
-// them.  The extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs).  The NintendoWare,
-// IDSP and HPS streams are decoded to WAVE with --out-format wav, and written from WAVE inputs only with --out-format
-// brstm|bcstm|bfstm|idsp|hps; another --out-format does not take them as inputs.
+// the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, 4 .brstm, 5 .bcstm, 6 .bfstm, 7 .idsp, 8 .hps, 9 .brwav /
+// .rwav, 10 .bcwav / .cwav / .bms, 11 .bfwav, 12 .bcstp, 13 .bfstp, -1 none of them (from 4 on, the kind is the
+// VGB_CONTAINER_* of its reader).  The extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs).
+// The NintendoWare, IDSP and HPS streams are decoded to WAVE with --out-format wav, and written from WAVE inputs only
+// with --out-format brstm|bcstm|bfstm|idsp|hps; the wave and prefetch files are decoded to WAVE only.  Another
+// --out-format does not take them as inputs.
 static int kind_of(const fs::path &p)
 {
     std::string ext = p.extension().string();
     std::transform(ext.begin(), ext.end(), ext.begin(), ::tolower);
     return ext == ".dsp" ? 0 : ext == ".hca" ? 1 : ext == ".adx" ? 2 : (ext == ".wav" || ext == ".wave") ? 3
-         : ext == ".brstm" ? 4 : ext == ".bcstm" ? 5 : ext == ".bfstm" ? 6 : ext == ".idsp" ? 7 : ext == ".hps" ? 8 : -1;
+         : ext == ".brstm" ? 4 : ext == ".bcstm" ? 5 : ext == ".bfstm" ? 6 : ext == ".idsp" ? 7 : ext == ".hps" ? 8
+         : (ext == ".brwav" || ext == ".rwav") ? 9 : (ext == ".bcwav" || ext == ".cwav" || ext == ".bms") ? 10
+         : ext == ".bfwav" ? 11 : ext == ".bcstp" ? 12 : ext == ".bfstp" ? 13 : -1;
 }
+static_assert(VGB_CONTAINER_BRSTM == 4 && VGB_CONTAINER_HPS == 8 && VGB_CONTAINER_BRWAV == 9 && VGB_CONTAINER_BFSTP == 13,
+              "kinds 4..13 are their readers' container types");
 static const int32_t kContainerOfKind[3] = {VGB_CONTAINER_DSP, VGB_CONTAINER_HCA, VGB_CONTAINER_ADX};
 
 static int usage()
@@ -66,7 +73,8 @@ static int usage()
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian]\n"
-                         "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp and .hps inputs\n");
+                         "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
+                         "       .bfwav, .bcstp and .bfstp inputs\n");
     return 2;
 }
 
@@ -204,12 +212,12 @@ int main(int argc, char **argv)
         std::vector<int32_t> status(n);
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
         // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
-        // codec (one for the three NintendoWare streams, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
+        // codec (one for every NintendoWare reader, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
         // and one transcode call for the coded ones
         std::vector<int32_t> rows[6];
         for (int k = 0; k < n; k++) {
             const int kind = kind_of(files[first + k]);
-            rows[to_wave ? (kind >= 7 ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
+            rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
         }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
             for (int h = 0; h < 6; h++) {
@@ -223,7 +231,7 @@ int main(int argc, char **argv)
                     p.push_back(ptr[k]); l.push_back(len[k]); o.push_back(outs ? outs[k] : nullptr);
                     const int kind = kind_of(files[first + k]);
                     if (kind < 3) types.push_back(kContainerOfKind[kind]);
-                    else if (kind > 3) types.push_back(VGB_CONTAINER_BRSTM + (kind - 4));  // BRSTM .. BFSTM, IDSP, HPS
+                    else if (kind > 3) types.push_back(kind);  // BRSTM .. BFSTM, IDSP, HPS, BRWAV .. BFSTP
                 }
                 const int32_t m = (int32_t)r.size();
                 uint8_t *const *ot = outs ? o.data() : nullptr;

@@ -17,6 +17,9 @@ CONTAINER_DSP, CONTAINER_ADX, CONTAINER_HCA = 1, 2, 3
 CONTAINER_BRSTM, CONTAINER_BCSTM, CONTAINER_BFSTM = 4, 5, 6   # written by convert_wave_batch, read by convert_nw_to_wave_batch
 CONTAINER_IDSP, CONTAINER_HPS = 7, 8                          # GC-ADPCM only, written by convert_wave_batch,
 #                                                               read by convert_idsp_hps_to_wave_batch
+# NintendoWare wave files and prefetch streams, read only (nw_file_parse, convert_nw_to_wave_batch), named by the reader
+# the reference picks for the extension: .brwav/.rwav, .bcwav/.cwav/.bms, .bfwav, .bcstp, .bfstp
+CONTAINER_BRWAV, CONTAINER_BCWAV, CONTAINER_BFWAV, CONTAINER_BCSTP, CONTAINER_BFSTP = 9, 10, 11, 12, 13
 NW_CODEC_PCM8, NW_CODEC_PCM16, NW_CODEC_GCADPCM = 0, 1, 2        # NwCodec; convert_options(nw_codec_plus1=codec + 1)
 
 
@@ -317,9 +320,21 @@ def bcfstm_parse(file) -> N.VgbNwInfo:
     return info
 
 
+def nw_file_parse(file, in_type: int) -> Tuple[N.VgbNwInfo, List[int]]:
+    """Any NintendoWare reader on a file image (in_type: CONTAINER_BRSTM .. _BFSTM or CONTAINER_BRWAV .. _BFSTP):
+    (the structure, the absolute file offset of each wave channel's bytes - empty unless the file's channels are
+    separate runs); raises VgbError(VGB_E_DATA) where the reader fails, VgbError(VGB_E_ARG) for another in_type."""
+    f = _bytes_arr(file)
+    info = N.VgbNwInfo()
+    offsets = (C.c_int64 * N.VGB_NW_MAX_CHANNELS)()
+    N.check(N.lib.vgb_nw_file_parse(f.ctypes.data, f.size, in_type, C.byref(info), offsets))
+    return info, [int(v) for v in offsets[:max(info.channel_count, 0)] if v >= 0]
+
+
 def convert_nw_to_wave_batch(files: Sequence, in_types: Sequence[int]) -> Tuple[List[Optional[np.ndarray]], List[int]]:
-    """The decode direction of the batch job for .brstm / .bcstm / .bfstm images (in_types: CONTAINER_BRSTM, _BCSTM or
-    _BFSTM per file, naming the reader): ([WAVE bytes or None], [per-file status]); a file whose GC-ADPCM frames select a
+    """The decode direction of the batch job for NintendoWare images (in_types per file, naming the reader:
+    CONTAINER_BRSTM, _BCSTM, _BFSTM for streams, CONTAINER_BRWAV, _BCWAV, _BFWAV for wave files, CONTAINER_BCSTP,
+    _BFSTP for prefetch streams): ([WAVE bytes or None], [per-file status]); a file whose GC-ADPCM frames select a
     predictor outside 0..7 fails alone."""
     types = (C.c_int32 * max(len(in_types), 1))(*in_types)
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_nw_to_wave_batch(

@@ -91,12 +91,28 @@ void try_pin(const void *p, size_t bytes)
         (void)cudaGetLastError();  // stay pageable
 }
 
+// Whether every host-side address of the list is page-locked (vgb_host_alloc, cudaHostRegister, pinned framework
+// buffers).  With pageable caller memory, cudaMemcpyBatchAsync with stream-ordered source access faulted on the H100:
+// a group of 3571 NintendoWare wave images of 3-260 KB crashed the calling thread inside the call, or left the context
+// with an unspecified launch failure, with or without slack behind every image, before any kernel ran; one
+// cudaMemcpyAsync per region copied the same group clean.  Pageable regions therefore take the per-copy path.
+static bool host_side_locked(const std::vector<void *> &host)
+{
+    for (void *p : host) {
+        cudaPointerAttributes attr;
+        if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) { (void)cudaGetLastError(); return false; }
+        if (attr.type != cudaMemoryTypeHost) return false;
+    }
+    return true;
+}
+
 int32_t CopyList::run(cudaMemcpyKind kind, cudaStream_t st)
 {
     const size_t n = size.size();
     if (n == 0) return VGB_OK;
     static bool batch_ok = std::getenv("VGB_NO_MEMCPY_BATCH") == nullptr;
-    if (batch_ok && n >= 16) {
+    const bool locked = kind == cudaMemcpyHostToDevice ? host_side_locked(src) : kind == cudaMemcpyDeviceToHost ? host_side_locked(dst) : true;
+    if (batch_ok && n >= 16 && locked) {
         cudaMemcpyAttributes attr{};
         attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;  // sources stay valid until the call returns (we synchronise)
         attr.flags = 0;
