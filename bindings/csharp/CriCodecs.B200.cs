@@ -52,6 +52,9 @@ namespace VGAudio.Native
         public static extern int vgb_adx_encode_batch(short** pcm, int* nSamples, VgbAdxParams* parameters, int nChannels,
             short* historyOut, byte** adpcmOut, VgbProgress progress, IntPtr user);
 
+        // CriAdxCodec.Decode per channel.  VGB_E_DATA (InvalidDataException) names the lowest channel with a frame that
+        // yields a sample and selects a filter coefs[filterNum] cannot index: Fixed 4..7, Linear / Exponential 1..7
+        // (IndexOutOfRangeException in the reference).  vgb_adx_decode_dev_status applies the same rule.
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_adx_decode_batch(byte** adpcm, int* nBytes, int* sampleCount, VgbAdxParams* parameters,
             int nChannels, short** pcmOut);

@@ -344,7 +344,10 @@ int32_t vgb_adx_debug_encode_stats(uint64_t *out, int32_t n);
 
 /* CriAdxCodec.Decode(byte[] adpcm, int sampleCount, CriAdxParameters config) (CriAdxCodec.cs:9-54).
  * n_bytes[c] = length of adpcm[c]; pcm_out[c] receives sample_count[c] samples.
- * VGB_E_DATA: a Fixed-type frame selects a filter outside 0..3 (IndexOutOfRangeException at CriAdxCodec.Coefs, :186-191). */
+ * VGB_E_DATA for the lowest channel with a frame that yields a sample and whose filter number coefs[filterNum] cannot
+ * index (IndexOutOfRangeException, :12,26): a Fixed-type filter outside 0..3 (CriAdxCodec.Coefs, :186-191) or a Linear /
+ * Exponential filter other than 0 (a one-row table).  A frame that yields no sample (the head frame when sample_count
+ * <= padding % samples per frame) is not checked, as in the reference. */
 int32_t vgb_adx_decode_batch(const uint8_t *const *adpcm, const int32_t *n_bytes, const int32_t *sample_count,
                              const vgb_adx_params *params, int32_t n_channels, int16_t *const *pcm_out);
 
@@ -359,8 +362,8 @@ int32_t vgb_adx_decode_batch(const uint8_t *const *adpcm, const int32_t *n_bytes
  * that yields no sample (the head frame when sample_count <= padding % samples per frame) never indexes the coefficient
  * table, so its filter number is not checked, as in the reference.  The workspace (vgb_adx_decode_workspace_bytes from
  * the same sample counts and params) holds the channel table, per-channel status words and the splice bookkeeping:
- * vgb_adx_decode_dev_status synchronises the stream and returns VGB_E_DATA for the lowest channel whose Fixed-type
- * frame selects a filter 4..7, with vgb_adx_decode_batch's message. */
+ * vgb_adx_decode_dev_status synchronises the stream and returns VGB_E_DATA for the lowest channel whose frame selects a
+ * filter the reference cannot index (Fixed 4..7, other types 1..7), with vgb_adx_decode_batch's message for its kind. */
 uint64_t vgb_adx_decode_workspace_bytes(const int32_t *sample_count, const vgb_adx_params *params, int32_t n_channels);
 int32_t vgb_adx_decode_dev(const uint8_t *d_adpcm, const int64_t *adpcm_offset, const int32_t *n_bytes, const int32_t *sample_count,
                            const vgb_adx_params *params, int32_t n_channels, int16_t *d_pcm, const int64_t *pcm_offset,

@@ -332,3 +332,6 @@ def test_frame_that_yields_no_sample_never_checks_its_filter(vg, oracle):
     cfg = criadx.CriAdxParameters(48000, 500, 18, 4, 0, 20, 3)
     st, dev, _ = _decode_dev(vg, [row], [10], [cfg])
     assert st == 0 and np.array_equal(dev[0], np.zeros(10, np.int16))
+    # the control: one sample past the padding and the head frame yields, so its filter number faults
+    st, _, _ = _decode_dev(vg, [row], [21], [cfg])
+    assert st == vg._native.VGB_E_DATA and b"channel 0: a frame of type 3 selects a filter other than 0" in vg.lib.vgb_last_error()

@@ -75,6 +75,9 @@ def encode(pcm, config: CriAdxParameters) -> np.ndarray:
 
 
 def decode_batch(adpcm, sample_counts, configs) -> List[np.ndarray]:
+    """One CriAdxCodec.Decode per channel in a single call (vgb_adx_decode_batch); raises VgbError(VGB_E_DATA) naming the
+    lowest channel whose frame selects a filter the reference cannot index: a Fixed-type filter outside 0..3 or another
+    type's filter other than 0, in a frame that yields a sample."""
     chans = _channel_list(adpcm, _as_u8)
     n = len(chans)
     if isinstance(configs, CriAdxParameters):
@@ -103,7 +106,8 @@ def decode_dev(d_adpcm, adpcm_offset, n_bytes, sample_counts, configs, d_pcm, pc
     """CriAdxCodec.Decode for every channel on device buffers (vgb_adx_decode_dev, the time-parallel decoder): d_adpcm is
     a uint8 and d_pcm an int16 CUDA tensor (views at any element offset are fine); channel c reads n_bytes[c] bytes at
     adpcm_offset[c] and writes sample_counts[c] samples at pcm_offset[c].  Runs on `stream` (a torch.cuda.Stream, default
-    the current one) and waits for it; raises VgbError(VGB_E_DATA) for a Fixed-type frame with a filter outside 0..3.
+    the current one) and waits for it; raises VgbError(VGB_E_DATA) like decode_batch for a frame with a filter the
+    reference cannot index (Fixed 4..7, other types 1..7).
     `workspace` (a uint8 CUDA tensor of at least vgb_adx_decode_workspace_bytes) is allocated when None.  Returns the
     workspace: vgb_adx_debug_decode_stats reads the last decode's bookkeeping from it, so keep it while the tap is read."""
     import torch

@@ -317,7 +317,7 @@ static int32_t adx_decode_one(const uint8_t *const *adpcm, const int32_t *n_byte
     VGB_TRY(g_ctx.misc.reserve(o_status + 16 * (size_t)n_groups));
     const AdxChannel *d_tab = static_cast<const AdxChannel *>(g_ctx.misc.p);
     int32_t *d_status = reinterpret_cast<int32_t *>(static_cast<char *>(g_ctx.misc.p) + o_status);  // [group * 4]
-    std::vector<int32_t> bad(n_groups, INT_MAX);
+    std::vector<int32_t> bad(2 * (size_t)n_groups, INT_MAX);  // per group: lowest channel of a Fixed-type fault, of another type's
     auto h2d = [&](int g) -> int32_t {
         if (g == 0) {
             CUDA_TRY(cudaMemcpyAsync(g_ctx.misc.p, tab.data(), tab.size() * sizeof(AdxChannel), cudaMemcpyHostToDevice, g_ctx.s_in));
@@ -337,14 +337,21 @@ static int32_t adx_decode_one(const uint8_t *const *adpcm, const int32_t *n_byte
     };
     auto d2h = [&](int g) -> int32_t {
         VGB_TRY(copy_units(cudaMemcpyDeviceToHost, g_ctx.pcm.c(), out_off.data(), pcm_out, out_len.data(), bound[g], bound[g + 1] - bound[g], g_ctx.s_out));
-        CUDA_TRY(cudaMemcpyAsync(&bad[g], d_status + 4 * g, 4, cudaMemcpyDeviceToHost, g_ctx.s_out));
+        CUDA_TRY(cudaMemcpyAsync(&bad[2 * g], d_status + 4 * g, 8, cudaMemcpyDeviceToHost, g_ctx.s_out));
         return VGB_OK;
     };
     VGB_TRY(run_group_pipeline(n_groups, h2d, one_phase(kern), d2h, no_done));
-    // CriAdxCodec.Coefs[filterNum] (:186-191) has four rows: IndexOutOfRangeException in the reference
-    for (int g = 0; g < n_groups; g++)
-        if (bad[g] >= 0 && bad[g] < bound[g + 1] - bound[g])
-            return fail(VGB_E_DATA, "channel %d: a Fixed-type frame selects a filter outside 0..3", bound[g] + bad[g]);
+    // coefs[filterNum] (CriAdxCodec.cs:12,26): four rows for Fixed, one for the other types - IndexOutOfRangeException
+    for (int g = 0; g < n_groups; g++) {
+        const int n = bound[g + 1] - bound[g], fixed = bad[2 * g], other = bad[2 * g + 1];
+        const bool has_fixed = fixed >= 0 && fixed < n, has_other = other >= 0 && other < n;
+        if (has_fixed && (!has_other || fixed < other))
+            return fail(VGB_E_DATA, "channel %d: a Fixed-type frame selects a filter outside 0..3", bound[g] + fixed);
+        if (has_other) {
+            const int c = bound[g] + other;
+            return fail(VGB_E_DATA, "channel %d: a frame of type %d selects a filter other than 0", c, params[c].type);
+        }
+    }
     return VGB_OK;
 }
 
@@ -469,15 +476,23 @@ int32_t vgb_adx_decode_dev(const uint8_t *d_adpcm, const int64_t *adpcm_offset, 
 }
 
 /* Synchronises `cuda_stream` and maps the status words the last vgb_adx_decode_dev on this workspace left: the lowest
- * channel whose Fixed-type frame selects a filter 4..7 (IndexOutOfRangeException at CriAdxCodec.Coefs, :186-191). */
+ * channel with a frame whose filter number the reference's coefs[filterNum] cannot index (CriAdxCodec.cs:12,26:
+ * IndexOutOfRangeException for a Fixed-type filter 4..7 or another type's filter 1..7), with vgb_adx_decode_batch's
+ * message for its kind. */
 int32_t vgb_adx_decode_dev_status(const void *d_workspace, int32_t n_channels, void *cuda_stream)
 {
     if (n_channels <= 0) return VGB_OK;
     if (!d_workspace) return fail(VGB_E_ARG, "NULL argument");
     std::vector<int32_t> status(n_channels, 0);
     VGB_TRY(adx_decode_words(d_workspace, n_channels, status.data(), static_cast<cudaStream_t>(cuda_stream)));
-    for (int c = 0; c < n_channels; c++)
+    for (int c = 0; c < n_channels; c++) {
         if (status[c] & 1) return fail(VGB_E_DATA, "channel %d: a Fixed-type frame selects a filter outside 0..3", c);
+        if (status[c] & 2) {  // the channel's type from the table at the front of the workspace
+            AdxDecChannel t;
+            CUDA_TRY(cudaMemcpy(&t, static_cast<const AdxDecChannel *>(d_workspace) + c, sizeof t, cudaMemcpyDeviceToHost));
+            return fail(VGB_E_DATA, "channel %d: a frame of type %d selects a filter other than 0", c, t.type);
+        }
+    }
     return VGB_OK;
 }
 

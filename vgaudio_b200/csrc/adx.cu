@@ -359,6 +359,14 @@ adx_encode_kernel(const int16_t *__restrict__ pcm, const AdxChannel *__restrict_
     }
 }
 
+// The filter number of a frame header (:26) indexes CriAdxCodec.Coefs, four rows, for the Fixed type and a one-row table
+// of the computed pair for every other type: status bit 0 for a Fixed filter 4..7, bit 1 for another type's filter 1..7
+// (both IndexOutOfRangeException in the reference)
+__device__ __forceinline__ uint32_t adx_filter_fault(uint32_t b0, int type)
+{
+    return type == 2 ? (b0 >> 7) & 1u : ((b0 & 0xE0u) ? 2u : 0u);
+}
+
 __global__ void __launch_bounds__(kAdxThreads)
 adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restrict__ tab, int n_channels, int32_t *__restrict__ status,
                   int16_t *__restrict__ pcm)
@@ -374,7 +382,7 @@ adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restric
     const int frame_count = div_round_up(sample_count, spf);
     const bool v4 = c.version == 4;
     int32_t hist1 = c.history, hist2 = c.history;  // :16-17
-    uint32_t bad_filter = 0;                       // OR of the header bytes of Fixed-type frames
+    uint32_t bad_filter = 0;                       // adx_filter_fault of every frame that yields a sample
     int current = 0;
     int start_sample = c.padding > 0 ? c.padding % spf : 0;       // :21
     int64_t in = (int64_t)(c.padding / spf) * c.frame_size;      // :22
@@ -408,9 +416,9 @@ adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restric
                 auto byte_at = [&](int k) -> uint32_t { return (w[(base + k) >> 2] >> (((base + k) & 3) * 8)) & 0xFFu; };
                 const uint32_t b0 = byte_at(0), b1 = byte_at(1);
                 int32_t c0 = c.coef0, c1 = c.coef1;
+                bad_filter |= adx_filter_fault(b0, c.type);
                 if (c.type == 2) {
                     const int k = ((int)((b0 >> 4) & 0xF) >> 1) & 3;
-                    bad_filter |= b0;  // bit 7: filter number 4..7
                     c0 = k == 0 ? 0 : (k == 1 ? 0x0F00 : (k == 2 ? 0x1CC0 : 0x1880));
                     c1 = k == 0 ? 0 : (k == 1 ? 0 : (k == 2 ? (int16_t)0xF300 : (int16_t)0xF240));
                 }
@@ -465,9 +473,8 @@ adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restric
         const uint32_t b0 = src[in], b1 = src[in + 1];
         const int filter_num = (int)((b0 >> 4) & 0xF) >> 1;  // :26
         int32_t c0 = c.coef0, c1 = c.coef1;
-        if (c.type == 2) {  // CriAdxCodec.Coefs (:186-191); the reference throws for filter numbers 4..7
+        if (c.type == 2) {  // CriAdxCodec.Coefs (:186-191)
             const int k = filter_num & 3;
-            bad_filter |= b0;
             c0 = k == 0 ? 0 : (k == 1 ? 0x0F00 : (k == 2 ? 0x1CC0 : 0x1880));
             c1 = k == 0 ? 0 : (k == 1 ? 0 : (k == 2 ? (int16_t)0xF300 : (int16_t)0xF240));
         }
@@ -475,6 +482,7 @@ adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restric
         scale = (int16_t)(c.type == 4 ? (1 << ((12 - scale) & 31)) : scale + 1);      // :28 (C# masks the shift count)
         in += 2 + start_sample / 2;
         const int to_read = min(spf, sample_count - current);
+        if (to_read > start_sample) bad_filter |= adx_filter_fault(b0, c.type);  // coefs[filterNum] is indexed in the sample loop only
         for (int s = start_sample; s < to_read; s++) {
             const uint32_t byte = src[in];
             int32_t sample = (s & 1) == 0 ? ((int32_t)(byte << 24) >> 28) : ((int32_t)(byte << 28) >> 28);
@@ -488,8 +496,11 @@ adx_decode_kernel(const uint8_t *__restrict__ adpcm, const AdxChannel *__restric
         }
         start_sample = 0;
     }
-    // CriAdxCodec.Coefs[filterNum] (:186-191) has four rows: the reference throws IndexOutOfRangeException for 4..7
-    if ((bad_filter & 0x80u) && status) atomicMin(status, ch);
+    // IndexOutOfRangeException in the reference: status[0] is the lowest channel of a Fixed-type fault, status[1] of another type's
+    if (status) {
+        if (bad_filter & 1u) atomicMin(status, ch);
+        if (bad_filter & 2u) atomicMin(status + 1, ch);
+    }
     // `new short[sampleCount]` is zero-initialised: samples the padding logic never produces stay 0 (:14,:31-33)
     for (; current < sample_count; current++) dst[current] = 0;
 }
@@ -515,14 +526,6 @@ __device__ __forceinline__ void adx_fixed_coefs(uint32_t b0, int32_t &c0, int32_
     const int k = ((int)((b0 >> 4) & 0xF) >> 1) & 3;
     c0 = k == 0 ? 0 : (k == 1 ? 0x0F00 : (k == 2 ? 0x1CC0 : 0x1880));
     c1 = k == 0 ? 0 : (k == 1 ? 0 : (k == 2 ? (int16_t)0xF300 : (int16_t)0xF240));
-}
-
-// The filter number of a frame header (:26) indexes CriAdxCodec.Coefs, four rows, for the Fixed type and a one-row table
-// of the computed pair for every other type: status bit 0 for a Fixed filter 4..7, bit 1 for another type's filter 1..7
-// (both IndexOutOfRangeException in the reference)
-__device__ __forceinline__ uint32_t adx_filter_fault(uint32_t b0, int type)
-{
-    return type == 2 ? (b0 >> 7) & 1u : ((b0 & 0xE0u) ? 2u : 0u);
 }
 
 // One frame by the reference's loop (:24-51): header at byte fb of src, samples s in [start, to_read) to dst[0..).  A frame

@@ -55,7 +55,8 @@ int adx_encode_pick_segments(int n_channels, int max_whole_frames, int *min_seg_
 void launch_adx_encode(const int16_t *pcm, const AdxChannel *tab, int n_channels, uint8_t *adpcm, int16_t *history_out,
                        AdxSegArgs seg, cudaStream_t stream);  // seg.trace == nullptr: one segment (plain serial encode)
 void launch_adx_decode(const uint8_t *adpcm, const AdxChannel *tab, int n_channels, int16_t *pcm, int32_t *status,
-                       cudaStream_t stream);  // status: lowest channel with a fixed-filter number 4..7 (atomicMin), may be null
+                       cudaStream_t stream);  // status[0] / [1]: lowest channel whose Fixed-type / other-type frame selects a filter
+                                             // the reference cannot index (atomicMin), may be null
 // the time-parallel decode (chain / run-on / cascade); seg.status, seg.stats and the trace live in the caller's workspace
 int adx_decode_pick_segments(int n_channels, int max_body_frames, int *min_seg_out);
 void launch_adx_decode_seg(const uint8_t *adpcm, const AdxDecChannel *tab, int n_channels, int16_t *pcm, AdxDecSegArgs seg,
