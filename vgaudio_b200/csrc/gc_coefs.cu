@@ -280,26 +280,48 @@ __device__ __forceinline__ RefineSum gc_refine_consume(int lane, int n_blocks, i
     const int my_bucket = (lane >> 1) & 7, my_comp = lane & 1;
     double a = 0.0;
     int h = 0;
+    const bool active = lane < 16 && my_bucket < NB;
     refine_chunk_barrier<W>();  // chunk 0 classified
     for (int c = 1; c <= n_chunks; c++) {
         const int first = (c - 1) * P;
-        for (int j = 0; j < P && first + j < n_blocks; j++) {
-            const RefineSlot &slot = sh.slot[(c - 1) & 1][j];
-            const int n_mine = (lane < 16 && my_bucket < NB) ? slot.count[my_bucket] : 0;
-            const double *col = reinterpret_cast<const double *>(slot.q + (my_bucket < NB ? my_bucket : 0) * ROW) + my_comp;
-            // STEP queue entries per iteration (the producers pad every queue to a multiple of STEP with -0.0, the additive
-            // identity): loads issued together, then the bare DADD chain - the shared-memory latency and the loop overhead are
-            // paid once per STEP records, so the passes with one or two long queues (STEP 16 / 8) run close to the 8.3 cycles
-            // a dependent add costs.  The trip count differs per lane; lanes whose bucket is done simply drop out.
-            const int n_pad = (n_mine + STEP - 1) / STEP * STEP;
-            for (int j0 = 0; j0 < n_pad; j0 += STEP) {
-                double v[STEP];
+        const RefineSlot *slot = sh.slot[(c - 1) & 1];
+        const int off = (my_bucket < NB ? my_bucket : 0) * ROW * 2 + my_comp;  // the lane's column in a slot, in doubles
+        // The lane's entries of the whole chunk form one stream: block 0's queue padded to a multiple of STEP with -0.0
+        // (the additive identity; the producers write the padding), then block 1's, ...  All counts are read up front,
+        // and every group of STEP entries is loaded while the previous group is being added, so the shared-memory latency
+        // of the counts and of the entries sits on the DADD chain once per chunk (after the barrier) instead of once per
+        // block and per group.  The trip count differs per lane; lanes whose stream ends drop out.
+        int pre[P + 1];  // pre[j] = padded entries before block j
+        pre[0] = 0;
 #pragma unroll
-                for (int i = 0; i < STEP; i++) v[i] = col[2 * (j0 + i)];
+        for (int j = 0; j < P; j++) {
+            const int n = (active && first + j < n_blocks) ? slot[j].count[my_bucket] : 0;
+            h += n;
+            pre[j + 1] = pre[j] + (n + STEP - 1) / STEP * STEP;
+        }
+        auto group = [&](int t) {  // the first entry of the group at stream position t
+            const double *q = reinterpret_cast<const double *>(slot[0].q) + off + 2 * t;
 #pragma unroll
-                for (int i = 0; i < STEP; i++) a += v[i];
-            }
-            h += n_mine;
+            for (int j = 1; j < P; j++)
+                if (t >= pre[j]) q = reinterpret_cast<const double *>(slot[j].q) + off + 2 * (t - pre[j]);
+            return q;
+        };
+        const int total = pre[P];
+        double v[STEP];
+        {
+            const double *q = group(0);
+#pragma unroll
+            for (int i = 0; i < STEP; i++) v[i] = q[2 * i];
+        }
+        for (int t = 0; t < total; t += STEP) {
+            double nx[STEP];
+            const double *q = group(t + STEP < total ? t + STEP : t);  // the last group reloads itself (unused)
+#pragma unroll
+            for (int i = 0; i < STEP; i++) nx[i] = q[2 * i];
+#pragma unroll
+            for (int i = 0; i < STEP; i++) a += v[i];
+#pragma unroll
+            for (int i = 0; i < STEP; i++) v[i] = nx[i];
         }
         refine_chunk_barrier<W>();
     }
