@@ -36,6 +36,16 @@ namespace VGAudio.Native
     internal struct VgbAdxKey { public int Seed, Mult, Inc; }
 
     [StructLayout(LayoutKind.Sequential)]
+    internal struct VgbAdxFoundKey   // one key of vgb_adx_find_keys (GuessAdx.AddKey)
+    {
+        public VgbAdxKey Key;
+        public int Status;                     // Ok, or the confidence pass's error (confidences NaN)
+        public ulong KeyCode;                  // CriAdxKey.KeyCode
+        public long DiffShort, TotalShort, DiffFull, TotalFull;
+        public double ConfidenceShort, ConfidenceFull;
+    }
+
+    [StructLayout(LayoutKind.Sequential)]
     internal unsafe struct VgbAdxFileInfo   // AdxStructure (Containers/Adx/AdxStructure.cs) + where the audio sits
     {
         public int HeaderSize, Type, FrameSize, BitDepth, ChannelCount, SampleRate, SampleCount, HighpassFrequency;
@@ -140,6 +150,10 @@ namespace VGAudio.Native
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_adx_parse(byte* file, long length, VgbAdxFileInfo* info);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_adx_to_wave_batch(byte** files, long* lengths, int nFiles, VgbAdxKey* key, long* outSizes, byte** filesOut, int* statusOut);
+        // GuessAdx (VGAudio.Tools/CrackAdx/GuessAdx.cs) on the GPU: fileStatus may be null, revision may be null
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_adx_find_keys(byte** files, long* lengths, int nFiles, VgbAdxFoundKey* keysOut, int maxKeys, int* nKeysOut,
+            int* fileStatusOut, int* revisionOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_hca_to_wave_batch(byte** files, long* lengths, int nFiles, ulong* keyCode, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_brstm_parse(byte* file, long length, VgbNwInfo* info);
@@ -310,10 +324,34 @@ namespace VGAudio.Cli
             }
         }
 
+        // GuessAdx.Run over .adx files of one revision (the first file's; others are skipped): every key valid on every file,
+        // ascending by (seed, mult, inc), with AddKey's confidences.  More than maxKeys keys throw, with no partial list.
+        public static unsafe VgbAdxFoundKey[] FindAdxKeys(string[] inPaths, int maxKeys = 256)
+        {
+            int n = inPaths.Length;
+            byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
+            var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            try
+            {
+                byte** inPtr = stackalloc byte*[Math.Max(n, 1)];
+                long* len = stackalloc long[Math.Max(n, 1)];
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
+                var keys = new VgbAdxFoundKey[Math.Max(maxKeys, 1)];
+                int found = 0;
+                fixed (VgbAdxFoundKey* k = keys)
+                    VgAudioB200.Check(VgAudioB200Containers.vgb_adx_find_keys(inPtr, len, n, k, maxKeys, &found, null, null));
+                return keys.Take(found).ToArray();
+            }
+            finally
+            {
+                foreach (var h in inPins) h.Free();
+            }
+        }
+
         // The decode direction for a chunk of .adx files (`-b --out-format wav`): AdxReader -> ToPcm16 -> WaveWriter per file
         // in one native call per pass.  key (CriAdxKey from --keystring / --keycode, as vgb_adx_key_from_string / _code make it)
-        // decrypts files of revision 8 and 9; the native library carries no list of known keys, so a caller that wants
-        // CriAdxEncryption.FindKey's search runs it on the file and passes the key it finds.  A file whose frames select a
+        // decrypts files of revision 8 and 9; the native library carries no list of known keys, so a caller passes the key
+        // CriAdxEncryption.FindKey or FindAdxKeys (GuessAdx) finds.  A file whose frames select a
         // filter the reference cannot index fails in the second pass alone.
         public static unsafe void ConvertAdxToWave(string[] inPaths, string[] outPaths, VgbAdxKey? key, Action<string> log, Action<int> reportAdd)
         {

@@ -802,8 +802,8 @@ int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t
  * Keys (*key from vgb_adx_key_from_code / _from_string, or NULL): revision 8 or 9 is decrypted with *key, and fails with
  * "encrypted ADX file (type N) and no key" without one; any other revision is not decrypted.  Two differences on
  * purpose: AdxReader.EncryptionKey would also "decrypt" files of other revisions, but a directory mixes files, so the key
- * goes to types 8 and 9 only; and the reference's built-in key list (CriAdxEncryption.FindKey) is not carried - there is
- * no key search.  A sample rate <= 0 decodes as in the reference (CalculateCoefficients' double math; a rate of 0 gives
+ * goes to types 8 and 9 only; and the reference's built-in key list (CriAdxEncryption.FindKey) is not carried: a keyed
+ * file needs the caller's key, which vgb_adx_find_keys can recover from the files.  A sample rate <= 0 decodes as in the reference (CalculateCoefficients' double math; a rate of 0 gives
  * NaN, which C#'s (int) makes int.MinValue and (short) 0).  Per-file errors, each failing that file only: a parse error, a missing key, bad loop points, a negative
  * unaligned sample count, decoded frames past a channel's audio (IndexOutOfRangeException), 2 GiB of PCM or more, too many
  * channels for the WAVE join - all known in the sizing pass - and a Fixed-type frame with a filter 4..7, found on the
@@ -811,6 +811,78 @@ int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t
  * status_out NULL such a file fails the call (VGB_E_DATA) after every other file has been written. */
 int32_t vgb_convert_adx_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_adx_key *key,
                                       int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* The key search of VGAudio.Tools/CrackAdx/GuessAdx.cs: recovers the CriAdxKey (seed, mult, inc) of keyed .adx files
+ * (revisions 8 and 9) from the files alone, with no list of known keys.
+ *   - Loading (LoadFiles, GuessAdx.cs:79-97): each image's header as AdxReader.ReadMetadata reads it; the search's
+ *     revision is the first read file's (a file of revision 0 read before it sets nothing and is kept, as in the
+ *     reference), files of another revision are skipped.  A kept file's AudioDataLength bytes from HeaderSize + 4 are
+ *     read, bytes past the image as zero; Scales[i] is the big-endian u16 at i * FrameSize over the raw, interleaved
+ *     region (file order = key stream order), StartFrame the frame of the first non-zero byte (0 if none).
+ *   - Candidates (:48-71, TryScale :160-189): revision 8 takes the 0x400 primes above 0x4000 as seeds, multipliers and
+ *     increments, validation mask 0xE000, MaxSeed 0x8000; revision 9 seeds 0..0x1FFF, multipliers x & 3 == 1 and odd
+ *     increments below 0x2000, mask 0x1000, MaxSeed 0x2000.  For every scale index 0..0xFFF and every file:
+ *     seed = (Scales[StartFrame] ^ index) & (MaxSeed - 1) (skipped when StartFrame is 0 and the seed is not listed), and
+ *     every (mult, inc) walks the frames from StartFrame; a frame fails when ((scale ^ x) & mask) != 0 && scale != 0.
+ *   - A full match is wound back to frame 0 (FindStartingKey :191-215; revision 8 drops a seed that is not a listed
+ *     prime) and kept when KeyIsValid (:217-229) holds on every loaded file.  The keys are the union over every file's
+ *     scan, each distinct key once, sorted ascending by (seed, mult, inc) - the reference logs them in thread order.
+ *     Revision 9 only reads the low 13 bits of a key, so a file keyed with a 15-bit key (vgb_adx_key_from_code) is found
+ *     as its 13-bit equivalent, which decrypts it byte for byte the same.
+ *   - Confidence (AddKey :126-158, GetReencodeConfidence :231-263), per key and file: AdxReader with the key -> ToPcm16
+ *     -> CriAdxFormat.EncodeFromPcm16 with default CriAdxParameters (frame size 18, version 4, Linear, the loop-start
+ *     alignment of CriAdxFormat.cs:57-89), on the device through the .adx source stage of vgb_convert_adx_to_wave_batch
+ *     and the ADX target encode of vgb_convert_wave_batch.  Each channel's decrypted audio is compared with its
+ *     re-encode (Common.DiffArrays: bytes that DIFFER, -2 when the lengths differ) over n = channel 0's audio length
+ *     ("full") and min(FrameSize * 100, full) ("short"); totals add n per channel.  confidence = 1 - (double)sum of
+ *     differences / sum of totals over the files, short and full.
+ * keys_out receives *n_keys_out entries; key_code is CriAdxKey.KeyCode.  When more than max_keys keys are valid on every
+ * file the call fails (VGB_E_ARG) with nothing written to keys_out: no partial set, whatever the internal buffers hold.
+ * *n_keys_out is then the number of keys when the search ran to its end, or 0 when it stopped early (more than max_keys
+ * hits per scanned file already prove the set too large).  file_status_out[i] (may be NULL): VGB_OK for a file in the search,
+ * VGB_ADX_KEY_SKIPPED for a file of another revision, else the file's read error.  *revision_out (may be NULL): the
+ * search's revision.  With several devices bound (vgb_init_devices) the scale indices are split over them, and the
+ * keys' confidences are spread over them key by key.
+ * Revision 9 scans one file with a non-zero Scales[StartFrame] in place of every file: any key another file's scan finds
+ * is valid on that file, and that file's scan finds every such key (the bits the scale pins are the bits validation
+ * reads), so the set is the same.
+ * Differences on purpose, where the reference throws and ends the whole run:
+ *   - a file whose header cannot be read, or whose audio length or offset is invalid, gets that status and is left
+ *     out; the revision comes from the first file that is read;
+ *   - a first revision other than 8 or 9 (or no file read) fails the call with VGB_E_ARG (a NullReferenceException);
+ *   - a file with no whole frame adds no candidates and validates every key (IndexOutOfRangeException at
+ *     Scales[StartFrame]);
+ *   - a key for which a file's re-read or re-encode throws gets that error as its status and NaN confidences; so does a
+ *     sum past int.MaxValue (LINQ's checked Sum, VGB_E_DATA). */
+#define VGB_ADX_KEY_SKIPPED 1
+typedef struct vgb_adx_found_key {
+    vgb_adx_key key;
+    int32_t status;                        /* VGB_OK, or the error of the confidence pass (confidences NaN) */
+    uint64_t key_code;                     /* CriAdxKey.KeyCode */
+    int64_t diff_short, total_short;       /* sums over the files: differing bytes (IdenticalBytesShort) and compared bytes */
+    int64_t diff_full, total_full;
+    double confidence_short, confidence_full;
+} vgb_adx_found_key;
+int32_t vgb_adx_find_keys(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, vgb_adx_found_key *keys_out,
+                          int32_t max_keys, int32_t *n_keys_out, int32_t *file_status_out, int32_t *revision_out);
+/* vgb_adx_find_keys over a box of the search: scale indices [index_first, index_end) of 0..0x1000, multipliers
+ * [mult_first, mult_end) and increments [inc_first, inc_end) of the revision's lists (indices into them).  Every file is
+ * scanned, as in the reference, unless flags holds VGB_ADX_KEYS_ONE_FILE: then revision 9 over every scale index scans
+ * one file as vgb_adx_find_keys does.  Out-of-range boxes are VGB_E_ARG (after the files are read). */
+#define VGB_ADX_KEYS_ONE_FILE 1
+int32_t vgb_adx_debug_find_keys_box(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, int32_t index_first,
+                                    int32_t index_end, int32_t mult_first, int32_t mult_end, int32_t inc_first, int32_t inc_end,
+                                    int32_t flags, vgb_adx_found_key *keys_out, int32_t max_keys, int32_t *n_keys_out,
+                                    int32_t *file_status_out, int32_t *revision_out);
+/* LoadFiles' body for one image, host only: *revision_inout is the search's revision so far (0 before the first file;
+ * set from this file's header while it is 0).  Returns VGB_OK with the file's Scales (the first scales_cap of them),
+ * their number and StartFrame; VGB_ADX_KEY_SKIPPED for another revision; or the read error. */
+int32_t vgb_adx_key_load(const uint8_t *file, int64_t length, int32_t *revision_inout, uint16_t *scales_out, int32_t scales_cap,
+                         int32_t *n_frames_out, int32_t *start_frame_out);
+/* The counts of the most recent search (any thread, every device): out[0] candidates tried ((seed, mult, inc) triples
+ * walked), [1] frame steps (frames tested, the failing one included), [2] full matches (candidates that walked every
+ * frame, before FindStartingKey), [3] device time of the search kernels in microseconds (CUDA events around each
+ * device's launches, summed over the devices). */
+int32_t vgb_adx_debug_key_search_stats(uint64_t *out, int32_t n);
 /* The decode direction of the batch job for NintendoWare files: .brstm, .bcstm and .bfstm streams, .brwav, .bcwav and
  * .bfwav wave files and .bcstp / .bfstp prefetch streams in, 16-bit WAVE images out - BrstmReader / BrwavReader /
  * BCFstmReader (vgb_nw_file_parse) -> Common.ToAudioStream (Containers/NintendoWare/Common.cs:45-116) -> ToPcm16 ->
@@ -873,7 +945,7 @@ int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n);
  * the PCM, loop points and rate their ToPcm16 yields (.adx: sample_count - inserted_samples samples, loop points shifted;
  * .hca: trimmed at the loop end; .dsp: from the header's start history), and their keys: *in_adx_key decrypts revision 8
  * and 9 .adx files, *in_hca_key_code "ciph" 56 .hca files, "ciph" 1 uses the built-in table; a keyed source without its
- * key fails alone, keys are never applied to other revisions and there is no key search.  No PCM leaves the device:
+ * key fails alone, keys are never applied to other revisions (vgb_adx_find_keys recovers a key from the files).  No PCM leaves the device:
  * per batch one H2D of the coded regions, the source's decode straight into the encoder's channel rows, encode and file
  * assembly, one D2H of the finished files.  Same two-pass protocol, per-file status, progress and sharding (files weigh
  * sample_count * channel_count + 1024) as vgb_convert_wave_batch.

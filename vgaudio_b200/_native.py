@@ -104,6 +104,16 @@ class VgbAdxKey(C.Structure):
     _fields_ = [("seed", C.c_int32), ("mult", C.c_int32), ("inc", C.c_int32)]
 
 
+class VgbAdxFoundKey(C.Structure):
+    """One key of vgb_adx_find_keys: the key, its confidence pass's status, CriAdxKey.KeyCode, the summed byte counts
+    (differing and compared, short and full) and the two confidences."""
+    _fields_ = [("key", VgbAdxKey), ("status", C.c_int32), ("key_code", C.c_uint64), ("diff_short", C.c_int64),
+                ("total_short", C.c_int64), ("diff_full", C.c_int64), ("total_full", C.c_int64),
+                ("confidence_short", C.c_double), ("confidence_full", C.c_double)]
+
+
+VGB_ADX_KEY_SKIPPED = 1
+VGB_ADX_KEYS_ONE_FILE = 1
 VGB_ADX_MAX_CHANNELS = 255
 
 
@@ -275,6 +285,11 @@ SIGNATURES = {
     "vgb_adx_write_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_adx_crypt_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32]),
     "vgb_adx_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p]),
+    "vgb_adx_find_keys": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_adx_debug_find_keys_box": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32] + [C.c_int32] * 7 +
+                                    [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "vgb_adx_debug_key_search_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
+    "vgb_adx_key_load": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "vgb_hca_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "vgb_hca_key_tables": (C.c_int32, [C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
     "vgb_hca_crypt_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int32]),

@@ -18,7 +18,11 @@
 // --keycode / --keystring are the output's key; --in-keycode N is the key of type-56 .hca inputs, and --in-keystring S,
 // or else --in-keycode N, the CriAdxKey of type-8 / type-9 .adx inputs.
 // With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
-// --keycode N, the CriAdxKey of type-8 / type-9 .adx files; there is no list of known keys.
+// --keycode N, the CriAdxKey of type-8 / type-9 .adx files.  There is no list of known keys; instead
+// --find-adx-key, when no key option names the .adx inputs' key (--keystring / --keycode with wav, --in-keystring /
+// --in-keycode otherwise), recovers it from the files first (vgb_adx_find_keys, GuessAdx): for each of revisions 8 and 9,
+// over that revision's .adx inputs, every key is printed as GuessAdx prints it and the files are decoded with the one of
+// highest full confidence (then short confidence, then the lowest key).  Without a key found they fail as without a key.
 // --devices 0,1,2,3 binds those CUDA devices (vgb_init_devices): every chunk of files is then sharded over them, one
 // worker and one copy / kernel pipeline per device.  A device may be listed more than once.  The default is device 0.
 #include <sys/stat.h>
@@ -72,7 +76,7 @@ static int usage()
     std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
-                         "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian]\n"
+                         "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key]\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
                          "       .bfwav, .bcstp and .bfstp inputs\n");
     return 2;
@@ -94,10 +98,51 @@ static bool parse_devices(const std::string &list, std::vector<int32_t> &out)
     return out.size() <= 64;  // vgb_init_devices' limit
 }
 
+// the revision of an .adx image (0 when its header cannot be read)
+static int adx_revision(const std::vector<uint8_t> &img)
+{
+    int32_t rev = 0, n = 0, start = 0;
+    return vgb_adx_key_load(img.data(), (int64_t)img.size(), &rev, nullptr, 0, &n, &start) == VGB_OK ? rev : 0;
+}
+
+// GuessAdx over the .adx inputs of one revision: prints every key as AddKey does (GuessAdx.cs:146-155) and picks the
+// one of highest full confidence, then short confidence, then the lowest (the keys come sorted)
+static bool find_adx_key(const std::vector<fs::path> &paths, int revision, vgb_adx_key &out)
+{
+    std::vector<std::vector<uint8_t>> imgs;
+    for (const fs::path &p : paths) {
+        std::vector<uint8_t> img;
+        if (read_file(p, img) && adx_revision(img) == revision) imgs.push_back(std::move(img));
+    }
+    if (imgs.empty()) return false;
+    std::vector<const uint8_t *> ptr;
+    std::vector<int64_t> len;
+    for (const auto &img : imgs) { ptr.push_back(img.data()); len.push_back((int64_t)img.size()); }
+    std::vector<vgb_adx_found_key> keys(256);
+    int32_t n = 0;
+    if (vgb_adx_find_keys(ptr.data(), len.data(), (int32_t)imgs.size(), keys.data(), (int32_t)keys.size(), &n, nullptr, nullptr) != VGB_OK) {
+        std::fprintf(stderr, "ADX key search (revision %d): %s\n", revision, vgb_last_error());
+        return false;
+    }
+    const vgb_adx_found_key *best = nullptr;
+    for (int i = 0; i < n; i++) {
+        const vgb_adx_found_key &k = keys[(size_t)i];
+        std::printf("----------------------------------------\nSeed - %04x Multiplier - %04x Increment - %04x\n", k.key.seed, k.key.mult, k.key.inc);
+        std::printf("Confidence Short - %.3f %% Full - %.3f %%\n", 100.0 * k.confidence_short, 100.0 * k.confidence_full);
+        if (revision == 9) std::printf("Key code: %llu\n", (unsigned long long)k.key_code);
+        std::printf("----------------------------------------\n");
+        if (k.status != VGB_OK) continue;
+        if (!best || k.confidence_full > best->confidence_full ||
+            (k.confidence_full == best->confidence_full && k.confidence_short > best->confidence_short)) best = &k;
+    }
+    if (best) out = best->key;
+    return best != nullptr;
+}
+
 int main(int argc, char **argv)
 {
     std::string in_dir, out_dir, fmt, key_string, in_key_string;
-    bool recurse = false, have_code = false, have_in_code = false;
+    bool recurse = false, have_code = false, have_in_code = false, find_key = false;
     uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
     std::vector<int32_t> devices;  // empty: device 0 through vgb_init
@@ -122,6 +167,7 @@ int main(int argc, char **argv)
         else if (a == "--chunk-mb") chunk_mb = (size_t)std::atoll(next());
         else if (a == "--devices") { if (!parse_devices(next(), devices)) return usage(); }
         else if (a == "--loop-align") opt.nw_loop_point_alignment = std::atoi(next());
+        else if (a == "--find-adx-key") find_key = true;
         else if (a == "--little-endian") opt.nw_endianness = 1;
         else if (a == "--big-endian") opt.nw_endianness = 2;
         else if (a == "-f") {  // NwCodec + 1
@@ -193,6 +239,16 @@ int main(int argc, char **argv)
     const int32_t bound = devices.empty() ? vgb_init(0, 0) : vgb_init_devices(devices.data(), (int32_t)devices.size(), 0);
     if (bound != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
 
+    // --find-adx-key: the keys of the keyed .adx inputs, per revision, when no key option gives them
+    const bool adx_key_given = to_wave ? have_adx_key : have_in_adx_key;
+    vgb_adx_key found[2]{};
+    bool have_found[2] = {false, false};
+    if (find_key && !adx_key_given && (to_wave || opt.out_type != VGB_CONTAINER_ADX)) {
+        std::vector<fs::path> adx;
+        for (const fs::path &p : files) if (kind_of(p) == 2) adx.push_back(p);
+        for (int r = 0; r < 2; r++) have_found[r] = find_adx_key(adx, 8 + r, found[r]);
+    }
+
     const auto t0 = std::chrono::steady_clock::now();
     size_t done = 0, failed = 0;
     uint64_t bytes_in = 0, bytes_out = 0;
@@ -214,13 +270,16 @@ int main(int argc, char **argv)
         // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
         // codec (one for every NintendoWare reader, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
         // and one transcode call for the coded ones
-        std::vector<int32_t> rows[6];
+        // rows 6 and 7: .adx files of revision 8 / 9 whose key --find-adx-key found, each revision with its own key
+        std::vector<int32_t> rows[8];
         for (int k = 0; k < n; k++) {
             const int kind = kind_of(files[first + k]);
-            rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
+            const int rev = kind == 2 && (have_found[0] || have_found[1]) ? adx_revision(in[k]) : 0;
+            if ((rev == 8 || rev == 9) && have_found[rev - 8]) rows[rev - 2].push_back(k);
+            else rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
         }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
-            for (int h = 0; h < 6; h++) {
+            for (int h = 0; h < 8; h++) {
                 const std::vector<int32_t> &r = rows[h];
                 if (r.empty()) continue;
                 std::vector<const uint8_t *> p;
@@ -236,12 +295,14 @@ int main(int argc, char **argv)
                 const int32_t m = (int32_t)r.size();
                 uint8_t *const *ot = outs ? o.data() : nullptr;
                 int32_t s;
+                const vgb_adx_key *wave_adx_key = h >= 6 ? &found[h - 6] : have_adx_key ? &adx_key : nullptr;
+                const vgb_adx_key *tx_adx_key = h >= 6 ? &found[h - 6] : have_in_adx_key ? &in_adx_key : nullptr;
                 if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
-                else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, have_in_adx_key ? &in_adx_key : nullptr,
+                else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key,
                                                            have_in_code ? &in_key_code : nullptr, sz.data(), ot, st.data(), nullptr, nullptr);
                 else if (h == 4) s = vgb_convert_nw_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
                 else if (h == 5) s = vgb_convert_idsp_hps_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
-                else s = h == 2 ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, have_adx_key ? &adx_key : nullptr, sz.data(), ot, st.data())
+                else s = (h == 2 || h >= 6) ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, wave_adx_key, sz.data(), ot, st.data())
                        : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
                                 : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());
                 if (s != VGB_OK) return s;

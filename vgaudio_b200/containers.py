@@ -304,6 +304,57 @@ def convert_adx_to_wave_batch(files: Sequence, key: Optional[N.VgbAdxKey] = None
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
 
 
+@dataclass
+class AdxKeySearch:
+    """What adx_find_keys returns: the search's revision, per-file status (0 in the search, N.VGB_ADX_KEY_SKIPPED for
+    another revision, else the read error) and the keys (N.VgbAdxFoundKey, ascending by seed, mult, inc)."""
+    revision: int
+    file_status: List[int]
+    keys: List[N.VgbAdxFoundKey]
+
+
+def adx_find_keys(files: Sequence, max_keys: int = 256, box: Optional[Tuple[int, int, int, int, int, int]] = None,
+                  flags: int = 0) -> AdxKeySearch:
+    """GuessAdx on the GPU: the CriAdxKey of keyed .adx images (revision 8 / 9) from the files alone, each key with its
+    re-encode confidence.  box = (index_first, index_end, mult_first, mult_end, inc_first, inc_end) restricts the search
+    (vgb_adx_debug_find_keys_box, every file scanned unless flags = N.VGB_ADX_KEYS_ONE_FILE).  Raises VgbError when
+    more than max_keys keys are valid on every file."""
+    arrs = [_bytes_arr(f) for f in files]
+    n = len(arrs)
+    ftab = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in arrs])
+    lens = (C.c_int64 * max(n, 1))(*[a.size for a in arrs])
+    keys = (N.VgbAdxFoundKey * max(max_keys, 1))()
+    n_keys, revision = C.c_int32(0), C.c_int32(0)
+    status = (C.c_int32 * max(n, 1))()
+    if box is None:
+        N.check(N.lib.vgb_adx_find_keys(ftab, lens, n, keys, max_keys, C.byref(n_keys), status, C.byref(revision)))
+    else:
+        N.check(N.lib.vgb_adx_debug_find_keys_box(ftab, lens, n, *box, flags, keys, max_keys, C.byref(n_keys), status, C.byref(revision)))
+    return AdxKeySearch(revision.value, [int(status[i]) for i in range(n)], [keys[i] for i in range(n_keys.value)])
+
+
+def adx_key_load(file, revision: int = 0) -> Tuple[int, int, Optional[np.ndarray], int]:
+    """The key search's view of one image, host only: (status, revision so far, Scales or None, StartFrame); status 0
+    loaded, N.VGB_ADX_KEY_SKIPPED for another revision, else the read error (no exception)."""
+    f = _bytes_arr(file)
+    rev, n, start = C.c_int32(revision), C.c_int32(0), C.c_int32(0)
+    st = N.lib.vgb_adx_key_load(f.ctypes.data, f.size, C.byref(rev), None, 0, C.byref(n), C.byref(start))
+    if st != 0:
+        return st, rev.value, None, start.value
+    scales = np.zeros(max(n.value, 1), dtype=np.uint16)
+    rev = C.c_int32(revision)
+    st = N.lib.vgb_adx_key_load(f.ctypes.data, f.size, C.byref(rev), scales.ctypes.data, scales.size, C.byref(n), C.byref(start))
+    return st, rev.value, scales[:n.value], start.value
+
+
+def adx_key_search_stats(with_time: bool = False) -> tuple:
+    """(candidates tried, frame steps, full matches) of the most recent key search, and with with_time the device time of
+    its search kernels in microseconds."""
+    out = (C.c_uint64 * 4)()
+    N.check(N.lib.vgb_adx_debug_key_search_stats(out, 4))
+    return tuple(int(v) for v in out[:4 if with_time else 3])
+
+
 def brstm_parse(file) -> N.VgbNwInfo:
     """BrstmReader.ReadFile on a file image, reduced to what decoding needs; raises VgbError(VGB_E_DATA)."""
     f = _bytes_arr(file)

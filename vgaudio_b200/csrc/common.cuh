@@ -225,4 +225,27 @@ struct HcaTables {
     const int8_t (*dequantize_value)[16]; // [8][16] QuantizedSpectrumValue
 };
 
+// CriAdxKey's LCG (CriAdxEncryption.cs:23,38): x -> (x * mult + inc) & 0x7fff applied `steps` times is one affine map
+// x -> (a * x + b) & 0x7fff, found by repeated squaring
+__device__ __forceinline__ void adx_key_jump(int mult, int inc, uint32_t steps, uint32_t &a, uint32_t &b)
+{
+    uint32_t pa = (uint32_t)mult & 0x7fffu, pb = (uint32_t)inc & 0x7fffu;
+    a = 1;
+    b = 0;
+    while (steps) {
+        if (steps & 1u) { a = (pa * a) & 0x7fffu; b = (pa * b + pb) & 0x7fffu; }
+        pb = (pa * pb + pb) & 0x7fffu;
+        pa = (pa * pa) & 0x7fffu;
+        steps >>= 1;
+    }
+}
+
+// the key stream's value `steps` steps after the seed
+__device__ __forceinline__ int adx_key_at(int seed, int mult, int inc, uint32_t steps)
+{
+    uint32_t a, b;
+    adx_key_jump(mult, inc, steps, a, b);
+    return (int)((a * ((uint32_t)seed & 0x7fffu) + b) & 0x7fffu);
+}
+
 }  // namespace vgb

@@ -12,6 +12,7 @@
 // All of it is HBM-bound byte work (every payload byte read once, written once); headers are a few dozen bytes per file
 // and are built on the host, except the fields that only exist on the device (DSP: coefficients, first predictor/scale
 // byte, loop context), which the assemble kernel patches in.  Citations are relative to VGAudio's src/VGAudio/.
+#include <array>
 #include <chrono>
 #include <cmath>
 #include <cstdarg>
@@ -327,19 +328,6 @@ __global__ void __launch_bounds__(256) dsp_assemble_kernel(const DspFile *__rest
 // interleave frames: thread = (frame, channel), frame_size bytes each, with CriAdxEncryption.EncryptDecryptChannel
 // applied on the way (the key stream position of frame j of channel c is c + j * channels steps of the LCG).
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int adx_key_at(int seed, int mult, int inc, uint32_t steps)
-{
-    // x -> (x * mult + inc) & 0x7fff applied `steps` times = one affine map mod 2^15, by repeated squaring
-    uint32_t a = 1, b = 0, pa = (uint32_t)mult & 0x7fffu, pb = (uint32_t)inc & 0x7fffu;
-    while (steps) {
-        if (steps & 1u) { a = (pa * a) & 0x7fffu; b = (pa * b + pb) & 0x7fffu; }
-        pb = (pa * pb + pb) & 0x7fffu;
-        pa = (pa * pa) & 0x7fffu;
-        steps >>= 1;
-    }
-    return (int)((a * ((uint32_t)seed & 0x7fffu) + b) & 0x7fffu);
-}
-
 constexpr int kAdxFramesPerTile = 1024;
 
 __global__ void __launch_bounds__(256) adx_assemble_kernel(const AdxFile *__restrict__ files, int n_files, const AdxChanRef *__restrict__ chans,

@@ -97,4 +97,39 @@ constexpr int kHpsGatherTile = 8192;
 __global__ void __launch_bounds__(256) hps_gather_kernel(const uint8_t *__restrict__ in, const HpsPiece *__restrict__ pieces, int n_pieces,
                                                           uint8_t *__restrict__ rows);
 
+// adx_keys.cu — the key search of VGAudio.Tools/CrackAdx/GuessAdx.cs (TryScale :160-189, FindStartingKey :191-215,
+// KeyIsValid :217-229) and the byte comparison of its re-encode confidence (Common.DiffArrays).
+// A file's frames as the search reads them: frame i's scale s becomes one word (s & mask) | (s ? mask : 0) << 16, so
+// that a key stream value x fails the frame exactly when ((x ^ w) & (w >> 16)) != 0.
+struct AdxKeyFileDev {
+    int64_t word_off;     // its words in the search's word array, frame 0 first
+    int32_t frames;       // Scales.Length
+    int32_t start;        // StartFrame
+    int32_t first_scale;  // Scales[StartFrame]
+    int32_t pad;
+};
+struct AdxKeyHit { int32_t seed, mult, inc; };
+struct AdxKeySearch {
+    const uint32_t *words;
+    const AdxKeyFileDev *files;   // every file of the search: a key is kept only when it is valid on all of them
+    int32_t n_files, file;        // file: the one whose TryScale this launch runs
+    const int32_t *mults, *incs;  // the multiplier and increment lists of the box
+    int32_t n_mult, n_inc;
+    int32_t index0, n_index;      // scale indices index0 .. index0 + n_index - 1
+    uint32_t seed_mask;           // MaxSeed - 1
+    int32_t check_seed;           // revision 8: a seed must be in seed_bits (the prime list), for StartFrame 0 and FindStartingKey
+    const uint32_t *seed_bits;    // 0x8000 bits
+    unsigned long long *tried;    // kAdxKeyTried slots, zeroed: the keys already validated
+    AdxKeyHit *hits;              // keys valid on every file, in no order, duplicates possible
+    unsigned long long *n_hits;   // all of them are counted; only the first cap are stored
+    uint32_t cap;
+    unsigned long long *stats;    // [0] candidates tried, [1] frame steps, [2] full matches
+};
+constexpr int kAdxKeyTried = 1 << 16;
+constexpr int kAdxKeyStage = 12288;  // words of the scanned file staged in shared memory (48 KiB)
+cudaError_t launch_adx_key_search(const AdxKeySearch &a, int frames_after_start, cudaStream_t stream);
+// out[2r] / out[2r+1]: the bytes of rows a + a_off[r] and b + b_off[r] that differ among their first n[2r] / n[2r+1]
+cudaError_t launch_adx_byte_diff(const uint8_t *a, const int64_t *a_off, const uint8_t *b, const int64_t *b_off, const int32_t *n,
+                                 int n_rows, int32_t *out, cudaStream_t stream);
+
 }  // namespace vgb
