@@ -154,6 +154,11 @@ namespace VGAudio.Native
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_adx_find_keys(byte** files, long* lengths, int nFiles, VgbAdxFoundKey* keysOut, int maxKeys, int* nKeysOut,
             int* fileStatusOut, int* revisionOut);
+        // HcaReader.FindKey over a caller's list of type-56 key codes: per file the first index and VgAudioB200.Ok, or -1 and
+        // VGB_E_DATA (a bad sync word), HcaKeySkipped, HcaKeyNotFound or the read error
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_hca_find_keys(byte** files, long* lengths, int nFiles, ulong* keyCodes, int nKeys, int* keyIndexOut, int* fileStatusOut);
+        public const int HcaKeySkipped = 1, HcaKeyNotFound = 2;
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_hca_to_wave_batch(byte** files, long* lengths, int nFiles, ulong* keyCode, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_brstm_parse(byte* file, long length, VgbNwInfo* info);
@@ -276,9 +281,10 @@ namespace VGAudio.Cli
         }
 
         // The decode direction for a chunk of .hca files (`-b --out-format wav`): HcaReader -> ToPcm16 -> WaveWriter per file
-        // in one native call per pass.  keyCode is the type-56 key (CriHcaKey(ulong)); the native library carries no list of
-        // known keys, so a caller that wants HcaReader.FindKey's search runs CriHcaEncryption.FindKey on the file and passes
-        // the code it finds.  A file whose frames the decoder refuses (a wrong key, a bad frame) fails in the second pass alone.
+        // in one native call per pass.  keyCode is the type-56 key (CriHcaKey(ulong)), used untested as HcaReader's
+        // EncryptionKey is; the native library carries no list of known keys, so a caller with a list of codes runs
+        // FindHcaKeys (HcaReader.FindKey on the GPU) first and converts each key's files with it.  A file whose frames the
+        // decoder refuses (a wrong key, a bad frame) fails in the second pass alone.
         public static unsafe void ConvertHcaToWave(string[] inPaths, string[] outPaths, ulong? keyCode, Action<string> log, Action<int> reportAdd)
         {
             int n = inPaths.Length;
@@ -321,6 +327,32 @@ namespace VGAudio.Cli
             {
                 foreach (var h in inPins) h.Free();
                 foreach (var h in outPins) h.Free();
+            }
+        }
+
+        // HcaReader.FindKey over the keys in list order for each file: (index of the first key that decrypts it or -1, status:
+        // VgAudioB200.Ok, VGB_E_DATA for a bad sync word in the test window, HcaKeySkipped when "ciph" is not 56,
+        // HcaKeyNotFound, or the file's read error)
+        public static unsafe (int[] Index, int[] Status) FindHcaKeys(byte[][] files, ulong[] keys)
+        {
+            int n = files.Length;
+            var pins = files.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            try
+            {
+                byte** inPtr = stackalloc byte*[Math.Max(n, 1)];
+                long* len = stackalloc long[Math.Max(n, 1)];
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)pins[i].AddrOfPinnedObject(); len[i] = files[i].Length; }
+                var index = new int[Math.Max(n, 1)];
+                var status = new int[Math.Max(n, 1)];
+                fixed (ulong* k = keys.Length > 0 ? keys : new ulong[1])
+                fixed (int* ix = index)
+                fixed (int* st = status)
+                    VgAudioB200.Check(VgAudioB200Containers.vgb_hca_find_keys(inPtr, len, n, k, keys.Length, ix, st));
+                return (index.Take(n).ToArray(), status.Take(n).ToArray());
+            }
+            finally
+            {
+                foreach (var h in pins) h.Free();
             }
         }
 

@@ -779,7 +779,8 @@ int32_t vgb_convert_dsp_to_wave_batch(const uint8_t *const *files, const int64_t
  * two-pass protocol and sharding (files weigh frame_count * channel_count).  Decryption follows HcaReader.FindKey
  * (:238-252): "ciph" 1 uses the built-in type-1 table, 56 the table of *key_code, any other value none.  The reference's
  * list of known keys is not carried: a type-56 file without key_code fails with "Cannot find key to decrypt HCA file.",
- * and the given code is not tested against the frames.  Per file, on the device: the frames are copied in, decrypted in
+ * and the given code is not tested against the frames (HcaReader's EncryptionKey ?? FindKey: a given key wins untested).
+ * vgb_hca_find_keys runs FindKey over a caller's list of codes; convert each found key's files with it.  Per file, on the device: the frames are copied in, decrypted in
  * place, decoded (vgb_hca_decode_dev, one launch per group of files that share a codec configuration) and joined behind
  * the WAVE header (smpl when looping, extensible fmt above two channels).
  * Per-file errors, each failing that file only (Batch.cs:39-43): a parse error, more than 8 channels or a layout the
@@ -791,6 +792,41 @@ int32_t vgb_convert_dsp_to_wave_batch(const uint8_t *const *files, const int64_t
  * (VGB_E_DATA) after every other file has been written. */
 int32_t vgb_convert_hca_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files,
                                       const uint64_t *key_code, int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* HcaReader.FindKey for type-56 files (Containers/Hca/HcaReader.cs:32, 238-252) over the caller's key codes in list
+ * order: CriHcaEncryption.FindKey / TestKey (Codecs/CriHca/CriHcaEncryption.cs:34-87).  For each file whose "ciph" is
+ * 56: the window is the first frame whose encrypted bytes [2, FrameSize - 2) are not all zero (frame 0 if none) and up to
+ * nine frames after it; a key passes when every window frame, decrypted by CryptFrame (table substitution of bytes
+ * [0, FrameSize - 2), then their CRC-16 in the last two bytes), unpacks with UnpackingWasSuccessful true
+ * (CriHcaPacking.cs:10-229: 16 <= Remaining <= 128, or FrameEmpty, or noise level 0 and Remaining >= 16).  Codes go
+ * through CriHcaKey(ulong) (vgb_hca_key_tables), which reads bytes 0..6 of code - 1, so codes equal there are one key;
+ * duplicates are legal and the first one wins.  Runs on the device, one file per CTA and one key per lane.
+ * key_index_out[i] / file_status_out[i]:
+ *   - VGB_OK and the index of the first code FindKey accepts;
+ *   - VGB_E_DATA, -1: the first key that passes the window frames before frame j reaches a bad sync word there (an
+ *     InvalidDataException("Invalid frame header") out of FindKey: every type-56 table keeps 0x00 and 0xFF, so the sync
+ *     word decrypts to 0xFFFF exactly when the raw one is 0xFFFF);
+ *   - VGB_HCA_KEY_SKIPPED, -1: "ciph" is not 56 (not searched);
+ *   - VGB_HCA_KEY_NOT_FOUND, -1: no listed key passes ("Cannot find key to decrypt HCA file."), every type-56 file when
+ *     n_keys is 0;
+ *   - the error, -1: vgb_hca_parse refuses the file, or its channel layout is one the decoder cannot take (more than 8
+ *     channels, bands out of range).
+ * A file with zero frames has an empty window, so the first code passes.  Differences on purpose: the reference throws and
+ * ends the run for an unreadable file or a missing key; here each file gets its status and the others are searched.
+ * With several devices bound (vgb_init_devices) the files are split over them. */
+#define VGB_HCA_KEY_SKIPPED   1
+#define VGB_HCA_KEY_NOT_FOUND 2
+int32_t vgb_hca_find_keys(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const uint64_t *key_codes,
+                          int32_t n_keys, int32_t *key_index_out, int32_t *file_status_out);
+/* Every (file, key) outcome of vgb_hca_find_keys' test, with no skipping across keys: outcome_out[f * n_keys + k] = 0 the
+ * key passes, else 1 + 3 * j + r with j the window frame (0..9) it stops at and r 0 a bad sync word, 1 a scale-factor
+ * delta out of range, 2 UnpackingWasSuccessful false; -1 for every key of a file that is not searched (not type 56, or
+ * refused).  Returns VGB_OK unless the arguments are bad or the device fails. */
+int32_t vgb_hca_debug_key_outcomes(const uint8_t *const *files, const int64_t *lengths, int32_t n_files,
+                                   const uint64_t *key_codes, int32_t n_keys, int32_t *outcome_out);
+/* The counts of the most recent vgb_hca_find_keys / vgb_hca_debug_key_outcomes (every device): out[0] (file, key) pairs
+ * walked, [1] frames unpacked, [2] files searched, [3] device time of the search kernels in microseconds (CUDA events
+ * around each device's launch, summed over the devices). */
+int32_t vgb_hca_debug_key_search_stats(uint64_t *out, int32_t n);
 /* The decode direction of the batch job for .adx file images: AdxReader -> ToAudioStream (Containers/Adx/AdxReader.cs:14-58)
  * -> CriAdxFormat.ToPcm16 (Formats/CriAdx/CriAdxFormat.cs:35-55) -> WaveWriter, with vgb_convert_hca_to_wave_batch's
  * two-pass protocol, per-file status and sharding (files weigh frames * channels).  Per group of files, on the device:

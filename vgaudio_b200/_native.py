@@ -115,6 +115,8 @@ class VgbAdxFoundKey(C.Structure):
 VGB_ADX_KEY_SKIPPED = 1
 VGB_ADX_KEYS_ONE_FILE = 1
 VGB_ADX_MAX_CHANNELS = 255
+VGB_HCA_KEY_SKIPPED = 1     # vgb_hca_find_keys: "ciph" is not 56, not searched
+VGB_HCA_KEY_NOT_FOUND = 2   # no listed key passes
 
 
 class VgbAdxFileInfo(C.Structure):
@@ -292,6 +294,9 @@ SIGNATURES = {
     "vgb_adx_key_load": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "vgb_hca_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "vgb_hca_key_tables": (C.c_int32, [C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "vgb_hca_find_keys": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vgb_hca_debug_key_outcomes": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "vgb_hca_debug_key_search_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_hca_crypt_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_uint64, C.c_int32]),
     "vgb_hca_write_batch": (C.c_int32, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_convert_debug_stage_ms": (C.c_int32, [C.c_void_p, C.c_int32]),

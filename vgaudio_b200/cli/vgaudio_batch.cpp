@@ -23,18 +23,25 @@
 // --in-keycode otherwise), recovers it from the files first (vgb_adx_find_keys, GuessAdx): for each of revisions 8 and 9,
 // over that revision's .adx inputs, every key is printed as GuessAdx prints it and the files are decoded with the one of
 // highest full confidence (then short confidence, then the lowest key).  Without a key found they fail as without a key.
+// --hca-keys FILE, when no key option names the type-56 .hca inputs' key (--keycode with wav, --in-keycode otherwise: a
+// given key wins untested, as HcaReader's EncryptionKey ?? FindKey does), is a list of key codes, one per line, decimal or
+// 0x hex; blank lines and lines starting with # are skipped.  Per chunk of files the type-56 .hca files are searched
+// (vgb_hca_find_keys, HcaReader.FindKey over the list in order) and converted with one call per key found; each key is
+// printed with its number of files.  A file no listed key decrypts fails as without a key.
 // --devices 0,1,2,3 binds those CUDA devices (vgb_init_devices): every chunk of files is then sharded over them, one
 // worker and one copy / kernel pipeline per device.  A device may be listed more than once.  The default is device 0.
 #include <sys/stat.h>
 
 #include <algorithm>
 #include <chrono>
+#include <cerrno>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <filesystem>
 #include <fstream>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -76,7 +83,7 @@ static int usage()
     std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
-                         "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key]\n"
+                         "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key] [--hca-keys FILE]\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
                          "       .bfwav, .bcstp and .bfstp inputs\n");
     return 2;
@@ -99,6 +106,30 @@ static bool parse_devices(const std::string &list, std::vector<int32_t> &out)
 }
 
 // the revision of an .adx image (0 when its header cannot be read)
+// --hca-keys: one key code per line, decimal or 0x hex; blank lines and lines starting with # are skipped
+static bool read_hca_keys(const std::string &path, std::vector<uint64_t> &codes)
+{
+    std::ifstream f(path);
+    if (!f) { std::fprintf(stderr, "cannot read %s\n", path.c_str()); return false; }
+    std::string line;
+    for (int n = 1; std::getline(f, line); n++) {
+        const size_t a = line.find_first_not_of(" \t\r"), b = line.find_last_not_of(" \t\r");
+        if (a == std::string::npos || line[a] == '#') continue;
+        const std::string t = line.substr(a, b - a + 1);
+        const bool hex = t.size() > 2 && t[0] == '0' && (t[1] == 'x' || t[1] == 'X');
+        const size_t digits = hex ? t.find_first_not_of("0123456789abcdefABCDEF", 2) : t.find_first_not_of("0123456789");
+        errno = 0;
+        char *end = nullptr;
+        const unsigned long long v = std::strtoull(t.c_str(), &end, hex ? 16 : 10);
+        if (digits != std::string::npos || errno == ERANGE || t[0] == '-' || *end) {
+            std::fprintf(stderr, "%s:%d: not a key code: %s\n", path.c_str(), n, t.c_str());
+            return false;
+        }
+        codes.push_back((uint64_t)v);
+    }
+    return true;
+}
+
 static int adx_revision(const std::vector<uint8_t> &img)
 {
     int32_t rev = 0, n = 0, start = 0;
@@ -141,7 +172,7 @@ static bool find_adx_key(const std::vector<fs::path> &paths, int revision, vgb_a
 
 int main(int argc, char **argv)
 {
-    std::string in_dir, out_dir, fmt, key_string, in_key_string;
+    std::string in_dir, out_dir, fmt, key_string, in_key_string, hca_keys_path;
     bool recurse = false, have_code = false, have_in_code = false, find_key = false;
     uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
@@ -168,6 +199,7 @@ int main(int argc, char **argv)
         else if (a == "--devices") { if (!parse_devices(next(), devices)) return usage(); }
         else if (a == "--loop-align") opt.nw_loop_point_alignment = std::atoi(next());
         else if (a == "--find-adx-key") find_key = true;
+        else if (a == "--hca-keys") hca_keys_path = next();
         else if (a == "--little-endian") opt.nw_endianness = 1;
         else if (a == "--big-endian") opt.nw_endianness = 2;
         else if (a == "-f") {  // NwCodec + 1
@@ -220,6 +252,11 @@ int main(int argc, char **argv)
         const int32_t s = !in_key_string.empty() ? vgb_adx_key_from_string(in_key_string.c_str(), &in_adx_key) : vgb_adx_key_from_code(in_key_code, &in_adx_key);
         if (s != VGB_OK) { std::fprintf(stderr, "%s\n", vgb_last_error()); return 1; }
     }
+    // --hca-keys: the list is searched only when no key option names the .hca inputs' key
+    std::vector<uint64_t> hca_codes;
+    if (!hca_keys_path.empty() && !read_hca_keys(hca_keys_path, hca_codes)) return 1;
+    const bool search_hca = !hca_keys_path.empty() && !(to_wave ? have_code : have_in_code) && (to_wave || opt.out_type != VGB_CONTAINER_HCA);
+    std::map<int32_t, size_t> hca_key_files;  // key index -> files it decrypted
 
     // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca, .adx, NintendoWare, IDSP and HPS ones when decoding; else the WAVE
     // ones and the coded ones in another codec than the output's)
@@ -271,15 +308,36 @@ int main(int argc, char **argv)
         // codec (one for every NintendoWare reader, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
         // and one transcode call for the coded ones
         // rows 6 and 7: .adx files of revision 8 / 9 whose key --find-adx-key found, each revision with its own key
-        std::vector<int32_t> rows[8];
+        // rows 8 and up: type-56 .hca files whose key --hca-keys found, one row per key (hca_row_key)
+        std::vector<int32_t> hca_index(n, -1);
+        if (search_hca) {
+            std::vector<int32_t> hk;
+            for (int k = 0; k < n; k++) if (kind_of(files[first + k]) == 1) hk.push_back(k);
+            std::vector<const uint8_t *> hp;
+            std::vector<int64_t> hl;
+            for (int32_t k : hk) { hp.push_back(ptr[k]); hl.push_back(len[k]); }
+            std::vector<int32_t> idx(hk.size()), st(hk.size());
+            if (!hk.empty() && vgb_hca_find_keys(hp.data(), hl.data(), (int32_t)hk.size(), hca_codes.data(), (int32_t)hca_codes.size(), idx.data(), st.data()) != VGB_OK) {
+                std::fprintf(stderr, "%s\n", vgb_last_error());
+                return 1;
+            }
+            for (size_t j = 0; j < hk.size(); j++) if (st[j] == VGB_OK) hca_index[hk[j]] = idx[j];
+        }
+        std::vector<std::vector<int32_t>> rows(8);
+        std::vector<int32_t> hca_row_key(8, -1);
         for (int k = 0; k < n; k++) {
             const int kind = kind_of(files[first + k]);
             const int rev = kind == 2 && (have_found[0] || have_found[1]) ? adx_revision(in[k]) : 0;
-            if ((rev == 8 || rev == 9) && have_found[rev - 8]) rows[rev - 2].push_back(k);
+            if (hca_index[k] >= 0) {
+                const size_t row = std::find(hca_row_key.begin(), hca_row_key.end(), hca_index[k]) - hca_row_key.begin();
+                if (row == rows.size()) { rows.emplace_back(); hca_row_key.push_back(hca_index[k]); }
+                rows[row].push_back(k);
+                hca_key_files[hca_index[k]]++;
+            } else if ((rev == 8 || rev == 9) && have_found[rev - 8]) rows[rev - 2].push_back(k);
             else rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
         }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
-            for (int h = 0; h < 8; h++) {
+            for (int h = 0; h < (int)rows.size(); h++) {
                 const std::vector<int32_t> &r = rows[h];
                 if (r.empty()) continue;
                 std::vector<const uint8_t *> p;
@@ -295,14 +353,17 @@ int main(int argc, char **argv)
                 const int32_t m = (int32_t)r.size();
                 uint8_t *const *ot = outs ? o.data() : nullptr;
                 int32_t s;
-                const vgb_adx_key *wave_adx_key = h >= 6 ? &found[h - 6] : have_adx_key ? &adx_key : nullptr;
-                const vgb_adx_key *tx_adx_key = h >= 6 ? &found[h - 6] : have_in_adx_key ? &in_adx_key : nullptr;
-                if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
+                const bool adx_found = h == 6 || h == 7;
+                const vgb_adx_key *wave_adx_key = adx_found ? &found[h - 6] : have_adx_key ? &adx_key : nullptr;
+                const vgb_adx_key *tx_adx_key = adx_found ? &found[h - 6] : have_in_adx_key ? &in_adx_key : nullptr;
+                const uint64_t *hca_found = h >= 8 ? &hca_codes[(size_t)hca_row_key[h]] : nullptr;
+                if (h >= 8 && to_wave) s = vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, hca_found, sz.data(), ot, st.data());
+                else if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
                 else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key,
-                                                           have_in_code ? &in_key_code : nullptr, sz.data(), ot, st.data(), nullptr, nullptr);
+                                                           hca_found ? hca_found : have_in_code ? &in_key_code : nullptr, sz.data(), ot, st.data(), nullptr, nullptr);
                 else if (h == 4) s = vgb_convert_nw_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
                 else if (h == 5) s = vgb_convert_idsp_hps_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
-                else s = (h == 2 || h >= 6) ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, wave_adx_key, sz.data(), ot, st.data())
+                else s = (h == 2 || adx_found) ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, wave_adx_key, sz.data(), ot, st.data())
                        : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
                                 : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());
                 if (s != VGB_OK) return s;
@@ -336,6 +397,9 @@ int main(int argc, char **argv)
         first = last;
     }
     const double s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    for (const auto &kv : hca_key_files)
+        std::printf("HCA key %llu (0x%016llX, list entry %d): %zu files\n", (unsigned long long)hca_codes[(size_t)kv.first],
+                    (unsigned long long)hca_codes[(size_t)kv.first], kv.first, kv.second);
     std::printf("%zu files converted, %zu failed, %.1f MB in, %.1f MB out, %.3f s\n", done, failed, bytes_in / 1e6, bytes_out / 1e6, s);
     vgb_shutdown();
     return failed ? 3 : 0;

@@ -355,6 +355,43 @@ def adx_key_search_stats(with_time: bool = False) -> tuple:
     return tuple(int(v) for v in out[:4 if with_time else 3])
 
 
+def _hca_key_args(files: Sequence, keys: Sequence[int]):
+    arrs = [_bytes_arr(f) for f in files]
+    n = len(arrs)
+    ftab = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in arrs])
+    lens = (C.c_int64 * max(n, 1))(*[a.size for a in arrs])
+    codes = (C.c_uint64 * max(len(keys), 1))(*[int(k) & 0xFFFFFFFFFFFFFFFF for k in keys])
+    return arrs, ftab, lens, n, codes
+
+
+def hca_find_keys(files: Sequence, keys: Sequence[int]) -> Tuple[List[int], List[int]]:
+    """HcaReader.FindKey on the GPU for .hca images over a list of type-56 key codes: (indices, statuses), per file the
+    index of the first code that decrypts it (or -1) and VGB_OK, VGB_E_DATA (a bad sync word), N.VGB_HCA_KEY_SKIPPED
+    ("ciph" is not 56), N.VGB_HCA_KEY_NOT_FOUND or the file's read error."""
+    arrs, ftab, lens, n, codes = _hca_key_args(files, keys)
+    index = (C.c_int32 * max(n, 1))()
+    status = (C.c_int32 * max(n, 1))()
+    N.check(N.lib.vgb_hca_find_keys(ftab, lens, n, codes, len(keys), index, status))
+    return [int(index[i]) for i in range(n)], [int(status[i]) for i in range(n)]
+
+
+def hca_key_outcomes(files: Sequence, keys: Sequence[int]) -> np.ndarray:
+    """Every (file, key) outcome of hca_find_keys' test, int32 [files, keys]: 0 pass, else 1 + 3 * frame + reason (0 bad
+    sync, 1 scale-factor delta out of range, 2 UnpackingWasSuccessful false); -1 for a file that is not searched."""
+    arrs, ftab, lens, n, codes = _hca_key_args(files, keys)
+    out = np.zeros((n, len(keys)), dtype=np.int32)
+    N.check(N.lib.vgb_hca_debug_key_outcomes(ftab, lens, n, codes, len(keys), out.ctypes.data if out.size else None))
+    return out
+
+
+def hca_key_search_stats() -> tuple:
+    """((file, key) pairs walked, frames unpacked, files searched, device time in microseconds) of the most recent
+    hca_find_keys / hca_key_outcomes."""
+    out = (C.c_uint64 * 4)()
+    N.check(N.lib.vgb_hca_debug_key_search_stats(out, 4))
+    return tuple(int(v) for v in out)
+
+
 def brstm_parse(file) -> N.VgbNwInfo:
     """BrstmReader.ReadFile on a file image, reduced to what decoding needs; raises VgbError(VGB_E_DATA)."""
     f = _bytes_arr(file)

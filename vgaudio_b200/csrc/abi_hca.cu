@@ -186,23 +186,6 @@ void hca_channel_types(const vgb_hca_info &h, int32_t types[8])
     for (int i = 0; i < per_track; i++) types[i] = src[i];
 }
 
-// The codec configuration of a call, from the HcaInfo its streams share
-HcaConfig hca_config(const vgb_hca_info &h0)
-{
-    HcaConfig cfg{};
-    cfg.channel_count = h0.channel_count;
-    cfg.frame_size = h0.frame_size;
-    cfg.base_band_count = h0.base_band_count;
-    cfg.stereo_band_count = h0.stereo_band_count;
-    cfg.total_band_count = h0.total_band_count;
-    cfg.hfr_band_count = h0.hfr_band_count;
-    cfg.bands_per_hfr_group = h0.bands_per_hfr_group;
-    cfg.hfr_group_count = h0.hfr_group_count;
-    hca_channel_types(h0, cfg.channel_type);
-    hca_fill_ath(h0, cfg.ath);
-    return cfg;
-}
-
 // Initialize of every stream of an encode call; the streams must share the codec configuration
 int32_t hca_encode_infos(const vgb_hca_params *params, int32_t n_streams, std::vector<vgb_hca_info> &infos,
                          std::vector<HcaVirtual> &virt)
@@ -238,6 +221,23 @@ HcaStream hca_encode_stream(const vgb_hca_info &h, const HcaVirtual &v, int64_t 
 }
 
 }  // namespace
+
+// The codec configuration of a call, from the HcaInfo its streams share
+HcaConfig vgb::hca_config(const vgb_hca_info &h0)
+{
+    HcaConfig cfg{};
+    cfg.channel_count = h0.channel_count;
+    cfg.frame_size = h0.frame_size;
+    cfg.base_band_count = h0.base_band_count;
+    cfg.stereo_band_count = h0.stereo_band_count;
+    cfg.total_band_count = h0.total_band_count;
+    cfg.hfr_band_count = h0.hfr_band_count;
+    cfg.bands_per_hfr_group = h0.bands_per_hfr_group;
+    cfg.hfr_group_count = h0.hfr_group_count;
+    hca_channel_types(h0, cfg.channel_type);
+    hca_fill_ath(h0, cfg.ath);
+    return cfg;
+}
 
 int32_t vgb::hca_encode_fault(int32_t status, const char *what, int index)
 {

@@ -20,6 +20,7 @@
 // to the oracle.  ALU/latency bound: ~135 ops per sample (SURVEY.md §8d), algorithmic traffic 2 B/sample in +
 // frame_size/1024 B/sample out.
 #include "common.cuh"
+#include "hca_unpack.cuh"
 #include "kernels.h"
 
 namespace vgb {
@@ -636,6 +637,24 @@ constexpr int kRecScale = 0, kRecRes = 128, kRecIntensity = 256, kRecHfr = 264, 
 constexpr int kRecChannelBytes = kRecQuant + kSub * kBins * 2;  // 2320
 constexpr int kParseThreads = 64;
 
+// The decoder's sink of hca_unpack_walk: the parsed-frame record above; a frame that fails is left all zero
+struct HcaParseRecord {
+    uint8_t *rec;
+    int nch;
+    __device__ uint8_t *ch(int c) const { return rec + (size_t)c * kRecChannelBytes; }
+    __device__ void band(int c, int b, int sf, int res) const { ch(c)[kRecScale + b] = (uint8_t)sf; ch(c)[kRecRes + b] = (uint8_t)res; }
+    __device__ void clear_side(int c) const { for (int i = 0; i < 8; i++) { ch(c)[kRecIntensity + i] = 0; ch(c)[kRecHfr + i] = 0; } }
+    __device__ void intensity(int c, int i, int v) const { ch(c)[kRecIntensity + i] = (uint8_t)v; }
+    __device__ void hfr(int c, int i, int v) const { ch(c)[kRecHfr + i] = (uint8_t)v; }
+    __device__ void quant(int c, int sf, int b, int q) const { reinterpret_cast<int16_t *>(ch(c) + kRecQuant)[sf * kBins + b] = (int16_t)q; }
+    __device__ void quant_tail(int c, int sf, int coded) const
+    {
+        int16_t *q = reinterpret_cast<int16_t *>(ch(c) + kRecQuant) + sf * kBins;
+        for (int b = coded; b < kBins; b++) q[b] = 0;
+    }
+    __device__ void fail() const { for (int e = 0; e < nch * kRecChannelBytes; e++) rec[e] = 0; }
+};
+
 // CriHcaPacking.UnpackFrame (CriHcaPacking.cs:10-229), ONE THREAD PER FRAME.  Parsing a frame is inherently serial
 // (prefix codes), and a CTA-per-frame kernel that parks 127 threads behind one parser spent 90 % of its warp
 // instructions at 1/32 lane efficiency (ncu).  Frames are independent, so here the 32 lanes of a warp parse 32
@@ -679,9 +698,7 @@ hca_decode_parse_kernel(const uint8_t *__restrict__ frames, const HcaStream *__r
     uint8_t *rec = parsed + fi * ((int64_t)nch * kRecChannelBytes);
     const int frame_size = cfg.frame_size;
 
-    // BitReader.ReadInt / PeekInt (Utilities/BitReader.cs:51-99) over the frame's bytes in HBM: a 64-bit window keeps the
-    // next bits left-aligned, so a read is a shift; a refill happens once per 32 consumed bits from a word fetched at the
-    // previous refill; bits past the end of the frame read as zero, like the reference
+    // the frame's bytes in HBM; bits past the end of the frame read as zero, like the reference
     auto word = [&](int i) -> uint32_t {
         uint32_t v = 0;
 #pragma unroll
@@ -689,102 +706,10 @@ hca_decode_parse_kernel(const uint8_t *__restrict__ frames, const HcaStream *__r
             if (4 * i + j < frame_size) v |= (uint32_t)__ldg(src + 4 * i + j) << (24 - 8 * j);
         return v;
     };
-    uint64_t win = ((uint64_t)word(0) << 32) | word(1);
-    int avail = 64, next = 2;
-    uint32_t ahead = word(2);
-    auto peek = [&](int count) -> uint32_t { return (uint32_t)((win >> 1) >> (63 - count)); };
-    auto skip = [&](int count) {
-        win <<= count;
-        avail -= count;
-        if (avail <= 32) {
-            win |= (uint64_t)ahead << (32 - avail);
-            avail += 32;
-            ahead = word(++next);
-        }
-    };
-    auto read = [&](int count) -> int { const uint32_t v = peek(count); skip(count); return (int)v; };
-
-    int status = 0;
-    if (read(16) != 0xffff) status = VGB_HCA_BAD_SYNC;
-    const int noise_level = read(9);
-    const int eval_boundary = read(7);
-    for (int c = 0; c < nch && !status; c++) {
-        uint8_t *rc = rec + (size_t)c * kRecChannelBytes;
-        const int type = cfg.channel_type[c];
-        const int coded = type == 2 ? cfg.base_band_count : cfg.base_band_count + cfg.stereo_band_count;
-        const int delta_bits = read(3);  // ReadScaleFactors (:108-126)
-        // DeltaDecode reads output[0] before its loop, so a channel without coded bands still consumes 6 bits (:183-186)
-        if (coded == 0 && delta_bits != 0 && delta_bits < 6) skip(6);
-        int prev = 0;
-        for (int b = 0; b < kBins; b++) {
-            int sf = 0;
-            if (b < coded && delta_bits != 0) {
-                if (delta_bits >= 6 || b == 0) {
-                    sf = read(6);
-                } else {  // DeltaDecode (:183-208)
-                    const int max_delta = 1 << (delta_bits - 1);
-                    const int delta = read(delta_bits) - (max_delta - 1);  // ReadOffsetBinary, OffsetBias.Positive
-                    if (delta < max_delta) {
-                        sf = prev + delta;
-                        if (sf < 0 || sf > 63) { status = VGB_HCA_BAD_DELTA; sf = 0; }
-                    } else {
-                        sf = read(6);
-                    }
-                }
-            }
-            prev = sf;
-            int res = 0;
-            if (b < coded && sf != 0) {  // CalculateResolution (CriHcaPacking.cs:60-69) of athCurve[b] + noise (:86-94)
-                int pos = s_ath[b] + (b < eval_boundary ? noise_level - 1 : noise_level) - 5 * sf / 2 + 2;
-                pos = min(max(pos, 0), 58);
-                res = s_curve[pos];
-            }
-            rc[kRecScale + b] = (uint8_t)sf;
-            rc[kRecRes + b] = (uint8_t)res;
-            sres[((size_t)c * kBins + b) * kParseThreads + tid] = (uint8_t)res;
-        }
-        if (status) break;
-        for (int i = 0; i < 8; i++) { rc[kRecIntensity + i] = 0; rc[kRecHfr + i] = 0; }
-        if (type == 2) {
-            for (int i = 0; i < kSub; i++) {
-                int v = read(4);
-                if (v > 14) { status = VGB_HCA_BAD_INDEX; v = 14; }
-                rc[kRecIntensity + i] = (uint8_t)v;
-            }
-        } else if (cfg.hfr_group_count > 0) {
-            for (int i = 0; i < cfg.hfr_group_count; i++) rc[kRecHfr + i] = (uint8_t)read(6);
-        }
-    }
-    if (!status) {
-        for (int sf = 0; sf < kSub; sf++)  // ReadSpectralCoefficients (:144-181)
-            for (int c = 0; c < nch; c++) {
-                const int type = cfg.channel_type[c];
-                const int coded = type == 2 ? cfg.base_band_count : cfg.base_band_count + cfg.stereo_band_count;
-                int16_t *q = reinterpret_cast<int16_t *>(rec + (size_t)c * kRecChannelBytes + kRecQuant) + sf * kBins;
-                const uint8_t *rb = sres + (size_t)c * kBins * kParseThreads + tid;
-                int res = coded > 0 ? rb[0] : 0;
-                for (int b = 0; b < coded; b++) {
-                    const int res_next = b + 1 < coded ? rb[(size_t)(b + 1) * kParseThreads] : 0;
-                    const int mbits = s_maxbits[res];
-                    const unsigned long long lens = s_lens64[res], vals = s_vals64[res];
-                    const int code = (int)peek(mbits);
-                    // both code families, selected without a branch (lanes parse different frames)
-                    const int bits_p = (int)((lens >> (4 * code)) & 15u);
-                    const int v_p = (int)((unsigned)(vals >> (4 * code)) << 28) >> 28;
-                    const int mag = code >> 1;
-                    const int v_s = (code & 1) ? -mag : mag;
-                    const int bits_s = mbits - (mag == 0 ? 1 : 0);
-                    const bool prefix = mbits <= 4;
-                    q[b] = (int16_t)(prefix ? v_p : v_s);
-                    skip(prefix ? bits_p : bits_s);
-                    res = res_next;
-                }
-                for (int b = coded; b < kBins; b++) q[b] = 0;
-            }
-    } else {
-        atomicCAS(status_out + s, 0, status);
-        for (int e = 0; e < nch * kRecChannelBytes; e++) rec[e] = 0;
-    }
+    const HcaUnpackSmem S{s_lens64, s_vals64, s_maxbits, s_curve, s_ath};
+    const HcaParseRecord R{rec, nch};
+    const int status = hca_unpack_walk<false, kParseThreads>(word, cfg, S, sres + tid, R, nullptr);
+    if (status) atomicCAS(status_out + s, 0, status);
 }
 
 __global__ void __launch_bounds__(128)

@@ -132,4 +132,27 @@ cudaError_t launch_adx_key_search(const AdxKeySearch &a, int frames_after_start,
 cudaError_t launch_adx_byte_diff(const uint8_t *a, const int64_t *a_off, const uint8_t *b, const int64_t *b_off, const int32_t *n,
                                  int n_rows, int32_t *out, cudaStream_t stream);
 
+// hca_keys.cu — HcaReader.FindKey's frame test (CriHcaEncryption.FindKey / TestKey, Codecs/CriHca/CriHcaEncryption.cs:34-87)
+// over a list of type-56 key tables, one CTA per file.  Outcome of a (file, key): 0 pass, else 1 + 3 * j + r with j the
+// window frame it stops at and r 0 a bad sync word, 1 a scale-factor delta out of range, 2 UnpackingWasSuccessful false.
+constexpr int kHcaKeyWindow = 10;  // CriHcaEncryption.FramesToTest
+struct HcaKeyFileDev {
+    HcaConfig cfg;
+    int64_t frames_off;  // the window's first byte in the search's frame bytes
+    int32_t window;      // frames in the window, 0..kHcaKeyWindow
+    int32_t pad;
+};
+struct HcaKeySearch {
+    const uint8_t *frames;
+    const HcaKeyFileDev *files;
+    int32_t n_files, n_keys;
+    const uint8_t *tables;   // [n_keys][256] decryption tables, 16-byte aligned
+    int32_t every;           // 1: every outcome to outcomes[f * n_keys + k]; 0: first[2f] the decisive key of lowest index
+                             // (or -1), first[2f + 1] its outcome
+    int32_t max_channels;    // the largest channel count of the files (sizes the shared resolutions)
+    int32_t *outcomes, *first;
+    unsigned long long *stats;  // [0] (file, key) walks started, [1] frames unpacked: added to
+};
+cudaError_t launch_hca_key_search(const HcaKeySearch &a, cudaStream_t stream);
+
 }  // namespace vgb
