@@ -2,6 +2,8 @@
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 --fmad=false -o tools/microbench tools/microbench.cu
 // Default: one warp, one CTA; cycles per op = (clock after - clock before) / chain length.
 // `microbench t`: issue throughput of the integer and FP32 pipes with many warps and independent chains (run_tp below).
+// `microbench d`: a dependent DADD chain's cycles per add with 1, 2 or 4 chain warps per sub-partition beside 0, 2 or 6
+// warps that issue independent DMUL / DADD pairs (run_dc below), and the fp64 rate those warps reach.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -170,8 +172,90 @@ void run_tp(const char *name, int ops_per_chain_iter)
     cudaFree(d_out);
 }
 
+
+// ---- fp64 contention mode: CTA warp w sits on sub-partition w % 4 (its warp slot modulo 4); warps w / 4 < chains run
+// one dependent DADD chain each, the other warps run 8 independent DMUL -> DADD chains (--fmad=false keeps them two
+// instructions) until every chain warp is done.  Configurations above 8 warps per sub-partition use two CTAs per SM.
+#define D_ITER 8192
+
+__global__ void __launch_bounds__(1024) dadd_contention(long long *out, int chains, double seed)
+{
+    __shared__ int done;
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) done = 0;
+    __syncthreads();
+    long long *o = out + ((long long)blockIdx.x * 32 + w) * 2;
+    if ((w >> 2) < chains) {
+        double d = seed + threadIdx.x;
+        const long long t0 = clock64();
+#pragma unroll 16
+        for (int i = 0; i < D_ITER; i++) d = __dadd_rn(d, 1.5);
+        const long long t1 = clock64();
+        if (lane == 0) { o[0] = t1 - t0; o[1] = -1; atomicAdd(&done, 1); }
+        if (d == 0.125) o[1] = (long long)d;
+    } else {
+        double x[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) x[k] = seed + k + threadIdx.x;
+        const double m = 1.0000001, a = 0.5;
+        long long n = 0;
+        const long long t0 = clock64();
+        while (*(volatile int *)&done < chains * 4) {
+#pragma unroll 4
+            for (int i = 0; i < 16; i++) {
+#pragma unroll
+                for (int k = 0; k < 8; k++) x[k] = __dadd_rn(__dmul_rn(x[k], m), a);
+            }
+            n += 16 * 8 * 2;
+        }
+        const long long t1 = clock64();
+        double s = 0;
+#pragma unroll
+        for (int k = 0; k < 8; k++) s += x[k];
+        if (lane == 0) { o[0] = t1 - t0; o[1] = n; }
+        if (s == 0.125) o[1] = 0;
+    }
+}
+
+void run_dc(int chains, int noise)
+{
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int ctas = chains + noise > 8 ? 2 : 1;       // warps per sub-partition per CTA: (chains + noise) / ctas
+    const int c_per = chains / ctas, warps = (chains + noise) / ctas * 4;
+    long long *d_out;
+    const size_t bytes = 16ull * 32 * sms * ctas;
+    cudaMalloc(&d_out, bytes);
+    dadd_contention<<<sms * ctas, warps * 32>>>(d_out, c_per, 1.25);
+    dadd_contention<<<sms * ctas, warps * 32>>>(d_out, c_per, 1.25);
+    long long *h = new long long[bytes / 8];
+    cudaMemcpy(h, d_out, bytes, cudaMemcpyDeviceToHost);
+    double chain_cyc = 0, noise_ops = 0, noise_cyc = 0;
+    int nc = 0, nn = 0;
+    for (int b = 0; b < sms * ctas; b++)
+        for (int w = 0; w < warps; w++) {
+            const long long *o = h + ((long long)b * 32 + w) * 2;
+            if (o[1] < 0) { chain_cyc += (double)o[0]; nc++; }
+            else { noise_ops += (double)o[1]; noise_cyc += (double)o[0]; nn++; }
+        }
+    chain_cyc /= nc;
+    // fp64 warp instructions per cycle per sub-partition issued by the other warps while the chains ran
+    const double rate = nn ? noise_ops / (noise_cyc / nn) / (sms * 4.0) : 0.0;
+    printf("chains/sub %d  other fp64 warps/sub %d  %6.2f cycles per dependent DADD  %5.3f other fp64 warp instr / clk / sub\n",
+           chains, noise, chain_cyc / D_ITER, rate);
+    delete[] h;
+    cudaFree(d_out);
+}
+
 int main(int argc, char **argv)
 {
+    if (argc > 1 && argv[1][0] == 'd') {
+        const int chains[3] = {1, 2, 4}, noise[3] = {0, 2, 6};
+        for (int c : chains)
+            for (int k : noise) run_dc(c, k);
+        return 0;
+    }
     if (argc > 1 && argv[1][0] == 't') {
         run_tp<0>("IMAD only", 4);
         run_tp<1>("IMAD.WIDE + 64-bit sum (IMAD.WIDE only; +LOP3)", 1);

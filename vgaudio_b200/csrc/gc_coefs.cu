@@ -238,29 +238,32 @@ __device__ __forceinline__ int16_t gc_quantise_coef(double v)
 // warp per channel leaves most of the machine idle and each channel pays for both in sequence, so the work is split
 // and software-pipelined over CHUNKS of kRefineProducers blocks with one CTA barrier per chunk (no polling):
 //   warps 1..P (producers) classify one block of 32 records each and append every record to ITS bucket's queue in
-//              the chunk's shared-memory buffer (rank = number of earlier records of the block in the same bucket,
-//              from a ballot: record order is preserved inside a bucket);
-//   warp 0     (consumer) meanwhile walks the PREVIOUS chunk's blocks in order and lane (bucket, component) adds ONLY
+//              the chunk's shared-memory buffer (position = number of earlier records of the chunk in the same
+//              bucket: the block's from a match, the earlier blocks' from their published counts; record order is
+//              preserved inside a bucket);
+//   warp 0     (consumer) meanwhile walks the PREVIOUS chunk's queues and lane (bucket, component) adds ONLY
 //              its bucket's records, in record order - exactly the reference's sequence of additions.
 // W warps per CTA = 1 consumer + (W - 1) producers.  W = 4 keeps eight CTAs per SM (64 registers, 8 x 26 KB of shared
 // memory), which holds all 1024 channels of the headline batch at once on H100's 132 SMs (seven would leave 100 channels
 // for a second wave); W = 8 (7 producers, 61 KB of queues) is kept for experiments with small batches
 // (VGB_REFINE_WIDE_LIMIT).
 
+// One chunk of P blocks: each bucket's records of the whole chunk in ONE queue, in record order (block 0's, then block
+// 1's, ...), padded at its end only.  The rows have the same room as P per-block rows had: the 16 accumulator lanes
+// (bucket, comp) read entry j of all buckets at once, and rows of 33P / 66P / 132P / 264P entries (8 / 4 / 2 / 1 buckets)
+// put them in distinct bank pairs for P = 3 and 7.
+template <int P>
 struct __align__(16) RefineSlot {
-    double2 q[8 * 33];    // per-bucket queues of one block of 32 records, bucket b at q + b * refine_row(NB): 33 entries per
-                          // row with 8 buckets (the 16 accumulator lanes (bucket, comp) read entry j of all buckets at once,
-                          // 528-byte rows put them in 16 distinct bank pairs), 66 / 132 / 264 with 4 / 2 / 1 buckets - room
-                          // for the longer padding the consumer's wider steps need when few buckets share the block
-    int32_t count[8];     // records per bucket (buckets the pass does not use stay 0)
+    double2 q[8 * 33 * P];  // bucket b's queue at q + b * refine_row(NB, P)
+    int32_t count[P][8];    // records per block and bucket (buckets the pass does not use stay 0)
 };
 // queue row length and consumer step (entries added per loop iteration; queues are padded to a multiple of it with -0.0)
-__host__ __device__ constexpr int refine_row(int nb) { return nb >= 8 ? 33 : (nb == 4 ? 66 : (nb == 2 ? 132 : 264)); }
+__host__ __device__ constexpr int refine_row(int nb, int p) { return 33 * 8 / (nb >= 8 ? 8 : nb) * p; }
 __host__ __device__ constexpr int refine_step(int nb) { return nb >= 4 ? 4 : (nb == 2 ? 8 : 16); }
 
 template <int W>
 struct RefineShared {
-    RefineSlot slot[2][W - 1];             // double-buffered chunks
+    RefineSlot<W - 1> slot[2];              // double-buffered chunks
     double cent[8][3];                      // centroids (1, c1, c2)
     double econst[8][3];                    // per-centroid constants of ContrastVectors (:338-340), refreshed every pass
 };
@@ -268,54 +271,52 @@ struct RefineShared {
 // all kRefineWarps warps, once per chunk; PTX named barrier so that the two code paths may use different instructions
 template <int W>
 __device__ __forceinline__ void refine_chunk_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(W * 32) : "memory"); }
+// the producer warps only, once per chunk: every block's bucket counts are published before any record is placed
+template <int W>
+__device__ __forceinline__ void refine_producer_barrier() { asm volatile("bar.sync 2, %0;" ::"n"((W - 1) * 32) : "memory"); }
+
+// VGB_REFINE_DIAG (diagnostic builds of tools/refine_contention.py only; 0 everywhere else):
+//   1  the consumer adds nothing (producers only);  2  the producers queue record i of a block in bucket i % NB without
+//   the nearest-centroid search (consumer only, fixed chain);  3  the fp64 distances and compares are replaced by
+//   integer stand-ins of about the same instruction count (the centroids picked are meaningless).
+#ifndef VGB_REFINE_DIAG
+#define VGB_REFINE_DIAG 0
+#endif
 
 // consumer side of one pass: ordered accumulation (:382-386 / :67-72).  Lane (bucket*2 + comp) walks its bucket's queue
-// of every block in block order - a pure DADD chain over exactly the bucket's records, in record order.
+// of every chunk in chunk order - a pure DADD chain over exactly the bucket's records, in record order.
 struct RefineSum { double acc; int hits; };
 template <int NB, int W>
-__device__ __forceinline__ RefineSum gc_refine_consume(int lane, int n_blocks, int n_chunks, RefineShared<W> &sh)
+__device__ __forceinline__ RefineSum gc_refine_consume(int lane, int n_chunks, RefineShared<W> &sh)
 {
     constexpr int P = W - 1;
-    constexpr int STEP = refine_step(NB), ROW = refine_row(NB);
+    constexpr int STEP = refine_step(NB), ROW = refine_row(NB, P);
     const int my_bucket = (lane >> 1) & 7, my_comp = lane & 1;
+    const bool active = lane < 16 && my_bucket < NB;
+    const int off = (active ? my_bucket : 0) * ROW * 2 + my_comp;  // the lane's column in a slot, in doubles
     double a = 0.0;
     int h = 0;
-    const bool active = lane < 16 && my_bucket < NB;
     refine_chunk_barrier<W>();  // chunk 0 classified
     for (int c = 1; c <= n_chunks; c++) {
-        const int first = (c - 1) * P;
-        const RefineSlot *slot = sh.slot[(c - 1) & 1];
-        const int off = (my_bucket < NB ? my_bucket : 0) * ROW * 2 + my_comp;  // the lane's column in a slot, in doubles
-        // The lane's entries of the whole chunk form one stream: block 0's queue padded to a multiple of STEP with -0.0
-        // (the additive identity; the producers write the padding), then block 1's, ...  All counts are read up front,
-        // and every group of STEP entries is loaded while the previous group is being added, so the shared-memory latency
-        // of the counts and of the entries sits on the DADD chain once per chunk (after the barrier) instead of once per
-        // block and per group.  The trip count differs per lane; lanes whose stream ends drop out.
-        int pre[P + 1];  // pre[j] = padded entries before block j
-        pre[0] = 0;
+        const RefineSlot<P> &slot = sh.slot[(c - 1) & 1];
+        int n = 0;
+        if (active) {
 #pragma unroll
-        for (int j = 0; j < P; j++) {
-            const int n = (active && first + j < n_blocks) ? slot[j].count[my_bucket] : 0;
-            h += n;
-            pre[j + 1] = pre[j] + (n + STEP - 1) / STEP * STEP;
+            for (int j = 0; j < P; j++) n += slot.count[j][my_bucket];
         }
-        auto group = [&](int t) {  // the first entry of the group at stream position t
-            const double *q = reinterpret_cast<const double *>(slot[0].q) + off + 2 * t;
-#pragma unroll
-            for (int j = 1; j < P; j++)
-                if (t >= pre[j]) q = reinterpret_cast<const double *>(slot[j].q) + off + 2 * (t - pre[j]);
-            return q;
-        };
-        const int total = pre[P];
+        h += n;
+        // The lane's queue is contiguous and padded to a multiple of STEP with -0.0 (the additive identity; the producers
+        // write the padding), so the walk is a pointer increment per group.  Every group of STEP entries is loaded while
+        // the previous group is being added; the last load reads up to STEP entries past the queue, still inside the
+        // shared buffer, and is not used.  The trip count differs per lane; lanes whose queue ends drop out.
+        const int total = VGB_REFINE_DIAG == 1 ? 0 : (n + STEP - 1) / STEP * STEP;
+        const double *q = reinterpret_cast<const double *>(slot.q) + off;
         double v[STEP];
-        {
-            const double *q = group(0);
 #pragma unroll
-            for (int i = 0; i < STEP; i++) v[i] = q[2 * i];
-        }
+        for (int i = 0; i < STEP; i++) v[i] = q[2 * i];
         for (int t = 0; t < total; t += STEP) {
+            q += 2 * STEP;
             double nx[STEP];
-            const double *q = group(t + STEP < total ? t + STEP : t);  // the last group reloads itself (unused)
 #pragma unroll
             for (int i = 0; i < STEP; i++) nx[i] = q[2 * i];
 #pragma unroll
@@ -338,7 +339,7 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
 {
     constexpr int NB = COUNT > 0 ? COUNT : 1;
     constexpr int P = W - 1;
-    constexpr int STEP = refine_step(NB), ROW = refine_row(NB);
+    constexpr int STEP = refine_step(NB), ROW = refine_row(NB, P);
     const uint32_t lanes_below = (1u << lane) - 1u;
     const int p = warp - 1;                              // producer index (warp 0: unused)
     const int n_chunks = (n_blocks + P - 1) / P;
@@ -352,11 +353,35 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
             if (f < n_frames) r = rec[f];
         }
     };
-    // producer: classify block b (nearest centroid, parallel over its 32 records) into `slot`
-    auto stage = [&](int b, double2 r, uint32_t okbits, RefineSlot &slot) {
+    // producer: classify block b (nearest centroid, parallel over its 32 records) into the chunk's queues in `slot`.
+    // Called by every producer for every chunk, also for blocks past the end (no record of theirs is accepted), because
+    // of the producer barrier.
+    auto stage = [&](int b, double2 r, uint32_t okbits, RefineSlot<P> &slot) {
         const bool ok = ((okbits >> lane) & 1u) && (b * 32 + lane < n_frames);
         int pick = 0;
-        if (COUNT > 1) {
+        if (VGB_REFINE_DIAG == 2) {
+            pick = lane % NB;
+        } else if (COUNT > 1 && VGB_REFINE_DIAG == 3) {
+            const int ta = __double2loint(r.x) << 1, tb = __double2loint(r.y) << 1;
+            int d[NB], idx[NB];
+#pragma unroll
+            for (int i = 0; i < NB; i++) {
+                const int di = (__double2loint(sh.econst[i][0]) ^ (ta * __double2loint(sh.econst[i][1]))) +
+                               tb * __double2loint(sh.econst[i][2]);
+                d[i] = di < 0x40000000 ? di : 0x7FFFFFFF;
+                idx[i] = i;
+            }
+#pragma unroll
+            for (int step = 1; step < NB; step *= 2) {
+#pragma unroll
+                for (int i = 0; i + step < NB; i += 2 * step) {
+                    const bool right = d[i + step] < d[i];
+                    d[i] = right ? d[i + step] : d[i];
+                    idx[i] = right ? idx[i + step] : idx[i];
+                }
+            }
+            pick = d[0] < 0x40000000 ? idx[0] : 0;
+        } else if (COUNT > 1) {
             // ContrastVectors (:335-342); its `val` is r.x and (-rec1*val - rec2) is r.y (DESIGN.md §5.1)
             const double ta = 2.0 * r.x, tb = 2.0 * r.y;
             // all distances first (independent), then a tournament instead of the reference's sequential scan
@@ -383,19 +408,25 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
         }
         // lanes that picked the same bucket find each other with ONE match instead of a ballot per bucket; records that
         // were not accepted form their own group (key NB) and are not queued
-        if (lane < NB) slot.count[lane] = 0;
+        if (lane < NB) slot.count[p][lane] = 0;
         const uint32_t mine = __match_any_sync(0xFFFFFFFFu, ok ? pick : NB);
         __syncwarp();
-        if (ok) {
-            const int rank = __popc(mine & lanes_below);
-            if (rank == 0) slot.count[pick] = __popc(mine);  // the group's first lane publishes its size
-            slot.q[pick * ROW + rank] = r;
+        const int rank = __popc(mine & lanes_below);
+        if (ok && rank == 0) slot.count[p][pick] = __popc(mine);  // the group's first lane publishes its size
+        refine_producer_barrier<W>();
+        if (ok) {  // after the bucket's records of the chunk's earlier blocks
+            int base = rank;
+#pragma unroll
+            for (int j = 0; j < P - 1; j++)
+                if (j < p) base += slot.count[j][pick];
+            slot.q[pick * ROW + base] = r;
         }
-        __syncwarp();
-        {   // pad every queue to a multiple of STEP entries with -0.0 (lane = bucket * STEP + i; NB * STEP <= 32)
+        if (p == P - 1) {  // pad every queue to a multiple of STEP entries with -0.0 (lane = bucket * STEP + i; NB * STEP <= 32)
             const int bucket = lane / STEP, i = lane % STEP;
             if (bucket < NB) {
-                const int c = slot.count[bucket];
+                int c = 0;
+#pragma unroll
+                for (int j = 0; j < P; j++) c += slot.count[j][bucket];
                 if (i < ((STEP - (c % STEP)) % STEP)) slot.q[bucket * ROW + c + i] = make_double2(-0.0, -0.0);
             }
         }
@@ -413,7 +444,7 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
     if (warp == 0) {
         // consumer: deliberately small, rolled code (it is the critical path and must stay in the instruction cache
         // next to the producers' large unrolled loop); inlined so that `sh` stays a shared-window address
-        const RefineSum sum = gc_refine_consume<NB, W>(lane, n_blocks, n_chunks, sh);
+        const RefineSum sum = gc_refine_consume<NB, W>(lane, n_chunks, sh);
         acc = sum.acc;
         hits = sum.hits;
         return;
@@ -424,7 +455,7 @@ __device__ __forceinline__ void gc_refine_pass(int warp, int lane, int n_frames,
             const int c = c0 + k;
             if (c > n_chunks) break;
             const int b = c * P + p;
-            if (b < n_blocks) stage(b, ring_r[k], ring_ok[k], sh.slot[c & 1][p]);
+            if (c < n_chunks) stage(b, ring_r[k], ring_ok[k], sh.slot[c & 1]);
             fetch(b + kDepth * P, ring_r[k], ring_ok[k]);
             refine_chunk_barrier<W>();  // chunk c is classified, chunk c-1 is summed: the two buffers swap roles
         }
@@ -454,7 +485,7 @@ __device__ __forceinline__ void gc_coef_refine(GcChannelTable tab, const double2
     const uint32_t *mask = accept_mask + (tab.rec_off[ch] >> 5);
 
     if (threadIdx.x < 8) { best[threadIdx.x][0] = 1.0; best[threadIdx.x][1] = 0.0; best[threadIdx.x][2] = 0.0; }
-    if (threadIdx.x < 2 * kRefineProducers * 8) sh.slot[threadIdx.x / (kRefineProducers * 8)][(threadIdx.x / 8) % kRefineProducers].count[threadIdx.x & 7] = 0;
+    if (threadIdx.x < 2 * kRefineProducers * 8) sh.slot[threadIdx.x / (kRefineProducers * 8)].count[(threadIdx.x / 8) % kRefineProducers][threadIdx.x & 7] = 0;
     __syncthreads();
 
     // pass 0 is the plain ordered mean (:63-76); passes 1..6 are the FilterRecords rounds (:79-91): split, then two
