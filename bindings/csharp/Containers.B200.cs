@@ -185,6 +185,9 @@ namespace VGAudio.Native
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_transcode_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
             VgbAdxKey* inAdxKey, ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_rewrite_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, VgbAdxKey* inAdxKey,
+            ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
     }
 }
 
@@ -546,6 +549,56 @@ namespace VGAudio.Cli
                         Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
                         File.WriteAllBytes(outPaths[i], outputs[i]);
                     }
+                }
+            }
+            finally
+            {
+                foreach (var h in inPins) h.Free();
+                foreach (var h in outPins) h.Free();
+            }
+        }
+
+        // Convert.ConvertFile with the same container on both sides (.adx -> .adx or .hca -> .hca): the frames are
+        // decrypted with inAdxKey (revision 8 / 9 .adx files) or inHcaKeyCode ("ciph" 56 .hca files; "ciph" 1 uses the
+        // built-in table) and encrypted with the output key in options, or written in the clear - never re-encoded, so
+        // the encoder's options do not apply.  options.OutType (VGB_CONTAINER_ADX or _HCA) names the reader and the writer.
+        public static unsafe void Rewrite(string[] inPaths, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
+            ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd)
+        {
+            int n = inPaths.Length;
+            byte[][] images = inPaths.Select(File.ReadAllBytes).ToArray();
+            var inPins = images.Select(a => GCHandle.Alloc(a, GCHandleType.Pinned)).ToArray();
+            var outPins = new List<GCHandle>();
+            try
+            {
+                byte** inPtr = stackalloc byte*[n];
+                byte** outPtr = stackalloc byte*[n];
+                long* len = stackalloc long[n];
+                long* outSize = stackalloc long[n];
+                int* status = stackalloc int[n];
+                VgbAdxKey k = inAdxKey ?? default;
+                VgbAdxKey* keyPtr = inAdxKey.HasValue ? &k : null;
+                ulong code = inHcaKeyCode ?? 0;
+                ulong* codePtr = inHcaKeyCode.HasValue ? &code : null;
+                for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
+                VgAudioB200.Check(VgAudioB200Containers.vgb_rewrite_batch(inPtr, len, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero));
+                var outputs = new byte[n][];
+                for (int i = 0; i < n; i++)
+                {
+                    outPtr[i] = null;
+                    if (status[i] != VgAudioB200.Ok) continue;
+                    outputs[i] = new byte[outSize[i]];
+                    outPins.Add(GCHandle.Alloc(outputs[i], GCHandleType.Pinned));
+                    outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
+                }
+                VgbProgress cb = (user, delta) => reportAdd((int)delta);   // progress.ReportAdd(1) per file (Batch.cs:45)
+                VgAudioB200.Check(VgAudioB200Containers.vgb_rewrite_batch(inPtr, len, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero));
+                GC.KeepAlive(cb);
+                for (int i = 0; i < n; i++)
+                {
+                    if (status[i] != VgAudioB200.Ok) { log($"Error converting {Path.GetFileName(inPaths[i])}"); continue; }   // Batch.cs:39-43
+                    Directory.CreateDirectory(Path.GetDirectoryName(outPaths[i]));
+                    File.WriteAllBytes(outPaths[i], outputs[i]);
                 }
             }
             finally

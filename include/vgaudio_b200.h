@@ -994,6 +994,48 @@ int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n);
 int32_t vgb_transcode_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                             const vgb_convert_options *options, const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code,
                             int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
+/* Rewriting .adx or .hca files in their own codec without re-encoding: decrypted, re-keyed or left as they are
+ * (Convert.ConvertFile with the same container on both sides: the reader decrypts the frames, AudioData.GetFormat<T>
+ * hands the writer the source's own CriAdxFormat / CriHcaFormat, Formats/AudioData.cs:20-33, and the writer encrypts
+ * them with the output key or writes them in the clear).  options->out_type (VGB_CONTAINER_ADX or _HCA) names both the
+ * reader and the writer: every file is read by it.  Same two-pass protocol, per-file status, progress, group_bytes
+ * (INPUT bytes per GPU batch; 0: an eighth of the job, 64..512 MiB) and sharding over the bound devices (files weigh
+ * their payload bytes) as vgb_transcode_batch; the sizing pass runs on the host only.  No payload byte is touched on
+ * the host: per batch one H2D of the frame regions, one kernel pass, one D2H of the finished files.
+ * Input keys as in vgb_transcode_batch: *in_adx_key decrypts revision 8 and 9 .adx files, *in_hca_key_code "ciph" 56
+ * .hca files, "ciph" 1 uses the built-in table.  The output key: adx_has_key with the adx_key_* fields and
+ * adx_encryption_type (the header's encryption byte, written with or without a key), or hca_key_type (-1 none, 0, 1,
+ * 56) with hca_key_code.  adx_version, adx_frame_size, adx_type, adx_filter_plus1, hca_quality, hca_bitrate and
+ * hca_limit_bitrate are ignored: the writer receives the source's format and they only reach the encoder.
+ *   .adx (AdxReader.cs:14-58 -> AdxWriter.cs:18-140): the header is rebuilt from the source's frame size, version,
+ *   type byte and high-pass (0 for type 2, Fixed), SampleCount - InsertedSamples samples with AlignmentSamples =
+ *   InsertedSamples, the loop points minus InsertedSamples, and a version-4 history block holding each channel's first
+ *   history sample twice.  TrimFile (!no_trim) cuts a looping file at LoopEnd + 3 frames, which may be more frames than
+ *   the source holds: those stay zero.  Output frame j * channels + c is source frame j * channels + c; its two scale
+ *   bytes go through the source's key stream, then the output's, at that step, each side behind its own FrameNotEmpty
+ *   test and type-9 mask (adx_rewrite_kernel).
+ *   .hca (HcaReader.cs:20-49 -> HcaWriter.cs:21-178): the frames are decrypted where HcaReader decrypts them ("ciph" 1,
+ *   or 56 with a key) and encrypted with the output key: bytes [0, FrameSize - 2) through one composed substitution
+ *   table and the CRC-16 recomputed (also for an output key of type 0); with neither they are copied verbatim, a wrong
+ *   CRC included.  The header is regenerated at the source's header_size: version 0x0200, chunks HCA fmt comp [loop]
+ *   ciph [rva] comm|pad, ids masked with 0x80 iff an output key is given, "ciph" the output key's type, else 0 for a
+ *   decrypted source and the source's value otherwise; a dec chunk comes out as comp, track_count below 1 as 1, ath and
+ *   vbr are dropped (so a version < 2.0 file without ath decodes differently afterwards, as in the reference).  The
+ *   comment is ReadUTF8Z's (Utilities/Extensions.cs:60-73: from one byte past the comm id to the first byte 0x00 or
+ *   0x01; at the end of the image its last byte is dropped), written as pad when every character is white space to
+ *   string.IsNullOrWhiteSpace; rva is kept as its float bits and written whenever the volume is not 1 (NaN included).
+ *   Chunks that do not fit in header_size - 2 bytes are written on as the reference's writer does: the header CRC covers
+ *   the first header_size - 2 bytes as written, and the CRC and the frames overwrite the rest.
+ * Per-file errors of the sizing pass, each failing that file only: the parse errors of vgb_adx_parse / vgb_hca_parse, a
+ * keyed source without its key, loop points WithLoop refuses (AudioFormatBaseBuilder.cs:23-50), an InsertedSamples
+ * above the sample count or below 0 (VGB_E_ARG), 2 GiB of output or more.  Differences on purpose: an encrypted source
+ * without its key fails (the reference would pass the encrypted frames through, an .adx file even labelled with the
+ * output's encryption byte); a comment that is not valid UTF-8 fails with VGB_E_DATA (the reference would write U+FFFD
+ * in place of the bad bytes); HCA chunks that run past the end of the output file fail with VGB_E_DATA (the reference
+ * would grow the file: only a tiny header_size with few frames can do that).  There is no device-side refusal. */
+int32_t vgb_rewrite_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_convert_options *options,
+                          const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code, int64_t *out_sizes, uint8_t *const *files_out,
+                          int32_t *status_out, vgb_progress_cb cb, void *user);
 /* Measurement tap: device time of the most recent vgb_convert_wave_batch summed over its (first 32) batches per device,
  * over every device that converted part of it, out[0..3] = WAVE split, encode, loop-context decode, file assembly (ms,
  * CUDA events on the kernel streams); returns the number of batches timed on all devices together. */

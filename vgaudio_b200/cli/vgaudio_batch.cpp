@@ -11,10 +11,13 @@
 //
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav, .bcstp and .bfstp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
-//                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]
+//                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST] [--rewrite]
 //
 // With --out-format dsp|adx|hca the inputs are the .wav / .wave files and the .dsp, .adx and .hca files in another codec
 // than the output's (a file already in the output's codec is not listed: the same codec would be a rewrite).
+// --rewrite, with --out-format adx|hca only, also lists the .adx (respectively .hca) inputs and rewrites them in their own
+// codec without re-encoding (vgb_rewrite_batch): decrypted with their input key and written in the clear, or re-keyed
+// with the output key; the encoder's options do not apply to them.
 // --keycode / --keystring are the output's key; --in-keycode N is the key of type-56 .hca inputs, and --in-keystring S,
 // or else --in-keycode N, the CriAdxKey of type-8 / type-9 .adx inputs.
 // With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
@@ -81,7 +84,7 @@ static const int32_t kContainerOfKind[3] = {VGB_CONTAINER_DSP, VGB_CONTAINER_HCA
 static int usage()
 {
     std::fprintf(stderr, "usage: vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r] [--no-trim] [--hcaquality Q] [--bitrate N]\n"
-                         "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]\n"
+                         "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S] [--rewrite]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key] [--hca-keys FILE]\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
@@ -173,7 +176,7 @@ static bool find_adx_key(const std::vector<fs::path> &paths, int revision, vgb_a
 int main(int argc, char **argv)
 {
     std::string in_dir, out_dir, fmt, key_string, in_key_string, hca_keys_path;
-    bool recurse = false, have_code = false, have_in_code = false, find_key = false;
+    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false;
     uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
     std::vector<int32_t> devices;  // empty: device 0 through vgb_init
@@ -199,6 +202,7 @@ int main(int argc, char **argv)
         else if (a == "--devices") { if (!parse_devices(next(), devices)) return usage(); }
         else if (a == "--loop-align") opt.nw_loop_point_alignment = std::atoi(next());
         else if (a == "--find-adx-key") find_key = true;
+        else if (a == "--rewrite") rewrite = true;
         else if (a == "--hca-keys") hca_keys_path = next();
         else if (a == "--little-endian") opt.nw_endianness = 1;
         else if (a == "--big-endian") opt.nw_endianness = 2;
@@ -228,6 +232,10 @@ int main(int argc, char **argv)
     else if (fmt == "hps") opt.out_type = VGB_CONTAINER_HPS;
     else if (fmt == "hca") opt.out_type = VGB_CONTAINER_HCA;
     else if (!to_wave) return usage();
+    if (rewrite && opt.out_type != VGB_CONTAINER_ADX && opt.out_type != VGB_CONTAINER_HCA) {
+        std::fprintf(stderr, "--rewrite takes --out-format adx or hca\n");
+        return 2;
+    }
     if ((opt.out_type == VGB_CONTAINER_IDSP || opt.out_type == VGB_CONTAINER_HPS) && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2)) {
         // CreateConfiguration.Idsp / .Hps (src/VGAudio.Cli/CreateConfiguration.cs:57-75, 103-115): GC-ADPCM only
         std::fprintf(stderr, "Can't use format %s with %s files\n", opt.nw_codec_plus1 == 2 ? "PCM16" : "PCM8",
@@ -255,11 +263,11 @@ int main(int argc, char **argv)
     // --hca-keys: the list is searched only when no key option names the .hca inputs' key
     std::vector<uint64_t> hca_codes;
     if (!hca_keys_path.empty() && !read_hca_keys(hca_keys_path, hca_codes)) return 1;
-    const bool search_hca = !hca_keys_path.empty() && !(to_wave ? have_code : have_in_code) && (to_wave || opt.out_type != VGB_CONTAINER_HCA);
+    const bool search_hca = !hca_keys_path.empty() && !(to_wave ? have_code : have_in_code) && (to_wave || opt.out_type != VGB_CONTAINER_HCA || rewrite);
     std::map<int32_t, size_t> hca_key_files;  // key index -> files it decrypted
 
     // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca, .adx, NintendoWare, IDSP and HPS ones when decoding; else the WAVE
-    // ones and the coded ones in another codec than the output's)
+    // ones and the coded ones in another codec than the output's, and with --rewrite those in the output's codec too)
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
@@ -267,7 +275,7 @@ int main(int argc, char **argv)
         const int kind = kind_of(e.path());
         if (kind < 0) return;
         const bool nw_out = opt.out_type >= VGB_CONTAINER_BRSTM;  // NintendoWare, IDSP and HPS targets take WAVE inputs only
-        if (to_wave ? kind != 3 : (kind == 3 || (!nw_out && kind < 3 && kContainerOfKind[kind] != opt.out_type))) files.push_back(e.path());
+        if (to_wave ? kind != 3 : (kind == 3 || (!nw_out && kind < 3 && (rewrite || kContainerOfKind[kind] != opt.out_type)))) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -280,7 +288,7 @@ int main(int argc, char **argv)
     const bool adx_key_given = to_wave ? have_adx_key : have_in_adx_key;
     vgb_adx_key found[2]{};
     bool have_found[2] = {false, false};
-    if (find_key && !adx_key_given && (to_wave || opt.out_type != VGB_CONTAINER_ADX)) {
+    if (find_key && !adx_key_given && (to_wave || opt.out_type != VGB_CONTAINER_ADX || rewrite)) {
         std::vector<fs::path> adx;
         for (const fs::path &p : files) if (kind_of(p) == 2) adx.push_back(p);
         for (int r = 0; r < 2; r++) have_found[r] = find_adx_key(adx, 8 + r, found[r]);
@@ -306,7 +314,7 @@ int main(int argc, char **argv)
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
         // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
         // codec (one for every NintendoWare reader, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
-        // and one transcode call for the coded ones
+        // and one transcode call for the coded ones (with --rewrite, one rewrite call for those in the output's codec)
         // rows 6 and 7: .adx files of revision 8 / 9 whose key --find-adx-key found, each revision with its own key
         // rows 8 and up: type-56 .hca files whose key --hca-keys found, one row per key (hca_row_key)
         std::vector<int32_t> hca_index(n, -1);
@@ -337,8 +345,16 @@ int main(int argc, char **argv)
             else rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
         }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
-            for (int h = 0; h < (int)rows.size(); h++) {
-                const std::vector<int32_t> &r = rows[h];
+            for (int part = 0; part < (int)rows.size() * 2; part++) {
+                // every row splits into the files in another codec than the output's (part even) and, transcoding, the
+                // ones in the output's own codec (part odd), which only --rewrite lists
+                const int h = part / 2;
+                std::vector<int32_t> r;
+                for (int32_t k : rows[h]) {
+                    const int kind = kind_of(files[first + k]);
+                    const bool same = !to_wave && h != 3 && kind < 3 && kContainerOfKind[kind] == opt.out_type;
+                    if (same == (part % 2 == 1)) r.push_back(k);
+                }
                 if (r.empty()) continue;
                 std::vector<const uint8_t *> p;
                 std::vector<int64_t> l, sz(r.size());
@@ -357,10 +373,12 @@ int main(int argc, char **argv)
                 const vgb_adx_key *wave_adx_key = adx_found ? &found[h - 6] : have_adx_key ? &adx_key : nullptr;
                 const vgb_adx_key *tx_adx_key = adx_found ? &found[h - 6] : have_in_adx_key ? &in_adx_key : nullptr;
                 const uint64_t *hca_found = h >= 8 ? &hca_codes[(size_t)hca_row_key[h]] : nullptr;
-                if (h >= 8 && to_wave) s = vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, hca_found, sz.data(), ot, st.data());
+                const uint64_t *tx_hca_key = hca_found ? hca_found : have_in_code ? &in_key_code : nullptr;
+                if (part % 2) s = vgb_rewrite_batch(p.data(), l.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot, st.data(), nullptr, nullptr);
+                else if (h >= 8 && to_wave) s = vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, hca_found, sz.data(), ot, st.data());
                 else if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
-                else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key,
-                                                           hca_found ? hca_found : have_in_code ? &in_key_code : nullptr, sz.data(), ot, st.data(), nullptr, nullptr);
+                else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot,
+                                                           st.data(), nullptr, nullptr);
                 else if (h == 4) s = vgb_convert_nw_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
                 else if (h == 5) s = vgb_convert_idsp_hps_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
                 else s = (h == 2 || adx_found) ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, wave_adx_key, sz.data(), ot, st.data())

@@ -470,3 +470,16 @@ def transcode_batch(files: Sequence, in_types: Sequence[int], options: N.VgbConv
         ftab, lens, types, n, C.byref(options), C.byref(adx_key) if adx_key is not None else None,
         C.byref(code) if code is not None else None, sizes, otab, st, cb if otab is not None else None, None), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def rewrite_batch(files: Sequence, options: N.VgbConvertOptions, adx_key: Optional[N.VgbAdxKey] = None,
+                  hca_key_code: Optional[int] = None, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """.adx or .hca images rewritten in their own codec without re-encoding (options.out_type, CONTAINER_ADX or
+    CONTAINER_HCA, names the reader and the writer): decrypted with adx_key (revision 8 / 9 sources) or hca_key_code
+    ("ciph" 56 sources), then encrypted with the output key in options or written in the clear:
+    ([output file bytes or None], [per-file status])."""
+    code = C.c_uint64(hca_key_code) if hca_key_code is not None else None
+    cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
+    return _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_rewrite_batch(
+        ftab, lens, n, C.byref(options), C.byref(adx_key) if adx_key is not None else None,
+        C.byref(code) if code is not None else None, sizes, otab, st, cb if otab is not None else None, None), files)

@@ -78,6 +78,19 @@ struct AdxFile {
     int32_t tile_first;
 };
 
+// An .adx file rewritten in its own codec (vgb_rewrite_batch): both sides are frame-interleaved with the same channel
+// count and frame size, so output frame p (= j * channels + c) is source frame p, which is also its key stream step
+struct AdxRewriteFile {
+    int64_t out_off;         // bytes into the output slab
+    int64_t hdr_off;         // bytes into the header blob (audio_offset bytes)
+    int64_t src_off;         // bytes into the input slab: the source's interleaved audio region (multiple of 16)
+    int32_t frame_size, frames, src_frames;       // frames written / frames the source holds, over all channels
+    int32_t audio_offset, footer_offset, footer_size;
+    int32_t dec_type, dec_seed, dec_mult, dec_inc; // the source's key: revision 8 or 9, or dec_type 0 for none
+    int32_t has_key, enc_type, seed, mult, inc;    // the output's key and the encryption type its header states
+    int32_t tile_first;
+};
+
 struct HcaFile {
     int64_t out_off, hdr_off, frames_off;
     int32_t header_size, frame_size, frame_count;
@@ -372,6 +385,64 @@ __global__ void __launch_bounds__(256) adx_assemble_kernel(const AdxFile *__rest
             for (int k = 2; k < fs; k++) { const uint8_t v = s[k]; any |= v; o[k] = v; }
         }
         if (f.has_key && (any | b0 | b1)) {  // FrameNotEmpty (CriAdxEncryption.cs:104-115)
+            const int x = adx_key_at(f.seed, f.mult, f.inc, (uint32_t)p);
+            b0 ^= (uint8_t)(x >> 8);
+            if (f.enc_type == 9) b0 &= 0x1f;
+            b1 ^= (uint8_t)x;
+        }
+        o[0] = b0;
+        o[1] = b1;
+    }
+}
+
+// The same-codec rewrite of .adx files (AdxReader -> AdxWriter without an encode): tile 0 as in adx_assemble_kernel,
+// the others move kAdxFramesPerTile frames each from the source's interleaved region, thread = frame.  The scale bytes
+// go through the source's key stream, then the output's, both at step p (CriAdxEncryption.cs:8-44), each behind its own
+// FrameNotEmpty test: the decryption tests the bytes as read, the encryption the bytes as decrypted.  Frames past the
+// source stay zero (Interleave.cs:43-78 copies nothing there) and are never encrypted.
+__global__ void __launch_bounds__(256) adx_rewrite_kernel(const AdxRewriteFile *__restrict__ files, int n_files, const uint8_t *__restrict__ src,
+                                                           const uint8_t *__restrict__ hdr_blob, uint8_t *__restrict__ out)
+{
+    const int fi = find_item(files, n_files, (int)blockIdx.x);
+    const AdxRewriteFile f = files[fi];
+    const int tile = (int)blockIdx.x - f.tile_first;
+    uint8_t *dst = out + f.out_off;
+    if (tile == 0) {
+        for (int t = threadIdx.x; t < f.audio_offset; t += blockDim.x) dst[t] = hdr_blob[f.hdr_off + t];
+        for (int t = threadIdx.x; t < f.footer_size; t += blockDim.x) {  // WriteFooter (AdxWriter.cs:135-140)
+            const int pad = f.footer_size - 4;
+            dst[f.footer_offset + t] = t == 0 ? 0x80 : t == 1 ? 0x01 : t == 2 ? (uint8_t)(pad >> 8) : t == 3 ? (uint8_t)pad : 0;
+        }
+        return;
+    }
+    const int fs = f.frame_size;
+    const bool halves = ((fs | f.audio_offset | (int)(f.out_off & 1)) & 1) == 0;  // src_off is even
+    const int first = (tile - 1) * kAdxFramesPerTile;
+    for (int t = threadIdx.x; t < kAdxFramesPerTile; t += blockDim.x) {
+        const int p = first + t;
+        if (p >= f.frames) break;
+        uint8_t *o = dst + f.audio_offset + (int64_t)p * fs;
+        if (p >= f.src_frames) {
+            for (int k = 0; k < fs; k++) o[k] = 0;
+            continue;
+        }
+        const uint8_t *s = src + f.src_off + (int64_t)p * fs;
+        uint32_t any = 0;
+        uint8_t b0 = s[0], b1 = s[1];
+        if (halves) {
+            const uint16_t *s2 = reinterpret_cast<const uint16_t *>(s);
+            uint16_t *o2 = reinterpret_cast<uint16_t *>(o);
+            for (int k = 1; k < fs / 2; k++) { const uint16_t v = s2[k]; any |= v; o2[k] = v; }
+        } else {
+            for (int k = 2; k < fs; k++) { const uint8_t v = s[k]; any |= v; o[k] = v; }
+        }
+        if (f.dec_type && (any | b0 | b1)) {
+            const int x = adx_key_at(f.dec_seed, f.dec_mult, f.dec_inc, (uint32_t)p);
+            b0 ^= (uint8_t)(x >> 8);
+            if (f.dec_type == 9) b0 &= 0x1f;
+            b1 ^= (uint8_t)x;
+        }
+        if (f.has_key && (any | b0 | b1)) {
             const int x = adx_key_at(f.seed, f.mult, f.inc, (uint32_t)p);
             b0 ^= (uint8_t)(x >> 8);
             if (f.enc_type == 9) b0 &= 0x1f;
@@ -1328,11 +1399,17 @@ uint16_t crc16_host(const uint8_t *data, size_t n)  // Crc16.Compute (Utilities/
     for (size_t i = 0; i < n; i++) crc = (uint16_t)((crc << 8) ^ table[(crc >> 8) ^ data[i]]);
     return crc;
 }
-int32_t hca_build_header(const vgb_hca_info &h, bool masked, int key_type, const char *comment, uint32_t volume_bits,
-                         std::vector<uint8_t> &out, int index)
+// The header_size bytes in front of the frames.  ciph: the "ciph" chunk's value; comment: comment_len bytes of UTF-8
+// (no zero byte), written as "comm" unless blank (string.IsNullOrWhiteSpace, judged by the caller), else "pad".
+// file_size < 0: chunks that do not fit in header_size - 2 bytes are refused (VGB_E_ARG).  Otherwise the reference's
+// stream writer is followed: the chunks run on past header_size - 2, the CRC covers the first header_size - 2 bytes as
+// written and the CRC and the frames overwrite the rest; chunks running past file_size (where the reference would grow
+// the file) are refused (VGB_E_DATA).
+int32_t hca_write_header(const vgb_hca_info &h, bool masked, int ciph, const uint8_t *comment, size_t comment_len, bool blank,
+                         uint32_t volume_bits, int64_t file_size, std::vector<uint8_t> &out, int index)
 {
     if (h.header_size < 8 || h.header_size > 0xffff) return fail(VGB_E_ARG, "file %d: header_size %d", index, h.header_size);
-    out.assign((size_t)h.header_size + 64 + (comment ? std::strlen(comment) : 0), 0);
+    out.assign((size_t)h.header_size + 64 + comment_len, 0);
     uint8_t *p = out.data();
     auto id = [&](const char *s, int n) { for (int i = 0; i < n; i++) { uint8_t b = (uint8_t)s[i]; if (masked && b) b |= 0x80; p[i] = b; } p += n; };
     id("HCA\0", 4); be16(p, 0x0200); be16(p + 2, h.header_size); p += 4;
@@ -1342,16 +1419,29 @@ int32_t hca_build_header(const vgb_hca_info &h, bool masked, int key_type, const
     p[5] = (uint8_t)h.channel_config; p[6] = (uint8_t)h.total_band_count; p[7] = (uint8_t)h.base_band_count; p[8] = (uint8_t)h.stereo_band_count;
     p[9] = (uint8_t)h.bands_per_hfr_group; p += 12;
     if (h.looping) { id("loop", 4); be32(p, h.loop_start_frame); be32(p + 4, h.loop_end_frame); be16(p + 8, h.pre_loop_samples); be16(p + 10, h.post_loop_samples); p += 12; }
-    id("ciph", 4); be16(p, masked ? key_type : 0); p += 2;
+    id("ciph", 4); be16(p, ciph); p += 2;
     if (volume_bits != 0x3F800000u) { id("rva\0", 4); be32(p, (int32_t)volume_bits); p += 4; }
-    bool blank = true;  // string.IsNullOrWhiteSpace
-    if (comment) for (const char *c = comment; *c; c++) if (!std::strchr(" \t\n\r\v\f", *c)) blank = false;
     if (blank) id("pad", 3);
-    else { id("comm\0", 5); const size_t n = std::strlen(comment); std::memcpy(p, comment, n); p += n + 1; }
-    if (p - out.data() > h.header_size - 2) return fail(VGB_E_ARG, "file %d: header_size %d cannot hold the chunks (%d bytes)", index, h.header_size, (int)(p - out.data()) + 2);
+    else { id("comm\0", 5); std::memcpy(p, comment, comment_len); p += comment_len + 1; }
+    const int64_t end = p - out.data();
+    if (end > h.header_size - 2) {
+        if (file_size < 0) return fail(VGB_E_ARG, "file %d: header_size %d cannot hold the chunks (%d bytes)", index, h.header_size, (int)end + 2);
+        if (end > file_size)
+            return fail(VGB_E_DATA, "file %d: the header chunks (%lld bytes) run past the end of the %lld-byte file", index, (long long)end, (long long)file_size);
+    }
     out.resize((size_t)h.header_size);
     be16(out.data() + h.header_size - 2, crc16_host(out.data(), (size_t)h.header_size - 2));
     return VGB_OK;
+}
+// HcaWriter's header for the encoders' files: "ciph" is the key's type, the comment a C string judged blank by its ASCII
+// white space, and every chunk fits in header_size - 2 bytes
+int32_t hca_build_header(const vgb_hca_info &h, bool masked, int key_type, const char *comment, uint32_t volume_bits,
+                         std::vector<uint8_t> &out, int index)
+{
+    bool blank = true;  // string.IsNullOrWhiteSpace
+    if (comment) for (const char *c = comment; *c; c++) if (!std::strchr(" \t\n\r\v\f", *c)) blank = false;
+    return hca_write_header(h, masked, masked ? key_type : 0, reinterpret_cast<const uint8_t *>(comment), comment ? std::strlen(comment) : 0, blank,
+                            volume_bits, -1, out, index);
 }
 
 // CriHcaKey tables (Codecs/CriHca/CriHcaKey.cs:9-174)
