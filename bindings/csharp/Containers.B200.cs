@@ -120,6 +120,10 @@ namespace VGAudio.Native
         public int NwEndianness;            // 0 = the target's, 1 = little, 2 = big (BRSTM is always big)
         public int NwLoopPointAlignment;    // 0 = BytesToSamples(0x2000, codec)
         public int NwPad;
+        // AudioData.SetLoop on every source before any encode or write (Convert.cs:82-90): 0 keeps each file's loop,
+        // 1 (VGB_LOOP_SET, -l) loops every file over [LoopStart, LoopEnd), 2 (VGB_LOOP_CLEAR, --no-loop) clears it
+        public int LoopMode, LoopStart, LoopEnd;
+        public int LoopPad;
     }
 
     internal static unsafe class VgAudioB200Containers
@@ -178,6 +182,9 @@ namespace VGAudio.Native
         public static extern int vgb_hps_parse(byte* file, long length, VgbHpsInfo* info, VgbHpsBlock* blocks, int blockCapacity);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_idsp_hps_to_wave_batch(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_convert_to_wave_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
+            VgbAdxKey* adxKey, ulong* hcaKeyCode, long* outSizes, byte** filesOut, int* statusOut);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)] public static extern int vgb_gcadpcm_debug_decode_stats(ulong* output, int n);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_convert_wave_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, long* outSizes,
@@ -451,6 +458,26 @@ namespace VGAudio.Cli
         public static unsafe void ConvertIdspHpsToWave(string[] inPaths, int[] inTypes, string[] outPaths, Action<string> log, Action<int> reportAdd)
         {
             ConvertTypedToWave(inPaths, inTypes, outPaths, log, reportAdd, VgAudioB200Containers.vgb_convert_idsp_hps_to_wave_batch);
+        }
+
+        // The decode direction for a chunk of files of any readable container in one native call per pass, with the batch's
+        // -l / --no-loop: inTypes[i] names file i's reader (VGB_CONTAINER_DSP / _ADX / _HCA / _BRSTM .. _BFSTP / _IDSP /
+        // _HPS), options carries only the loop (LoopMode, LoopStart, LoopEnd; null keeps every file's loop), adxKey decrypts
+        // .adx files of revision 8 and 9 and hcaKeyCode "ciph" 56 .hca files.  A file whose loop its format's WithLoop
+        // refuses fails alone with the reference's message, as does a file the decoder refuses in the second pass.
+        // Like the rest of this file, ConvertToWave and the Loop* fields of VgbConvertOptions are not compiled or run by
+        // this repository's build or tests (no .NET toolchain); the struct layout follows vgb_convert_options field by field.
+        public static unsafe void ConvertToWave(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions? options, VgbAdxKey? adxKey,
+                                                ulong? hcaKeyCode, Action<string> log, Action<int> reportAdd)
+        {
+            ConvertTypedToWave(inPaths, inTypes, outPaths, log, reportAdd, (files, lengths, types, nFiles, outSizes, filesOut, statusOut) =>
+            {
+                VgbConvertOptions o = options ?? default;   // locals of the lambda: their addresses may be taken
+                VgbAdxKey k = adxKey ?? default;
+                ulong code = hcaKeyCode ?? 0;
+                return VgAudioB200Containers.vgb_convert_to_wave_batch(files, lengths, types, nFiles, options.HasValue ? &o : null,
+                    adxKey.HasValue ? &k : null, hcaKeyCode.HasValue ? &code : null, outSizes, filesOut, statusOut);
+            });
         }
 
         private unsafe delegate int TypedToWave(byte** files, long* lengths, int* inType, int nFiles, long* outSizes, byte** filesOut, int* statusOut);

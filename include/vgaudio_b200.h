@@ -757,14 +757,24 @@ typedef struct vgb_convert_options {
     int32_t nw_endianness;              /* 0 = the target's (BCSTM little, BFSTM big), 1 = little, 2 = big; BRSTM is always big */
     int32_t nw_loop_point_alignment;    /* 0 = BytesToSamples(0x2000, codec) (14336 for GC-ADPCM) */
     int32_t nw_pad;
+    /* AudioData.SetLoop on every source before any encode or write (the CLI's -l / --no-loop, Convert.cs:82-90):
+     * loop_mode 0 keeps each source's loop; VGB_LOOP_SET loops every file over [loop_start, loop_end); VGB_LOOP_CLEAR
+     * makes every file non-looping.  The source format's WithLoop rules decide per file (see vgb_convert_to_wave_batch).
+ * Any other loop_mode fails the whole call with VGB_E_ARG before a file is read, in every call that takes options. */
+    int32_t loop_mode, loop_start, loop_end, loop_pad;
 } vgb_convert_options;
+#define VGB_LOOP_SET   1
+#define VGB_LOOP_CLEAR 2
 /* Pass files_out == NULL for the sizing pass: out_sizes[i] = size of output i (0 for a file that failed), status_out[i]
  * (may be NULL) = VGB_OK or the error of file i - a bad file does not stop the batch (Batch.cs:39-43).  The sizing pass
  * runs on the host only and needs no device.  The second pass fills files_out[i] for every file whose status is VGB_OK.
  * cb receives the number of files finished (positive deltas summing to the good files).  With several devices bound
  * (vgb_init_devices) and at least two good files, the second pass is sharded: files weigh sample_count * channel_count
  * + 1024, every device converts its share in groups of its own (group_bytes = 0: an eighth of its share's input, 64..512
- * MiB), and an error of a device's share fails the call with " (device N)" appended to its message. */
+ * MiB), and an error of a device's share fails the call with " (device N)" appended to its message.  loop_mode sets or
+ * clears every WAVE file's loop (its smpl loop otherwise) before the encode, with the rules of vgb_convert_to_wave_batch;
+ * a file whose points WithLoop refuses fails alone, and the targets' own refusals then apply to the new loop (an empty
+ * loop is refused where the loop start must move, and by the .hca encoder). */
 int32_t vgb_convert_wave_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_convert_options *options,
                                int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
 /* The decode direction of the batch job: .dsp file images in, 16-bit WAVE file images out - DspReader (Containers/Dsp/DspReader.cs:15-127)
@@ -968,6 +978,27 @@ int32_t vgb_convert_nw_to_wave_batch(const uint8_t *const *files, const int64_t 
  * been written. */
 int32_t vgb_convert_idsp_hps_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                                            int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
+/* The decode direction of the batch job for every readable source in one call, with the batch's loop setting: in_type[i]
+ * names file i's reader (VGB_CONTAINER_DSP, _ADX, _HCA, _BRSTM ... _BFSTP, _IDSP, _HPS; any other value fails that file
+ * with VGB_E_ARG).  Each file is read, decoded and written exactly as by the one of vgb_convert_{dsp,adx,hca,nw,
+ * idsp_hps}_to_wave_batch that takes its in_type (same two-pass protocol, per-file status, sharding over the bound
+ * devices and fill-pass refusals; *adx_key and *hca_key_code as there, NULL for none), and with options NULL or
+ * loop_mode 0 its bytes are theirs.  Only the loop_* fields of *options are read: AudioData.SetLoop runs on the
+ * source's format before the WAVE is written (Convert.cs:82-90):
+ *   - VGB_LOOP_CLEAR (--no-loop): WithLoop(false), no smpl chunk.  An .hca file stays cut at its old loop end.
+ *   - VGB_LOOP_SET (-l loop_start-loop_end): WithLoop(true, s, e) (AudioFormatBaseBuilder.cs:23-58) against the sample
+ *     count ToPcm16 yields (the unaligned count for .adx, channel 0's row for PCM NintendoWare files), failing the file
+ *     with "Loop points must be less than the number of samples and non-negative." or "The loop end must be greater than
+ *     the loop start" (VGB_E_ARG); s == e is a loop.  An .hca file then refuses any points but its own ("Changing the
+ *     loop points on HCA audio without re-encoding is not supported.") and a loop it does not have ("Adding a loop to
+ *     HCA audio without re-encoding is not supported."), VGB_E_ARG.
+ * The same rules, at the same point of every source plan, drive vgb_convert_wave_batch (WAVE sources),
+ * vgb_transcode_batch and vgb_rewrite_batch through their options.  The files of each reader go through their own
+ * group loop, one reader after the other (.dsp last: a predictor outside 0..7 still fails the call).  Without
+ * status_out a fill-pass refusal fails the call (VGB_E_DATA) after the other files are written. */
+int32_t vgb_convert_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                                  const vgb_convert_options *options, const vgb_adx_key *adx_key, const uint64_t *hca_key_code,
+                                  int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
 /* Bookkeeping of the most recent time-parallel GC-ADPCM decode of vgb_convert_nw_to_wave_batch or
  * vgb_convert_idsp_hps_to_wave_batch on this thread's
  * context (its last group of files): out[0] segments per channel, [1] frames decoded by run-ons, [2] frames decoded by
@@ -990,7 +1021,9 @@ int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n);
  * converter, without the WAVE writer's limits), and the target's planning errors (as vgb_convert_wave_batch).
  * In the fill pass, an ADX frame with a filter the reference cannot index or an HCA frame the decoder refuses fails that
  * file alone (status_out entry, out_sizes[i] = 0, buffer not written; without status_out the call fails with VGB_E_DATA
- * after the other files are written), a GC-ADPCM predictor outside 0..7 fails the call (VGB_E_DATA). */
+ * after the other files are written), a GC-ADPCM predictor outside 0..7 fails the call (VGB_E_DATA).
+ * loop_mode sets or clears every source's loop on the source's format before the re-encode (vgb_convert_to_wave_batch's
+ * rules: an .hca source refuses new points and an added loop even here, as CriHcaFormatBuilder does). */
 int32_t vgb_transcode_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                             const vgb_convert_options *options, const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code,
                             int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
@@ -1032,7 +1065,11 @@ int32_t vgb_transcode_batch(const uint8_t *const *files, const int64_t *lengths,
  * without its key fails (the reference would pass the encrypted frames through, an .adx file even labelled with the
  * output's encryption byte); a comment that is not valid UTF-8 fails with VGB_E_DATA (the reference would write U+FFFD
  * in place of the bad bytes); HCA chunks that run past the end of the output file fail with VGB_E_DATA (the reference
- * would grow the file: only a tiny header_size with few frames can do that).  There is no device-side refusal. */
+ * would grow the file: only a tiny header_size with few frames can do that).  There is no device-side refusal.
+ * loop_mode sets or clears every source's loop with vgb_convert_to_wave_batch's rules: an .adx file gets the new
+ * (unaligned) points plus AlignmentSamples in its header and TrimFile cuts a looping file at the new loop end, shorter
+ * or longer than the source; an .hca file loses its loop chunk with VGB_LOOP_CLEAR (same header size and frames) and
+ * takes VGB_LOOP_SET only with its own points. */
 int32_t vgb_rewrite_batch(const uint8_t *const *files, const int64_t *lengths, int32_t n_files, const vgb_convert_options *options,
                           const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code, int64_t *out_sizes, uint8_t *const *files_out,
                           int32_t *status_out, vgb_progress_cb cb, void *user);

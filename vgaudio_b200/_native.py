@@ -177,7 +177,11 @@ class VgbConvertOptions(C.Structure):
                                          "adx_encryption_type", "adx_has_key", "adx_key_seed", "adx_key_mult", "adx_key_inc",
                                          "hca_quality", "hca_bitrate", "hca_limit_bitrate", "hca_key_type", "reserved")] + [
         ("hca_key_code", C.c_uint64), ("group_bytes", C.c_int64)] + [
-        (n, C.c_int32) for n in ("nw_codec_plus1", "nw_endianness", "nw_loop_point_alignment", "nw_pad")]
+        (n, C.c_int32) for n in ("nw_codec_plus1", "nw_endianness", "nw_loop_point_alignment", "nw_pad",
+                                 "loop_mode", "loop_start", "loop_end", "loop_pad")]
+
+
+VGB_LOOP_SET, VGB_LOOP_CLEAR = 1, 2  # vgb_convert_options.loop_mode (0 keeps every source's loop)
 
 
 PROGRESS_CB = C.CFUNCTYPE(None, C.c_void_p, C.c_int64)
@@ -311,6 +315,8 @@ SIGNATURES = {
     "vgb_hps_parse": (C.c_int32, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32]),
     "vgb_convert_idsp_hps_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                                        C.c_void_p]),
+    "vgb_convert_to_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p, C.c_void_p]),
     "vgb_gcadpcm_debug_decode_stats": (C.c_int32, [C.c_void_p, C.c_int32]),
     "vgb_convert_wave_batch": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p]),

@@ -12,7 +12,14 @@
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav, .bcstp and .bfstp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST] [--rewrite]
+//                 [-l <start>-<end> | --no-loop] [--loop-align N]
 //
+// -l <start>-<end> sets the loop of every file, --no-loop removes it (AudioData.SetLoop on each file as read, before any
+// encode or write, Convert.cs:82-90), in every direction: WAVE to any target, transcodes, --rewrite and --out-format wav
+// (vgb_convert_to_wave_batch).  A file whose format refuses the points fails alone with the reference's message: points
+// outside 0..sample count or an end below the start, and for .hca sources any points but the file's own or a loop the file
+// does not have (no re-encode can add one).  The key searches ignore them.  --loop-align N sets the loop point alignment
+// of the NintendoWare targets and, when N > 0, of .dsp output (CreateConfiguration.Dsp).
 // With --out-format dsp|adx|hca the inputs are the .wav / .wave files and the .dsp, .adx and .hca files in another codec
 // than the output's (a file already in the output's codec is not listed: the same codec would be a rewrite).
 // --rewrite, with --out-format adx|hca only, also lists the .adx (respectively .hca) inputs and rewrites them in their own
@@ -87,9 +94,40 @@ static int usage()
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S] [--rewrite]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key] [--hca-keys FILE]\n"
+                         "                     [-l <start-end>] [--no-loop]\n"
+                         "       -l <start-end>   Set the start and end loop points (zero-indexed samples) of every file\n"
+                         "       --no-loop        Sets the audio to not loop\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
                          "       .bfwav, .bcstp and .bfstp inputs\n");
     return 2;
+}
+
+// the reference's messages for a bad command line (CliArguments.cs: PrintWithUsage)
+static int usage(const char *why)
+{
+    std::fprintf(stderr, "%s\n", why);
+    return usage();
+}
+
+// int.TryParse with the default NumberStyles.Integer: white space around an optional sign and decimal digits, in range
+static bool parse_int(const std::string &t, int32_t &out)
+{
+    const char *ws = " \t\n\v\f\r";
+    const size_t a = t.find_first_not_of(ws), b = t.find_last_not_of(ws);
+    if (a == std::string::npos) return false;
+    std::string d = t.substr(a, b - a + 1);
+    bool neg = false;
+    if (d[0] == '+' || d[0] == '-') { neg = d[0] == '-'; d.erase(0, 1); }
+    if (d.empty() || d.find_first_not_of("0123456789") != std::string::npos) return false;
+    int64_t v = 0;
+    for (char c : d) {
+        v = v * 10 + (c - '0');
+        if (v > (int64_t)INT32_MAX + 1) return false;
+    }
+    if (neg) v = -v;
+    if (v < INT32_MIN || v > INT32_MAX) return false;
+    out = (int32_t)v;
+    return true;
 }
 
 // "0,1,3": comma-separated CUDA ordinals, at least one, repeats allowed
@@ -201,6 +239,20 @@ int main(int argc, char **argv)
         else if (a == "--chunk-mb") chunk_mb = (size_t)std::atoll(next());
         else if (a == "--devices") { if (!parse_devices(next(), devices)) return usage(); }
         else if (a == "--loop-align") opt.nw_loop_point_alignment = std::atoi(next());
+        else if (a == "-l") {  // CliArguments.cs:95-124
+            if (opt.loop_mode == VGB_LOOP_CLEAR) return usage("Can't set loop points while using --no-loop.");
+            if (i + 1 >= argc) return usage("No argument after -l switch.");
+            const std::string arg = argv[++i];
+            const size_t dash = arg.find('-');
+            if (dash == std::string::npos || arg.find('-', dash + 1) != std::string::npos)
+                return usage("-l switch requires two loop points in the format <start>-<end>.");
+            if (!parse_int(arg.substr(0, dash), opt.loop_start) || !parse_int(arg.substr(dash + 1), opt.loop_end))
+                return usage("Error parsing loop points.");
+            opt.loop_mode = VGB_LOOP_SET;
+        } else if (a == "--no-loop") {  // :125-134
+            if (opt.loop_mode == VGB_LOOP_SET) return usage("Can't set loop points while using --no-loop.");
+            opt.loop_mode = VGB_LOOP_CLEAR;
+        }
         else if (a == "--find-adx-key") find_key = true;
         else if (a == "--rewrite") rewrite = true;
         else if (a == "--hca-keys") hca_keys_path = next();
@@ -232,6 +284,8 @@ int main(int argc, char **argv)
     else if (fmt == "hps") opt.out_type = VGB_CONTAINER_HPS;
     else if (fmt == "hca") opt.out_type = VGB_CONTAINER_HCA;
     else if (!to_wave) return usage();
+    // CreateConfiguration.Dsp (src/VGAudio.Cli/CreateConfiguration.cs:49-52): a positive --loop-align aligns .dsp loops too
+    if (opt.out_type == VGB_CONTAINER_DSP && opt.nw_loop_point_alignment > 0) opt.dsp_loop_point_alignment = opt.nw_loop_point_alignment;
     if (rewrite && opt.out_type != VGB_CONTAINER_ADX && opt.out_type != VGB_CONTAINER_HCA) {
         std::fprintf(stderr, "--rewrite takes --out-format adx or hca\n");
         return 2;
@@ -375,15 +429,12 @@ int main(int argc, char **argv)
                 const uint64_t *hca_found = h >= 8 ? &hca_codes[(size_t)hca_row_key[h]] : nullptr;
                 const uint64_t *tx_hca_key = hca_found ? hca_found : have_in_code ? &in_key_code : nullptr;
                 if (part % 2) s = vgb_rewrite_batch(p.data(), l.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot, st.data(), nullptr, nullptr);
-                else if (h >= 8 && to_wave) s = vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, hca_found, sz.data(), ot, st.data());
-                else if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
-                else if (!to_wave) s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot,
-                                                           st.data(), nullptr, nullptr);
-                else if (h == 4) s = vgb_convert_nw_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
-                else if (h == 5) s = vgb_convert_idsp_hps_to_wave_batch(p.data(), l.data(), types.data(), m, sz.data(), ot, st.data());
-                else s = (h == 2 || adx_found) ? vgb_convert_adx_to_wave_batch(p.data(), l.data(), m, wave_adx_key, sz.data(), ot, st.data())
-                       : h == 1 ? vgb_convert_hca_to_wave_batch(p.data(), l.data(), m, have_code ? &key_code : nullptr, sz.data(), ot, st.data())
-                                : vgb_convert_dsp_to_wave_batch(p.data(), l.data(), m, sz.data(), ot, st.data());
+                else if (to_wave) {  // one reader per row; only the loop fields of opt are read
+                    const uint64_t *wave_hca_key = hca_found ? hca_found : have_code ? &key_code : nullptr;
+                    s = vgb_convert_to_wave_batch(p.data(), l.data(), types.data(), m, &opt, wave_adx_key, wave_hca_key, sz.data(), ot, st.data());
+                } else if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
+                else s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot,
+                                             st.data(), nullptr, nullptr);
                 if (s != VGB_OK) return s;
                 for (int32_t j = 0; j < m; j++) { out_size[r[j]] = sz[j]; status[r[j]] = st[j]; }
             }

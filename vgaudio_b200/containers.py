@@ -248,10 +248,18 @@ def hca_write_batch(infos: Sequence[N.VgbHcaInfo], frames: Sequence[np.ndarray],
 
 
 # ---- batch conversion (src/VGAudio.Cli/Batch.cs:11-51) -----------------------------------------------------------------
-def convert_options(out_type: int, **kw) -> N.VgbConvertOptions:
+def convert_options(out_type: int, loop: Optional[Tuple[int, int]] = None, no_loop: bool = False, **kw) -> N.VgbConvertOptions:
+    """Options of the batch converters.  loop=(start, end) sets every file's loop (the CLI's -l start-end), no_loop=True
+    clears it (--no-loop); neither keeps each source's loop.  The other keywords name vgb_convert_options fields."""
+    if loop is not None and no_loop:
+        raise ValueError("Can't set loop points while using --no-loop.")
     o = N.VgbConvertOptions()
     o.out_type = out_type
     o.hca_key_type = -1
+    if loop is not None:
+        o.loop_mode, o.loop_start, o.loop_end = N.VGB_LOOP_SET, int(loop[0]), int(loop[1])
+    elif no_loop:
+        o.loop_mode = N.VGB_LOOP_CLEAR
     for k, v in kw.items():
         if not hasattr(o, k):
             raise TypeError(f"unknown option {k}")
@@ -455,6 +463,19 @@ def convert_idsp_hps_to_wave_batch(files: Sequence, in_types: Sequence[int]) -> 
     types = (C.c_int32 * max(len(in_types), 1))(*in_types)
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_idsp_hps_to_wave_batch(
         ftab, lens, types, n, sizes, otab, st), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def convert_to_wave_batch(files: Sequence, in_types: Sequence[int], options: Optional[N.VgbConvertOptions] = None,
+                          adx_key: Optional[N.VgbAdxKey] = None, hca_key_code: Optional[int] = None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """The decode direction of the batch job for any readable images in one call (in_types: CONTAINER_* per file, naming
+    the reader), with the loop setting of options (convert_options(..., loop=(s, e)) or no_loop=True; only its loop
+    fields are read, None keeps every loop): ([WAVE bytes or None], [per-file status])."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    code = C.c_uint64(hca_key_code) if hca_key_code is not None else None
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_convert_to_wave_batch(
+        ftab, lens, types, n, C.byref(options) if options is not None else None, C.byref(adx_key) if adx_key is not None else None,
+        C.byref(code) if code is not None else None, sizes, otab, st), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
 
 
