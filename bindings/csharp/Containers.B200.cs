@@ -193,6 +193,9 @@ namespace VGAudio.Native
         public static extern int vgb_transcode_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
             VgbAdxKey* inAdxKey, ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_transcode_nw_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
+            VgbAdxKey* inAdxKey, ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_rewrite_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, VgbAdxKey* inAdxKey,
             ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
     }
@@ -536,7 +539,21 @@ namespace VGAudio.Cli
         // (1 / 2 / 3) for file i; a file already in options.OutType's codec fails alone (no rewrite is performed).
         // inAdxKey decrypts revision 8 / 9 .adx sources and inHcaKeyCode "ciph" 56 .hca sources; the output's key is in
         // options.  A file whose frames the decoder refuses fails in the second pass alone.
-        public static unsafe void Transcode(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
+        public static void Transcode(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
+            ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd) =>
+            Transcode(false, inPaths, inTypes, outPaths, options, inAdxKey, inHcaKeyCode, log, reportAdd);
+
+        // Coded files into a NintendoWare stream, IDSP or HPS file (`-b -i hca/ --out-format bfstm` and the like):
+        // options.OutType is VGB_CONTAINER_BRSTM / _BCSTM / _BFSTM / _IDSP / _HPS (4..8), inTypes and keys as in
+        // Transcode, the target's options (NwCodecPlus1, NwEndianness, NwLoopPointAlignment, NoTrim) as in ConvertWave.
+        // .adx and .hca sources are re-encoded; a .dsp source is taken into PCM16 / PCM8 only, and fails alone for a
+        // GC-ADPCM target (no rewrite is performed).
+        public static void TranscodeNw(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
+            ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd) =>
+            Transcode(true, inPaths, inTypes, outPaths, options, inAdxKey, inHcaKeyCode, log, reportAdd);
+
+        // nw: vgb_transcode_nw_batch, else vgb_transcode_batch
+        static unsafe void Transcode(bool nw, string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
             ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd)
         {
             int n = inPaths.Length;
@@ -557,7 +574,8 @@ namespace VGAudio.Cli
                 for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
                 fixed (int* types = inTypes)
                 {
-                    VgAudioB200.Check(VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero));
+                    VgAudioB200.Check(nw ? VgAudioB200Containers.vgb_transcode_nw_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero)
+                                         : VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero));
                     var outputs = new byte[n][];
                     for (int i = 0; i < n; i++)
                     {
@@ -568,7 +586,8 @@ namespace VGAudio.Cli
                         outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
                     }
                     VgbProgress cb = (user, delta) => reportAdd((int)delta);   // progress.ReportAdd(1) per file (Batch.cs:45)
-                    VgAudioB200.Check(VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero));
+                    VgAudioB200.Check(nw ? VgAudioB200Containers.vgb_transcode_nw_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero)
+                                         : VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero));
                     GC.KeepAlive(cb);
                     for (int i = 0; i < n; i++)
                     {

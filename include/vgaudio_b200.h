@@ -46,7 +46,7 @@ int32_t vgb_shutdown(void);
 /* Bind several devices (SURVEY §8b's vgb_init(n_devices, flags); the reference's counterpart is Parallel.ForEach over
  * files, src/VGAudio.Cli/Batch.cs:24-25).  devices[0] becomes the primary device (the one the *_dev entry points, timers
  * and debug taps use); every host-pointer codec *_batch call and every batch converter (vgb_convert_wave_batch,
- * vgb_convert_{dsp,hca,adx,nw,idsp_hps}_to_wave_batch, vgb_transcode_batch) are then sharded over all bound devices by greedy
+ * vgb_convert_{dsp,hca,adx,nw,idsp_hps}_to_wave_batch, vgb_transcode_batch, vgb_transcode_nw_batch) are then sharded over all bound devices by greedy
  * longest-first bin packing of the units' sample or frame counts - one worker thread and one H2D / kernel / D2H pipeline
  * per device, each over its own PCIe link, results written straight into the caller's arrays (no collective: host data
  * reaches a GPU fastest over that GPU's own link).  The single-shot container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.
@@ -716,7 +716,8 @@ int32_t vgb_hca_write_batch(const vgb_hca_info *info, int32_t n_files, const uin
 /* NintendoWare streams (BrstmWriter, BCFstmWriter with BxstmConfiguration's defaults: interleave 0x2000 bytes, a seek
  * entry every 0x2000 bytes' worth of samples, BRSTM standard track and seek-table types, BCSTM version 2.1, BFSTM
  * version 0.3, seek table and loop context recalculated).  vgb_convert_wave_batch writes them; vgb_transcode_batch does
- * not take them as a target; vgb_convert_nw_to_wave_batch reads them.  A looping GC-ADPCM file whose loop start is not
+ * not take them as a target; vgb_transcode_nw_batch writes them from .adx, .hca and (PCM16 / PCM8 only) .dsp sources;
+ * vgb_convert_nw_to_wave_batch reads them.  A looping GC-ADPCM file whose loop start is not
  * a multiple of the loop point alignment goes through GcAdpcmFormat.WithAlignment as in the reference: the loop moves
  * to the next multiple and the tail behind the kept frames is re-encoded on the device. */
 #define VGB_CONTAINER_BRSTM 4
@@ -725,7 +726,8 @@ int32_t vgb_hca_write_batch(const vgb_hca_info *info, int32_t n_files, const uin
 /* IDSP (IdspWriter with IdspConfiguration's default block size of 16 bytes: the loop start moves to a multiple of 28
  * samples, and no_trim maps to TrimFile as for .dsp) and HPS (HpsWriter: blocks of at most 0x10000 bytes, the loop start
  * moves to a multiple of one block's samples per channel), both GC-ADPCM only.  vgb_convert_wave_batch writes them;
- * vgb_transcode_batch does not take them as a target; the nw_* options are ignored.  Per-file refusals besides the
+ * vgb_transcode_batch does not take them as a target; vgb_transcode_nw_batch writes them from .adx and .hca sources;
+ * the nw_* options are ignored.  Per-file refusals besides the
  * usual ones (no samples, loop points GcAdpcmAlignment refuses, 2 GiB of output, more than 255 channels - this
  * converter's limit): an HPS file with 3, 7, 11 ... channels, whose block headers HpsWriter writes 0x20 bytes past the
  * block map's offsets; and an HPS file whose loop moved and that has a block starting more than one sample behind the
@@ -1027,6 +1029,20 @@ int32_t vgb_gcadpcm_debug_decode_stats(uint64_t *out, int32_t n);
 int32_t vgb_transcode_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                             const vgb_convert_options *options, const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code,
                             int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
+/* Transcoding in the batch job into the NintendoWare streams, IDSP and HPS: .dsp, .adx and .hca file images in,
+ * options->out_type (VGB_CONTAINER_BRSTM, _BCSTM, _BFSTM, _IDSP or _HPS; anything else fails the call with VGB_E_ARG)
+ * out.  The sources are read exactly as by vgb_transcode_batch (in_type, keys, loop_mode, what ToPcm16 yields); the
+ * target is planned and written exactly as by vgb_convert_wave_batch for the same PCM (nw_codec_plus1, nw_endianness,
+ * nw_loop_point_alignment, no_trim for IDSP): GC-ADPCM coefficients, encode, GcAdpcmFormat.WithAlignment of a loop start
+ * off the alignment, seek table, loop and block contexts, all on the device.  Same two-pass protocol, per-file status,
+ * progress, sharding and fill-pass failures as vgb_transcode_batch; options->group_bytes counts a file's decoded PCM plus,
+ * for GC-ADPCM, the full decode and ADPCM rows the target keeps resident, as vgb_convert_wave_batch counts it.
+ * Per-file errors of the sizing pass besides those of vgb_transcode_batch's sources and vgb_convert_wave_batch's
+ * targets: in_type not DSP / ADX / HCA, and a .dsp source into a GC-ADPCM target (IDSP, HPS, or NintendoWare without
+ * -f pcm16 / pcm8), where GetFormat<GcAdpcmFormat> hands back the source's own format: a rewrite, which is not performed. */
+int32_t vgb_transcode_nw_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                               const vgb_convert_options *options, const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code,
+                               int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
 /* Rewriting .adx or .hca files in their own codec without re-encoding: decrypted, re-keyed or left as they are
  * (Convert.ConvertFile with the same container on both sides: the reader decrypts the frames, AudioData.GetFormat<T>
  * hands the writer the source's own CriAdxFormat / CriHcaFormat, Formats/AudioData.cs:20-33, and the writer encrypts

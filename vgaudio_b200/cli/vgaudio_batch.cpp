@@ -1,18 +1,18 @@
 // vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
-// .dsp / .adx / .hca, WAVE files to .brstm / .bcstm / .bfstm / .idsp / .hps, and .dsp, .adx, .hca, .brstm, .bcstm, .bfstm,
+// .dsp / .adx / .hca, WAVE files (with --coded also .adx, .hca and .dsp files) to .brstm / .bcstm / .bfstm / .idsp / .hps, and .dsp, .adx, .hca, .brstm, .bcstm, .bfstm,
 // .idsp and .hps files, the NintendoWare wave files (.brwav / .rwav, .bcwav / .cwav / .bms, .bfwav) and prefetch
 // streams (.bcstp, .bfstp) to WAVE.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
 // reader -> encoder -> writer chain of a chunk of files runs as ONE coalesced call on the device per kind of input
-// (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch for coded files, vgb_convert_*_to_wave_batch for
+// (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch / vgb_transcode_nw_batch for coded files, vgb_convert_*_to_wave_batch for
 // --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav, .bcstp and .bfstp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST] [--rewrite]
-//                 [-l <start>-<end> | --no-loop] [--loop-align N]
+//                 [-l <start>-<end> | --no-loop] [--loop-align N] [--coded]
 //
 // -l <start>-<end> sets the loop of every file, --no-loop removes it (AudioData.SetLoop on each file as read, before any
 // encode or write, Convert.cs:82-90), in every direction: WAVE to any target, transcodes, --rewrite and --out-format wav
@@ -25,6 +25,10 @@
 // --rewrite, with --out-format adx|hca only, also lists the .adx (respectively .hca) inputs and rewrites them in their own
 // codec without re-encoding (vgb_rewrite_batch): decrypted with their input key and written in the clear, or re-keyed
 // with the output key; the encoder's options do not apply to them.
+// --coded, with --out-format brstm|bcstm|bfstm|idsp|hps only, also lists the .adx and .hca inputs, and with -f pcm16|pcm8
+// into brstm|bcstm|bfstm the .dsp inputs, and transcodes them on the device (vgb_transcode_nw_batch) with the same input
+// keys as the other transcodes.  Without it those targets take WAVE inputs only.  (A .dsp file into GC-ADPCM would be a
+// rewrite in its own codec, which is not performed.)
 // --keycode / --keystring are the output's key; --in-keycode N is the key of type-56 .hca inputs, and --in-keystring S,
 // or else --in-keycode N, the CriAdxKey of type-8 / type-9 .adx inputs.
 // With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
@@ -72,8 +76,8 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
 // the kind of an input file: 0 .dsp, 1 .hca, 2 .adx, 3 WAVE, 4 .brstm, 5 .bcstm, 6 .bfstm, 7 .idsp, 8 .hps, 9 .brwav /
 // .rwav, 10 .bcwav / .cwav / .bms, 11 .bfwav, 12 .bcstp, 13 .bfstp, -1 none of them (from 4 on, the kind is the
 // VGB_CONTAINER_* of its reader).  The extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs).
-// The NintendoWare, IDSP and HPS streams are decoded to WAVE with --out-format wav, and written from WAVE inputs only
-// with --out-format brstm|bcstm|bfstm|idsp|hps; the wave and prefetch files are decoded to WAVE only.  Another
+// The NintendoWare, IDSP and HPS streams are decoded to WAVE with --out-format wav, and written from WAVE inputs (with
+// --coded also from .adx, .hca and PCM-bound .dsp inputs) with --out-format brstm|bcstm|bfstm|idsp|hps; the wave and prefetch files are decoded to WAVE only.  Another
 // --out-format does not take them as inputs.
 static int kind_of(const fs::path &p)
 {
@@ -94,7 +98,7 @@ static int usage()
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S] [--rewrite]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key] [--hca-keys FILE]\n"
-                         "                     [-l <start-end>] [--no-loop]\n"
+                         "                     [-l <start-end>] [--no-loop] [--coded]\n"
                          "       -l <start-end>   Set the start and end loop points (zero-indexed samples) of every file\n"
                          "       --no-loop        Sets the audio to not loop\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
@@ -214,7 +218,7 @@ static bool find_adx_key(const std::vector<fs::path> &paths, int revision, vgb_a
 int main(int argc, char **argv)
 {
     std::string in_dir, out_dir, fmt, key_string, in_key_string, hca_keys_path;
-    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false;
+    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false, coded = false;
     uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
     std::vector<int32_t> devices;  // empty: device 0 through vgb_init
@@ -255,6 +259,7 @@ int main(int argc, char **argv)
         }
         else if (a == "--find-adx-key") find_key = true;
         else if (a == "--rewrite") rewrite = true;
+        else if (a == "--coded") coded = true;
         else if (a == "--hca-keys") hca_keys_path = next();
         else if (a == "--little-endian") opt.nw_endianness = 1;
         else if (a == "--big-endian") opt.nw_endianness = 2;
@@ -290,6 +295,11 @@ int main(int argc, char **argv)
         std::fprintf(stderr, "--rewrite takes --out-format adx or hca\n");
         return 2;
     }
+    const bool nw_out = opt.out_type >= VGB_CONTAINER_BRSTM;  // NintendoWare, IDSP and HPS targets
+    if (coded && !nw_out) {
+        std::fprintf(stderr, "--coded takes --out-format brstm, bcstm, bfstm, idsp or hps\n");
+        return 2;
+    }
     if ((opt.out_type == VGB_CONTAINER_IDSP || opt.out_type == VGB_CONTAINER_HPS) && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2)) {
         // CreateConfiguration.Idsp / .Hps (src/VGAudio.Cli/CreateConfiguration.cs:57-75, 103-115): GC-ADPCM only
         std::fprintf(stderr, "Can't use format %s with %s files\n", opt.nw_codec_plus1 == 2 ? "PCM16" : "PCM8",
@@ -321,15 +331,17 @@ int main(int argc, char **argv)
     std::map<int32_t, size_t> hca_key_files;  // key index -> files it decrypted
 
     // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca, .adx, NintendoWare, IDSP and HPS ones when decoding; else the WAVE
-    // ones and the coded ones in another codec than the output's, and with --rewrite those in the output's codec too)
+    // ones and the coded ones in another codec than the output's, and with --rewrite those in the output's codec too;
+    // the NintendoWare, IDSP and HPS targets take WAVE inputs, and with --coded .adx and .hca ones, and .dsp ones into PCM)
+    const bool nw_pcm = opt.out_type <= VGB_CONTAINER_BFSTM && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2);
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
         if (!e.is_regular_file()) return;
         const int kind = kind_of(e.path());
         if (kind < 0) return;
-        const bool nw_out = opt.out_type >= VGB_CONTAINER_BRSTM;  // NintendoWare, IDSP and HPS targets take WAVE inputs only
-        if (to_wave ? kind != 3 : (kind == 3 || (!nw_out && kind < 3 && (rewrite || kContainerOfKind[kind] != opt.out_type)))) files.push_back(e.path());
+        const bool coded_in = kind < 3 && (nw_out ? coded && (kind != 0 || nw_pcm) : rewrite || kContainerOfKind[kind] != opt.out_type);
+        if (to_wave ? kind != 3 : (kind == 3 || coded_in)) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -368,7 +380,8 @@ int main(int argc, char **argv)
         for (int k = 0; k < n; k++) { ptr[k] = in[k].data(); len[k] = (int64_t)in[k].size(); bytes_in += in[k].size(); }
         // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
         // codec (one for every NintendoWare reader, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
-        // and one transcode call for the coded ones (with --rewrite, one rewrite call for those in the output's codec)
+        // and one transcode call for the coded ones (vgb_transcode_nw_batch for the NintendoWare, IDSP and HPS targets; with
+        // --rewrite, one rewrite call for those in the output's codec)
         // rows 6 and 7: .adx files of revision 8 / 9 whose key --find-adx-key found, each revision with its own key
         // rows 8 and up: type-56 .hca files whose key --hca-keys found, one row per key (hca_row_key)
         std::vector<int32_t> hca_index(n, -1);
@@ -433,8 +446,8 @@ int main(int argc, char **argv)
                     const uint64_t *wave_hca_key = hca_found ? hca_found : have_code ? &key_code : nullptr;
                     s = vgb_convert_to_wave_batch(p.data(), l.data(), types.data(), m, &opt, wave_adx_key, wave_hca_key, sz.data(), ot, st.data());
                 } else if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
-                else s = vgb_transcode_batch(p.data(), l.data(), types.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot,
-                                             st.data(), nullptr, nullptr);
+                else s = (nw_out ? vgb_transcode_nw_batch : vgb_transcode_batch)(p.data(), l.data(), types.data(), m, &opt, tx_adx_key,
+                                                                               tx_hca_key, sz.data(), ot, st.data(), nullptr, nullptr);
                 if (s != VGB_OK) return s;
                 for (int32_t j = 0; j < m; j++) { out_size[r[j]] = sz[j]; status[r[j]] = st[j]; }
             }

@@ -14,9 +14,10 @@ import numpy as np
 from . import _native as N
 
 CONTAINER_DSP, CONTAINER_ADX, CONTAINER_HCA = 1, 2, 3
-CONTAINER_BRSTM, CONTAINER_BCSTM, CONTAINER_BFSTM = 4, 5, 6   # written by convert_wave_batch, read by convert_nw_to_wave_batch
-CONTAINER_IDSP, CONTAINER_HPS = 7, 8                          # GC-ADPCM only, written by convert_wave_batch,
-#                                                               read by convert_idsp_hps_to_wave_batch
+CONTAINER_BRSTM, CONTAINER_BCSTM, CONTAINER_BFSTM = 4, 5, 6   # written by convert_wave_batch and transcode_nw_batch,
+#                                                               read by convert_nw_to_wave_batch
+CONTAINER_IDSP, CONTAINER_HPS = 7, 8                          # GC-ADPCM only, written by convert_wave_batch and
+#                                                               transcode_nw_batch, read by convert_idsp_hps_to_wave_batch
 # NintendoWare wave files and prefetch streams, read only (nw_file_parse, convert_nw_to_wave_batch), named by the reader
 # the reference picks for the extension: .brwav/.rwav, .bcwav/.cwav/.bms, .bfwav, .bcstp, .bfstp
 CONTAINER_BRWAV, CONTAINER_BCWAV, CONTAINER_BFWAV, CONTAINER_BCSTP, CONTAINER_BFSTP = 9, 10, 11, 12, 13
@@ -488,6 +489,21 @@ def transcode_batch(files: Sequence, in_types: Sequence[int], options: N.VgbConv
     code = C.c_uint64(hca_key_code) if hca_key_code is not None else None
     cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
     outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_transcode_batch(
+        ftab, lens, types, n, C.byref(options), C.byref(adx_key) if adx_key is not None else None,
+        C.byref(code) if code is not None else None, sizes, otab, st, cb if otab is not None else None, None), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
+def transcode_nw_batch(files: Sequence, in_types: Sequence[int], options: N.VgbConvertOptions, adx_key: Optional[N.VgbAdxKey] = None,
+                       hca_key_code: Optional[int] = None, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """.adx / .hca images (and .dsp images into PCM16 / PCM8) in (in_types: CONTAINER_* per file), a NintendoWare stream,
+    IDSP or HPS file out (options.out_type: CONTAINER_BRSTM ... CONTAINER_HPS), decoded and re-encoded on the device:
+    ([output file bytes or None], [per-file status]).  Keys as in transcode_batch; the target's options (nw_codec_plus1,
+    nw_endianness, nw_loop_point_alignment, no_trim) as in convert_wave_batch."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    code = C.c_uint64(hca_key_code) if hca_key_code is not None else None
+    cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_transcode_nw_batch(
         ftab, lens, types, n, C.byref(options), C.byref(adx_key) if adx_key is not None else None,
         C.byref(code) if code is not None else None, sizes, otab, st, cb if otab is not None else None, None), files)
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
