@@ -196,6 +196,9 @@ namespace VGAudio.Native
         public static extern int vgb_transcode_nw_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
             VgbAdxKey* inAdxKey, ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
         [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
+        public static extern int vgb_transcode_from_nw_batch(byte** files, long* lengths, int* inType, int nFiles, VgbConvertOptions* options,
+            long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
+        [DllImport(Lib, CallingConvention = CallingConvention.Cdecl)]
         public static extern int vgb_rewrite_batch(byte** files, long* lengths, int nFiles, VgbConvertOptions* options, VgbAdxKey* inAdxKey,
             ulong* inHcaKeyCode, long* outSizes, byte** filesOut, int* statusOut, VgbProgress progress, IntPtr user);
     }
@@ -541,7 +544,7 @@ namespace VGAudio.Cli
         // options.  A file whose frames the decoder refuses fails in the second pass alone.
         public static void Transcode(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
             ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd) =>
-            Transcode(false, inPaths, inTypes, outPaths, options, inAdxKey, inHcaKeyCode, log, reportAdd);
+            Transcode(TxCall.Coded, inPaths, inTypes, outPaths, options, inAdxKey, inHcaKeyCode, log, reportAdd);
 
         // Coded files into a NintendoWare stream, IDSP or HPS file (`-b -i hca/ --out-format bfstm` and the like):
         // options.OutType is VGB_CONTAINER_BRSTM / _BCSTM / _BFSTM / _IDSP / _HPS (4..8), inTypes and keys as in
@@ -550,10 +553,28 @@ namespace VGAudio.Cli
         // GC-ADPCM target (no rewrite is performed).
         public static void TranscodeNw(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
             ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd) =>
-            Transcode(true, inPaths, inTypes, outPaths, options, inAdxKey, inHcaKeyCode, log, reportAdd);
+            Transcode(TxCall.IntoNw, inPaths, inTypes, outPaths, options, inAdxKey, inHcaKeyCode, log, reportAdd);
 
-        // nw: vgb_transcode_nw_batch, else vgb_transcode_batch
-        static unsafe void Transcode(bool nw, string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
+        // NintendoWare streams, wave and prefetch files, IDSP and HPS files into any coded target (`-b -i brstm/
+        // --out-format hca --nw-inputs` and the like): inTypes[i] is VGB_CONTAINER_BRSTM .. _BFSTP (4..13), options.OutType
+        // any of .dsp, .adx, .hca, .brstm, .bcstm, .bfstm, .idsp, .hps (1..8) with the target's options as in ConvertWave.
+        // None of these containers is encrypted, so there are no input keys.  A file already in the target's codec fails
+        // alone (no rewrite is performed); a file whose GC-ADPCM frames select a predictor outside 0..7 fails in the
+        // second pass alone.
+        public static void TranscodeFromNw(string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, Action<string> log,
+            Action<int> reportAdd) =>
+            Transcode(TxCall.FromNw, inPaths, inTypes, outPaths, options, null, null, log, reportAdd);
+
+        // vgb_transcode_batch, vgb_transcode_nw_batch or vgb_transcode_from_nw_batch
+        enum TxCall { Coded, IntoNw, FromNw }
+
+        static unsafe int TranscodeCall(TxCall call, byte** files, long* lengths, int* types, int n, VgbConvertOptions* options, VgbAdxKey* key,
+            ulong* code, long* outSizes, byte** filesOut, int* status, VgbProgress cb) =>
+            call == TxCall.FromNw ? VgAudioB200Containers.vgb_transcode_from_nw_batch(files, lengths, types, n, options, outSizes, filesOut, status, cb, IntPtr.Zero)
+            : call == TxCall.IntoNw ? VgAudioB200Containers.vgb_transcode_nw_batch(files, lengths, types, n, options, key, code, outSizes, filesOut, status, cb, IntPtr.Zero)
+            : VgAudioB200Containers.vgb_transcode_batch(files, lengths, types, n, options, key, code, outSizes, filesOut, status, cb, IntPtr.Zero);
+
+        static unsafe void Transcode(TxCall call, string[] inPaths, int[] inTypes, string[] outPaths, VgbConvertOptions options, VgbAdxKey? inAdxKey,
             ulong? inHcaKeyCode, Action<string> log, Action<int> reportAdd)
         {
             int n = inPaths.Length;
@@ -574,8 +595,7 @@ namespace VGAudio.Cli
                 for (int i = 0; i < n; i++) { inPtr[i] = (byte*)inPins[i].AddrOfPinnedObject(); len[i] = images[i].Length; }
                 fixed (int* types = inTypes)
                 {
-                    VgAudioB200.Check(nw ? VgAudioB200Containers.vgb_transcode_nw_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero)
-                                         : VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null, IntPtr.Zero));
+                    VgAudioB200.Check(TranscodeCall(call, inPtr, len, types, n, &options, keyPtr, codePtr, outSize, null, status, null));
                     var outputs = new byte[n][];
                     for (int i = 0; i < n; i++)
                     {
@@ -586,8 +606,7 @@ namespace VGAudio.Cli
                         outPtr[i] = (byte*)outPins[outPins.Count - 1].AddrOfPinnedObject();
                     }
                     VgbProgress cb = (user, delta) => reportAdd((int)delta);   // progress.ReportAdd(1) per file (Batch.cs:45)
-                    VgAudioB200.Check(nw ? VgAudioB200Containers.vgb_transcode_nw_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero)
-                                         : VgAudioB200Containers.vgb_transcode_batch(inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb, IntPtr.Zero));
+                    VgAudioB200.Check(TranscodeCall(call, inPtr, len, types, n, &options, keyPtr, codePtr, outSize, outPtr, status, cb));
                     GC.KeepAlive(cb);
                     for (int i = 0; i < n; i++)
                     {

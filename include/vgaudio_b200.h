@@ -46,7 +46,7 @@ int32_t vgb_shutdown(void);
 /* Bind several devices (SURVEY §8b's vgb_init(n_devices, flags); the reference's counterpart is Parallel.ForEach over
  * files, src/VGAudio.Cli/Batch.cs:24-25).  devices[0] becomes the primary device (the one the *_dev entry points, timers
  * and debug taps use); every host-pointer codec *_batch call and every batch converter (vgb_convert_wave_batch,
- * vgb_convert_{dsp,hca,adx,nw,idsp_hps}_to_wave_batch, vgb_transcode_batch, vgb_transcode_nw_batch) are then sharded over all bound devices by greedy
+ * vgb_convert_{dsp,hca,adx,nw,idsp_hps}_to_wave_batch, vgb_transcode_batch, vgb_transcode_nw_batch, vgb_transcode_from_nw_batch) are then sharded over all bound devices by greedy
  * longest-first bin packing of the units' sample or frame counts - one worker thread and one H2D / kernel / D2H pipeline
  * per device, each over its own PCIe link, results written straight into the caller's arrays (no collective: host data
  * reaches a GPU fastest over that GPU's own link).  The single-shot container calls (vgb_*_read_batch, vgb_*_write_batch, vgb_*_crypt_batch) stay on the primary.
@@ -1043,6 +1043,25 @@ int32_t vgb_transcode_batch(const uint8_t *const *files, const int64_t *lengths,
 int32_t vgb_transcode_nw_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                                const vgb_convert_options *options, const vgb_adx_key *in_adx_key, const uint64_t *in_hca_key_code,
                                int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out, vgb_progress_cb cb, void *user);
+/* Transcoding in the batch job from the NintendoWare streams, wave and prefetch files, IDSP and HPS: file images of
+ * in_type VGB_CONTAINER_BRSTM .. _BFSTP (4..13) in, options->out_type any of the eight coded targets (VGB_CONTAINER_DSP
+ * .. _HPS; anything else fails the call with VGB_E_ARG) out.  The sources are read exactly as by
+ * vgb_convert_to_wave_batch (the reader in_type names, loop_mode, what ToPcm16 yields: GC-ADPCM, or the header's PCM16 /
+ * PCM8); the target is planned and written exactly as by vgb_convert_wave_batch for the same PCM (the output key, ADX
+ * type / frame size / version, HCA quality / bitrate, nw_codec_plus1, nw_endianness, nw_loop_point_alignment, no_trim).
+ * None of these containers is encrypted: there are no input keys.  Same two-pass protocol, per-file status, progress,
+ * group_bytes and sharding over the bound devices as vgb_transcode_batch.
+ * A source whose codec is the target's (AudioData.GetFormat<T> hands back its own format) is a rewrite, which is not
+ * performed: GC-ADPCM into .dsp / IDSP / HPS / a NintendoWare stream without -f pcm16|pcm8, PCM16 into -f pcm16, PCM8
+ * into -f pcm8.  Per-file errors of the sizing pass, in this order: in_type outside 4..13; IDSP / HPS into a GC-ADPCM
+ * target (the rewrite message, before the file is read); the reader's and the loop setting's errors, as in
+ * vgb_convert_to_wave_batch; a NintendoWare file whose header's codec is the target's (the rewrite message); the
+ * target's errors, as in vgb_convert_wave_batch.  Fill pass: a GC-ADPCM frame header selecting a predictor outside 0..7
+ * fails its own file with VGB_E_DATA (an HCA target's encoder status of that file is not reported); without status_out
+ * the call then fails. */
+int32_t vgb_transcode_from_nw_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                                    const vgb_convert_options *options, int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out,
+                                    vgb_progress_cb cb, void *user);
 /* Rewriting .adx or .hca files in their own codec without re-encoding: decrypted, re-keyed or left as they are
  * (Convert.ConvertFile with the same container on both sides: the reader decrypts the frames, AudioData.GetFormat<T>
  * hands the writer the source's own CriAdxFormat / CriHcaFormat, Formats/AudioData.cs:20-33, and the writer encrypts

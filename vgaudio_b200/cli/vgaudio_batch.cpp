@@ -1,18 +1,18 @@
 // vgaudio_batch — batch conversion of a directory of audio files on the GPU: WAVE, .dsp, .adx and .hca files to
 // .dsp / .adx / .hca, WAVE files (with --coded also .adx, .hca and .dsp files) to .brstm / .bcstm / .bfstm / .idsp / .hps, and .dsp, .adx, .hca, .brstm, .bcstm, .bfstm,
 // .idsp and .hps files, the NintendoWare wave files (.brwav / .rwav, .bcwav / .cwav / .bms, .bfwav) and prefetch
-// streams (.bcstp, .bfstp) to WAVE.
+// streams (.bcstp, .bfstp) to WAVE; with --nw-inputs also the NintendoWare, IDSP and HPS files to any other codec.
 //
 // The counterpart of `VGAudioCli -b` (src/VGAudio.Cli/Batch.cs:11-51): the reference enumerates the input files and runs
 // Convert.ConvertFile on each from a Parallel.ForEach; here the host only reads and writes files, and every
 // reader -> encoder -> writer chain of a chunk of files runs as ONE coalesced call on the device per kind of input
-// (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch / vgb_transcode_nw_batch for coded files, vgb_convert_*_to_wave_batch for
+// (vgb_convert_wave_batch for WAVE files, vgb_transcode_batch / vgb_transcode_nw_batch / vgb_transcode_from_nw_batch for coded files, vgb_convert_*_to_wave_batch for
 // --out-format wav).  A file that fails is reported and skipped, like the reference's try/catch (:39-43).
 //
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav, .bcstp and .bfstp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST] [--rewrite]
-//                 [-l <start>-<end> | --no-loop] [--loop-align N] [--coded]
+//                 [-l <start>-<end> | --no-loop] [--loop-align N] [--coded] [--nw-inputs]
 //
 // -l <start>-<end> sets the loop of every file, --no-loop removes it (AudioData.SetLoop on each file as read, before any
 // encode or write, Convert.cs:82-90), in every direction: WAVE to any target, transcodes, --rewrite and --out-format wav
@@ -29,6 +29,11 @@
 // into brstm|bcstm|bfstm the .dsp inputs, and transcodes them on the device (vgb_transcode_nw_batch) with the same input
 // keys as the other transcodes.  Without it those targets take WAVE inputs only.  (A .dsp file into GC-ADPCM would be a
 // rewrite in its own codec, which is not performed.)
+// --nw-inputs, with any --out-format but wav, also lists the NintendoWare inputs (.brstm, .bcstm, .bfstm, .brwav, .rwav,
+// .bcwav, .cwav, .bms, .bfwav, .bcstp, .bfstp), and the .idsp and .hps inputs when the output is not GC-ADPCM (adx, hca,
+// or brstm|bcstm|bfstm with -f pcm16|pcm8), and transcodes them on the device (vgb_transcode_from_nw_batch).  A file
+// already in the output's codec (a GC-ADPCM stream into dsp, idsp, hps or GC-ADPCM NintendoWare, a PCM16 one into
+// -f pcm16, a PCM8 one into -f pcm8) is a rewrite, which is not performed: it is reported as a failed file.
 // --keycode / --keystring are the output's key; --in-keycode N is the key of type-56 .hca inputs, and --in-keystring S,
 // or else --in-keycode N, the CriAdxKey of type-8 / type-9 .adx inputs.
 // With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
@@ -77,8 +82,8 @@ static bool read_file(const fs::path &p, std::vector<uint8_t> &out)
 // .rwav, 10 .bcwav / .cwav / .bms, 11 .bfwav, 12 .bcstp, 13 .bfstp, -1 none of them (from 4 on, the kind is the
 // VGB_CONTAINER_* of its reader).  The extension picks the reader, as in the reference (src/VGAudio.Cli/ContainerTypes.cs).
 // The NintendoWare, IDSP and HPS streams are decoded to WAVE with --out-format wav, and written from WAVE inputs (with
-// --coded also from .adx, .hca and PCM-bound .dsp inputs) with --out-format brstm|bcstm|bfstm|idsp|hps; the wave and prefetch files are decoded to WAVE only.  Another
-// --out-format does not take them as inputs.
+// --coded also from .adx, .hca and PCM-bound .dsp inputs) with --out-format brstm|bcstm|bfstm|idsp|hps; the wave and
+// prefetch files are decoded to WAVE.  With --nw-inputs every coded --out-format also takes them as inputs.
 static int kind_of(const fs::path &p)
 {
     std::string ext = p.extension().string();
@@ -98,11 +103,13 @@ static int usage()
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S] [--rewrite]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key] [--hca-keys FILE]\n"
-                         "                     [-l <start-end>] [--no-loop] [--coded]\n"
+                         "                     [-l <start-end>] [--no-loop] [--coded] [--nw-inputs]\n"
                          "       -l <start-end>   Set the start and end loop points (zero-indexed samples) of every file\n"
                          "       --no-loop        Sets the audio to not loop\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
-                         "       .bfwav, .bcstp and .bfstp inputs\n");
+                         "       .bfwav, .bcstp and .bfstp inputs\n"
+                         "       --nw-inputs      Also transcode the .brstm, .bcstm, .bfstm, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav,\n"
+                         "                        .bcstp, .bfstp (and, into a codec other than GC-ADPCM, .idsp and .hps) inputs\n");
     return 2;
 }
 
@@ -218,7 +225,7 @@ static bool find_adx_key(const std::vector<fs::path> &paths, int revision, vgb_a
 int main(int argc, char **argv)
 {
     std::string in_dir, out_dir, fmt, key_string, in_key_string, hca_keys_path;
-    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false, coded = false;
+    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false, coded = false, nw_inputs = false;
     uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
     std::vector<int32_t> devices;  // empty: device 0 through vgb_init
@@ -260,6 +267,7 @@ int main(int argc, char **argv)
         else if (a == "--find-adx-key") find_key = true;
         else if (a == "--rewrite") rewrite = true;
         else if (a == "--coded") coded = true;
+        else if (a == "--nw-inputs") nw_inputs = true;
         else if (a == "--hca-keys") hca_keys_path = next();
         else if (a == "--little-endian") opt.nw_endianness = 1;
         else if (a == "--big-endian") opt.nw_endianness = 2;
@@ -300,6 +308,10 @@ int main(int argc, char **argv)
         std::fprintf(stderr, "--coded takes --out-format brstm, bcstm, bfstm, idsp or hps\n");
         return 2;
     }
+    if (nw_inputs && to_wave) {
+        std::fprintf(stderr, "--nw-inputs takes --out-format dsp, adx, hca, brstm, bcstm, bfstm, idsp or hps\n");
+        return 2;
+    }
     if ((opt.out_type == VGB_CONTAINER_IDSP || opt.out_type == VGB_CONTAINER_HPS) && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2)) {
         // CreateConfiguration.Idsp / .Hps (src/VGAudio.Cli/CreateConfiguration.cs:57-75, 103-115): GC-ADPCM only
         std::fprintf(stderr, "Can't use format %s with %s files\n", opt.nw_codec_plus1 == 2 ? "PCM16" : "PCM8",
@@ -332,8 +344,11 @@ int main(int argc, char **argv)
 
     // Batch.cs:16-19: the files of the input directory (here: the .dsp, .hca, .adx, NintendoWare, IDSP and HPS ones when decoding; else the WAVE
     // ones and the coded ones in another codec than the output's, and with --rewrite those in the output's codec too;
-    // the NintendoWare, IDSP and HPS targets take WAVE inputs, and with --coded .adx and .hca ones, and .dsp ones into PCM)
+    // the NintendoWare, IDSP and HPS targets take WAVE inputs, and with --coded .adx and .hca ones, and .dsp ones into PCM;
+    // with --nw-inputs every target also takes the NintendoWare inputs, and the IDSP and HPS ones into another codec than
+    // GC-ADPCM, the only codec they hold)
     const bool nw_pcm = opt.out_type <= VGB_CONTAINER_BFSTM && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2);
+    const bool gc_out = opt.out_type == VGB_CONTAINER_DSP || opt.out_type >= VGB_CONTAINER_IDSP || (nw_out && !nw_pcm);
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
@@ -341,7 +356,8 @@ int main(int argc, char **argv)
         const int kind = kind_of(e.path());
         if (kind < 0) return;
         const bool coded_in = kind < 3 && (nw_out ? coded && (kind != 0 || nw_pcm) : rewrite || kContainerOfKind[kind] != opt.out_type);
-        if (to_wave ? kind != 3 : (kind == 3 || coded_in)) files.push_back(e.path());
+        const bool nw_in = nw_inputs && kind > 3 && ((kind != VGB_CONTAINER_IDSP && kind != VGB_CONTAINER_HPS) || !gc_out);
+        if (to_wave ? kind != 3 : (kind == 3 || coded_in || nw_in)) files.push_back(e.path());
     };
     if (recurse) for (auto &e : fs::recursive_directory_iterator(in_dir, ec)) take(e);
     else for (auto &e : fs::directory_iterator(in_dir, ec)) take(e);
@@ -381,7 +397,8 @@ int main(int argc, char **argv)
         // every kind of input goes to its own call, each on its rows of the chunk's tables: decoding, one converter per
         // codec (one for every NintendoWare reader, one for IDSP and HPS); encoding, the WAVE converter for WAVE files
         // and one transcode call for the coded ones (vgb_transcode_nw_batch for the NintendoWare, IDSP and HPS targets; with
-        // --rewrite, one rewrite call for those in the output's codec)
+        // --rewrite, one rewrite call for those in the output's codec), and row 4 for the NintendoWare, IDSP and HPS inputs
+        // (vgb_transcode_from_nw_batch)
         // rows 6 and 7: .adx files of revision 8 / 9 whose key --find-adx-key found, each revision with its own key
         // rows 8 and up: type-56 .hca files whose key --hca-keys found, one row per key (hca_row_key)
         std::vector<int32_t> hca_index(n, -1);
@@ -409,7 +426,7 @@ int main(int argc, char **argv)
                 rows[row].push_back(k);
                 hca_key_files[hca_index[k]]++;
             } else if ((rev == 8 || rev == 9) && have_found[rev - 8]) rows[rev - 2].push_back(k);
-            else rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : (kind == 3 ? 3 : 0)].push_back(k);
+            else rows[to_wave ? ((kind == 7 || kind == 8) ? 5 : std::min(kind, 4)) : kind > 3 ? 4 : (kind == 3 ? 3 : 0)].push_back(k);
         }
         auto convert = [&](uint8_t *const *outs) -> int32_t {
             for (int part = 0; part < (int)rows.size() * 2; part++) {
@@ -446,6 +463,7 @@ int main(int argc, char **argv)
                     const uint64_t *wave_hca_key = hca_found ? hca_found : have_code ? &key_code : nullptr;
                     s = vgb_convert_to_wave_batch(p.data(), l.data(), types.data(), m, &opt, wave_adx_key, wave_hca_key, sz.data(), ot, st.data());
                 } else if (h == 3) s = vgb_convert_wave_batch(p.data(), l.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
+                else if (h == 4) s = vgb_transcode_from_nw_batch(p.data(), l.data(), types.data(), m, &opt, sz.data(), ot, st.data(), nullptr, nullptr);
                 else s = (nw_out ? vgb_transcode_nw_batch : vgb_transcode_batch)(p.data(), l.data(), types.data(), m, &opt, tx_adx_key,
                                                                                tx_hca_key, sz.data(), ot, st.data(), nullptr, nullptr);
                 if (s != VGB_OK) return s;

@@ -509,6 +509,19 @@ def transcode_nw_batch(files: Sequence, in_types: Sequence[int], options: N.VgbC
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
 
 
+def transcode_from_nw_batch(files: Sequence, in_types: Sequence[int], options: N.VgbConvertOptions,
+                            progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """NintendoWare stream, wave / prefetch, IDSP and HPS images in (in_types: CONTAINER_BRSTM ... CONTAINER_BFSTP per
+    file), any coded container out (options.out_type: CONTAINER_DSP ... CONTAINER_HPS), decoded and re-encoded or written
+    on the device: ([output file bytes or None], [per-file status]).  No input keys (none of these containers is
+    encrypted); the target's options as in convert_wave_batch.  A file already in the target's codec fails alone."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    cb = N.PROGRESS_CB(lambda user, delta: progress(delta)) if progress else None
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_transcode_from_nw_batch(
+        ftab, lens, types, n, C.byref(options), sizes, otab, st, cb if otab is not None else None, None), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
 def rewrite_batch(files: Sequence, options: N.VgbConvertOptions, adx_key: Optional[N.VgbAdxKey] = None,
                   hca_key_code: Optional[int] = None, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
     """.adx or .hca images rewritten in their own codec without re-encoding (options.out_type, CONTAINER_ADX or
