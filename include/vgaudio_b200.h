@@ -996,7 +996,7 @@ int32_t vgb_convert_idsp_hps_to_wave_batch(const uint8_t *const *files, const in
  *     HCA audio without re-encoding is not supported."), VGB_E_ARG.
  * The same rules, at the same point of every source plan, drive vgb_convert_wave_batch (WAVE sources),
  * vgb_transcode_batch and vgb_rewrite_batch through their options.  The files of each reader go through their own
- * group loop, one reader after the other (.dsp last: a predictor outside 0..7 still fails the call).  Without
+ * groups, .dsp last (a predictor outside 0..7 still fails the call).  Without
  * status_out a fill-pass refusal fails the call (VGB_E_DATA) after the other files are written. */
 int32_t vgb_convert_to_wave_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                                   const vgb_convert_options *options, const vgb_adx_key *adx_key, const uint64_t *hca_key_code,

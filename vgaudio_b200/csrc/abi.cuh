@@ -313,7 +313,7 @@ std::vector<std::vector<int>> shard_units(int n, Size size, int64_t extra)
 {
     std::vector<int> order(n);
     std::vector<int64_t> weight(n);
-    for (int i = 0; i < n; i++) { order[i] = i; weight[i] = (int64_t)std::max<int32_t>(size(i), 0) + extra; }
+    for (int i = 0; i < n; i++) { order[i] = i; weight[i] = std::max<int64_t>(size(i), 0) + extra; }
     std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return weight[a] > weight[b]; });
     const int n_dev = 1 + (int)g_extra.size();
     std::vector<int64_t> load(n_dev, 0);
