@@ -1062,6 +1062,25 @@ int32_t vgb_transcode_nw_batch(const uint8_t *const *files, const int64_t *lengt
 int32_t vgb_transcode_from_nw_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
                                     const vgb_convert_options *options, int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out,
                                     vgb_progress_cb cb, void *user);
+/* Rewriting .dsp files into BRSTM, BCSTM, BFSTM, IDSP or HPS without re-encoding (DspReader -> GetFormat<GcAdpcmFormat>
+ * hands the writer the source's own ADPCM, Formats/AudioData.cs:20-33).  in_type[i] must be VGB_CONTAINER_DSP (any other
+ * value fails that file with VGB_E_ARG); options->out_type is VGB_CONTAINER_BRSTM .. _HPS and nw_codec_plus1 is 0 or 3
+ * (GC-ADPCM), else the call fails with VGB_E_ARG.  The loop setting, nw_endianness, nw_loop_point_alignment and no_trim
+ * mean what they mean in vgb_convert_wave_batch; the sizes and per-file refusals of the sizing pass are those of
+ * vgb_convert_to_wave_batch's .dsp reader and loop setting, then vgb_convert_wave_batch's target for the same PCM
+ * description (an HPS file keeps its refusals, except the history read past the unaligned decode when the writer's
+ * channels hold no decode: there HpsWriter writes history 0).  Same two-pass protocol, per-file status and sharding over
+ * the bound devices as vgb_transcode_batch (no progress callback; group_bytes as there).
+ * Every ADPCM byte is copied except the loop tail GcAdpcmAlignment re-encodes when the loop start is not a multiple of
+ * the target's alignment.  The output keeps each channel's coefficients, gain and start history (the start
+ * predictor/scale is the first ADPCM byte, GcAdpcmChannel.cs:44).  The NintendoWare and HPS writers recalculate the loop
+ * context from a decode (history 0) at the unaligned loop start, as does the NintendoWare seek table; IDSP keeps the
+ * header's loop context verbatim when the file is read and written with the header's loop start
+ * (GcAdpcmChannelBuilder.PreviousLoopContextIsValid), and decodes it otherwise (-l, --no-loop on a looping file).  Fill
+ * pass: a frame header selecting a predictor outside 0..7 fails its own file with VGB_E_DATA; without status_out the
+ * call then fails. */
+int32_t vgb_rewrite_gc_batch(const uint8_t *const *files, const int64_t *lengths, const int32_t *in_type, int32_t n_files,
+                             const vgb_convert_options *options, int64_t *out_sizes, uint8_t *const *files_out, int32_t *status_out);
 /* Rewriting .adx or .hca files in their own codec without re-encoding: decrypted, re-keyed or left as they are
  * (Convert.ConvertFile with the same container on both sides: the reader decrypts the frames, AudioData.GetFormat<T>
  * hands the writer the source's own CriAdxFormat / CriHcaFormat, Formats/AudioData.cs:20-33, and the writer encrypts

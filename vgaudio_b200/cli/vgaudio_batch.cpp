@@ -12,7 +12,7 @@
 //   vgaudio_batch -i <indir> -o <outdir> --out-format dsp|adx|hca|brstm|bcstm|bfstm|idsp|hps|wav [-r]   (wav: .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav, .bcstp and .bfstp inputs are decoded) [--no-trim] [--hcaquality Highest|High|Middle|Low|Lowest]
 //                 [--bitrate N] [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S]
 //                 [--adxtype Linear|Fixed|Exp|ExpEnc...] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST] [--rewrite]
-//                 [-l <start>-<end> | --no-loop] [--loop-align N] [--coded] [--nw-inputs]
+//                 [-l <start>-<end> | --no-loop] [--loop-align N] [--coded] [--nw-inputs] [--keep-codec]
 //
 // -l <start>-<end> sets the loop of every file, --no-loop removes it (AudioData.SetLoop on each file as read, before any
 // encode or write, Convert.cs:82-90), in every direction: WAVE to any target, transcodes, --rewrite and --out-format wav
@@ -34,6 +34,9 @@
 // or brstm|bcstm|bfstm with -f pcm16|pcm8), and transcodes them on the device (vgb_transcode_from_nw_batch).  A file
 // already in the output's codec (a GC-ADPCM stream into dsp, idsp, hps or GC-ADPCM NintendoWare, a PCM16 one into
 // -f pcm16, a PCM8 one into -f pcm8) is a rewrite, which is not performed: it is reported as a failed file.
+// --keep-codec, with --out-format brstm|bcstm|bfstm|idsp|hps into GC-ADPCM only, also lists the .dsp inputs and rewrites
+// them into the output's container without re-encoding (vgb_rewrite_gc_batch): the source's ADPCM is copied, only a loop
+// tail that the target's alignment moves is re-encoded.
 // --keycode / --keystring are the output's key; --in-keycode N is the key of type-56 .hca inputs, and --in-keystring S,
 // or else --in-keycode N, the CriAdxKey of type-8 / type-9 .adx inputs.
 // With --out-format wav, --keycode N is the key of type-56 .hca files (HcaReader.FindKey), and --keystring S, or else
@@ -103,13 +106,14 @@ static int usage()
                          "                     [--limit-bitrate] [--keycode N] [--keystring S] [--in-keycode N] [--in-keystring S] [--rewrite]\n"
                          "                     [--adxtype linear|fixed|exp] [--framesize N] [--version 3|4] [--chunk-mb N] [--devices LIST]\n"
                          "                     [-f gcadpcm|pcm16|pcm8] [--loop-align N] [--little-endian|--big-endian] [--find-adx-key] [--hca-keys FILE]\n"
-                         "                     [-l <start-end>] [--no-loop] [--coded] [--nw-inputs]\n"
+                         "                     [-l <start-end>] [--no-loop] [--coded] [--nw-inputs] [--keep-codec]\n"
                          "       -l <start-end>   Set the start and end loop points (zero-indexed samples) of every file\n"
                          "       --no-loop        Sets the audio to not loop\n"
                          "       wav decodes .dsp, .hca, .adx, .brstm, .bcstm, .bfstm, .idsp, .hps, .brwav, .rwav, .bcwav, .cwav, .bms,\n"
                          "       .bfwav, .bcstp and .bfstp inputs\n"
                          "       --nw-inputs      Also transcode the .brstm, .bcstm, .bfstm, .brwav, .rwav, .bcwav, .cwav, .bms, .bfwav,\n"
-                         "                        .bcstp, .bfstp (and, into a codec other than GC-ADPCM, .idsp and .hps) inputs\n");
+                         "                        .bcstp, .bfstp (and, into a codec other than GC-ADPCM, .idsp and .hps) inputs\n"
+                         "       --keep-codec     Also rewrite the .dsp inputs into brstm, bcstm, bfstm, idsp or hps without re-encoding\n");
     return 2;
 }
 
@@ -225,7 +229,8 @@ static bool find_adx_key(const std::vector<fs::path> &paths, int revision, vgb_a
 int main(int argc, char **argv)
 {
     std::string in_dir, out_dir, fmt, key_string, in_key_string, hca_keys_path;
-    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false, coded = false, nw_inputs = false;
+    bool recurse = false, have_code = false, have_in_code = false, find_key = false, rewrite = false, coded = false, nw_inputs = false,
+         keep_codec = false;
     uint64_t key_code = 0, in_key_code = 0;
     size_t chunk_mb = 1024;
     std::vector<int32_t> devices;  // empty: device 0 through vgb_init
@@ -268,6 +273,7 @@ int main(int argc, char **argv)
         else if (a == "--rewrite") rewrite = true;
         else if (a == "--coded") coded = true;
         else if (a == "--nw-inputs") nw_inputs = true;
+        else if (a == "--keep-codec") keep_codec = true;
         else if (a == "--hca-keys") hca_keys_path = next();
         else if (a == "--little-endian") opt.nw_endianness = 1;
         else if (a == "--big-endian") opt.nw_endianness = 2;
@@ -349,13 +355,18 @@ int main(int argc, char **argv)
     // GC-ADPCM, the only codec they hold)
     const bool nw_pcm = opt.out_type <= VGB_CONTAINER_BFSTM && (opt.nw_codec_plus1 == 1 || opt.nw_codec_plus1 == 2);
     const bool gc_out = opt.out_type == VGB_CONTAINER_DSP || opt.out_type >= VGB_CONTAINER_IDSP || (nw_out && !nw_pcm);
+    if (keep_codec && (!nw_out || nw_pcm)) {
+        std::fprintf(stderr, "--keep-codec takes --out-format brstm, bcstm, bfstm, idsp or hps in GC-ADPCM\n");
+        return 2;
+    }
     std::vector<fs::path> files;
     std::error_code ec;
     auto take = [&](const fs::directory_entry &e) {
         if (!e.is_regular_file()) return;
         const int kind = kind_of(e.path());
         if (kind < 0) return;
-        const bool coded_in = kind < 3 && (nw_out ? coded && (kind != 0 || nw_pcm) : rewrite || kContainerOfKind[kind] != opt.out_type);
+        const bool coded_in = kind < 3 && (nw_out ? (coded && (kind != 0 || nw_pcm)) || (keep_codec && kind == 0)
+                                                  : rewrite || kContainerOfKind[kind] != opt.out_type);
         const bool nw_in = nw_inputs && kind > 3 && ((kind != VGB_CONTAINER_IDSP && kind != VGB_CONTAINER_HPS) || !gc_out);
         if (to_wave ? kind != 3 : (kind == 3 || coded_in || nw_in)) files.push_back(e.path());
     };
@@ -431,12 +442,12 @@ int main(int argc, char **argv)
         auto convert = [&](uint8_t *const *outs) -> int32_t {
             for (int part = 0; part < (int)rows.size() * 2; part++) {
                 // every row splits into the files in another codec than the output's (part even) and, transcoding, the
-                // ones in the output's own codec (part odd), which only --rewrite lists
+                // ones in the output's own codec (part odd), which only --rewrite (.adx, .hca) and --keep-codec (.dsp) list
                 const int h = part / 2;
                 std::vector<int32_t> r;
                 for (int32_t k : rows[h]) {
                     const int kind = kind_of(files[first + k]);
-                    const bool same = !to_wave && h != 3 && kind < 3 && kContainerOfKind[kind] == opt.out_type;
+                    const bool same = !to_wave && h != 3 && kind < 3 && (kContainerOfKind[kind] == opt.out_type || (keep_codec && kind == 0));
                     if (same == (part % 2 == 1)) r.push_back(k);
                 }
                 if (r.empty()) continue;
@@ -458,7 +469,8 @@ int main(int argc, char **argv)
                 const vgb_adx_key *tx_adx_key = adx_found ? &found[h - 6] : have_in_adx_key ? &in_adx_key : nullptr;
                 const uint64_t *hca_found = h >= 8 ? &hca_codes[(size_t)hca_row_key[h]] : nullptr;
                 const uint64_t *tx_hca_key = hca_found ? hca_found : have_in_code ? &in_key_code : nullptr;
-                if (part % 2) s = vgb_rewrite_batch(p.data(), l.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot, st.data(), nullptr, nullptr);
+                if (part % 2 && keep_codec) s = vgb_rewrite_gc_batch(p.data(), l.data(), types.data(), m, &opt, sz.data(), ot, st.data());
+                else if (part % 2) s = vgb_rewrite_batch(p.data(), l.data(), m, &opt, tx_adx_key, tx_hca_key, sz.data(), ot, st.data(), nullptr, nullptr);
                 else if (to_wave) {  // one reader per row; only the loop fields of opt are read
                     const uint64_t *wave_hca_key = hca_found ? hca_found : have_code ? &key_code : nullptr;
                     s = vgb_convert_to_wave_batch(p.data(), l.data(), types.data(), m, &opt, wave_adx_key, wave_hca_key, sz.data(), ot, st.data());

@@ -522,6 +522,17 @@ def transcode_from_nw_batch(files: Sequence, in_types: Sequence[int], options: N
     return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
 
 
+def rewrite_gc_batch(files: Sequence, in_types: Sequence[int], options: N.VgbConvertOptions) -> Tuple[List[Optional[np.ndarray]], List[int]]:
+    """.dsp images (in_types: CONTAINER_DSP per file) rewritten into a GC-ADPCM container (options.out_type:
+    CONTAINER_BRSTM ... CONTAINER_HPS) without re-encoding: the source's ADPCM is copied, only a loop tail that
+    alignment moves is re-encoded.  ([output file bytes or None], [per-file status]); the target's options as in
+    convert_wave_batch (nw_codec_plus1 0 or GC-ADPCM)."""
+    types = (C.c_int32 * max(len(in_types), 1))(*in_types)
+    outs, status = _convert(lambda ftab, lens, n, sizes, otab, st: N.lib.vgb_rewrite_gc_batch(
+        ftab, lens, types, n, C.byref(options), sizes, otab, st), files)
+    return [o if s == 0 else None for o, s in zip(outs, status)], status  # the fill pass may refuse a file's frames
+
+
 def rewrite_batch(files: Sequence, options: N.VgbConvertOptions, adx_key: Optional[N.VgbAdxKey] = None,
                   hca_key_code: Optional[int] = None, progress=None) -> Tuple[List[Optional[np.ndarray]], List[int]]:
     """.adx or .hca images rewritten in their own codec without re-encoding (options.out_type, CONTAINER_ADX or

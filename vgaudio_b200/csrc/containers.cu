@@ -584,7 +584,8 @@ struct NwChan {
     int64_t row_off;         // GC-ADPCM: bytes into the ADPCM slab (multiple of 16); PCM: samples into the PCM slab (multiple of 8)
     int64_t pcm_off;         // GC-ADPCM: samples into the decoded-PCM slab (the channel decoded in full)
     int64_t tail_off;        // GC-ADPCM, aligned loop: bytes of the re-encoded tail into the tail slab (multiple of 16)
-    int32_t coef_index, pad;
+    int32_t coef_index;
+    int32_t start_hist;      // GC-ADPCM: the start context's Hist1 | Hist2 << 16 (0 for an encoded channel; a rewrite keeps the source's)
 };
 struct NwFile {
     int64_t out_off;         // bytes into the output slab (multiple of 16)
@@ -641,8 +642,8 @@ __global__ void __launch_bounds__(256) nw_assemble_kernel(const NwFile *__restri
             int v = 0;
             switch (loop_ctx ? k - 3 : k % 3) {
             case 0: v = loop_ctx ? adpcm[cc.row_off + (int64_t)(ls / kGcFrameSamples) * kGcFrameBytes] : adpcm[cc.row_off]; break;
-            case 1: v = loop_ctx && ls >= 1 ? decoded[cc.pcm_off + ls - 1] : 0; break;
-            default: v = loop_ctx && ls >= 2 ? decoded[cc.pcm_off + ls - 2] : 0; break;
+            case 1: v = loop_ctx ? (ls >= 1 ? decoded[cc.pcm_off + ls - 1] : 0) : (int16_t)(cc.start_hist & 0xffff); break;
+            default: v = loop_ctx ? (ls >= 2 ? decoded[cc.pcm_off + ls - 2] : 0) : (int16_t)((uint32_t)cc.start_hist >> 16); break;
             }
             put16(info + f.ctx_off + 2 * k, v, be);
         }
@@ -718,7 +719,7 @@ struct IdspFile {
     int32_t in_size;         // bytes of each channel's array
     int32_t keep_bytes;      // bytes of that array taken from the encoded row
     int32_t data_size;       // AudioDataSize (a multiple of the 16-byte interleave)
-    int32_t ctx_loop_start;  // where the loop context is taken (the unaligned loop start); 0: the context stays (0, 0, 0)
+    int32_t ctx_loop_start;  // where the loop context is taken (the unaligned loop start); -1: the header blob's context stays
     int32_t tile_first;
 };
 struct HpsBlock {
@@ -735,7 +736,8 @@ struct HpsFile {
     int32_t block_hdr;       // bytes in front of a block's audio: GetNextMultiple(12 + 8 * channels, 0x20)
     int32_t first_block, n_blocks;
     int32_t file_size;
-    int32_t tile_first, pad;
+    int32_t tile_first;
+    int32_t no_hist;         // the channels' Pcm is null (a rewrite that never decoded before the loop moved): block histories 0
 };
 
 __device__ __forceinline__ void put16be(uint8_t *p, int v) { p[0] = (uint8_t)(v >> 8); p[1] = (uint8_t)v; }
@@ -759,8 +761,9 @@ __device__ __forceinline__ uint2 gc_array_word(const NwChan &cc, int64_t pos, in
     return v;
 }
 
-// IdspWriter: per channel the coefficients, the start context's predictor/scale (Adpcm[0], history 0) and the loop
-// context (the first encode's, at the unaligned loop start), then Interleave(16, AudioDataSize) (Interleave.cs:43-73):
+// IdspWriter: per channel the coefficients, the start context's predictor/scale (Adpcm[0]; its history is in the header
+// blob) and the loop context (the first encode's, at the unaligned loop start, or the blob's), then Interleave(16,
+// AudioDataSize) (Interleave.cs:43-73):
 // AudioDataSize is a multiple of 16, so every block is whole and byte `pos` of a channel is in the file iff pos < in_size.
 __global__ void __launch_bounds__(256) idsp_assemble_kernel(const IdspFile *__restrict__ files, int n_files, const NwChan *__restrict__ chans,
                                                              const uint8_t *__restrict__ hdr_blob, const uint8_t *__restrict__ adpcm,
@@ -782,7 +785,7 @@ __global__ void __launch_bounds__(256) idsp_assemble_kernel(const IdspFile *__re
             uint8_t *info = dst + 0x40 + 0x60 * c;
             if (h < 16) put16be(info + 0x1c + 2 * h, coefs[(int64_t)cc.coef_index * 16 + h]);
             else if (h == 16) put16be(info + 0x3e, adpcm[cc.row_off]);
-            else if (ls > 0) {
+            else if (ls >= 0) {
                 const int k = h - 17;
                 const int v = k == 0 ? adpcm[cc.row_off + (int64_t)(ls / kGcFrameSamples) * kGcFrameBytes]
                                      : ls >= k ? decoded[cc.pcm_off + ls - k] : 0;
@@ -846,7 +849,7 @@ __global__ void __launch_bounds__(256) hps_assemble_kernel(const HpsFile *__rest
                 const NwChan cc = chans[f.first_ch + c];
                 const int s = blk.start_sample;
                 if (m == 0) v = gc_array_byte(cc, blk.byte_in, f.keep_bytes, adpcm, tail);
-                else if (m < 3 && s >= m) v = decoded[cc.pcm_off + s - m];
+                else if (m < 3 && s >= m && !f.no_hist) v = decoded[cc.pcm_off + s - m];
             }
             put16be(dst + blk.at + j, v);
         }
